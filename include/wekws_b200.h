@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 4   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt */
+#define WEKWS_B200_ABI_VERSION 5   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -68,11 +68,18 @@ typedef enum {
 } wekws_backbone;
 
 typedef enum { WEKWS_ACT_IDENTITY = 0, WEKWS_ACT_SIGMOID = 1 } wekws_activation;
+/* Classifier head (kws_model.py:175-195).  LINEAR: classifier.linear.* on every frame, output (B, T, odim).
+ * GLOBAL / LAST: the utterance-level heads of the speech-command recipes (classifier.py:19-40): the MLP
+ * Linear(hidden, 64) -> ReLU -> Linear(64, odim) (tensors classifier.classifier.0.{weight,bias} and
+ * classifier.classifier.3.{weight,bias}) on the mean of all T frames of the call (GLOBAL) or on frame T-1 (LAST);
+ * output (B, odim).  MDTC, TCN and DS-TCN backbones only.                                                     */
+typedef enum { WEKWS_HEAD_LINEAR = 0, WEKWS_HEAD_GLOBAL = 1, WEKWS_HEAD_LAST = 2 } wekws_head;
 typedef enum { WEKWS_PCM_S16 = 0, WEKWS_PCM_F32 = 1 } wekws_pcm_dtype;
 typedef enum { WEKWS_WINDOW_POVEY = 0, WEKWS_WINDOW_HAMMING = 1 } wekws_window;
 
 /* forward flags */
-#define WEKWS_FWD_SOFTMAX 1u  /* apply softmax over odim after the activation (forward_softmax) */
+#define WEKWS_FWD_SOFTMAX 1u  /* apply softmax over odim after the activation (forward_softmax); with a GLOBAL /
+                                 LAST head it normalises each of the B output rows                               */
 
 WEKWS_API const char* wekws_last_error(void);
 WEKWS_API int wekws_abi_version(void);
@@ -150,6 +157,9 @@ WEKWS_API int wekws_model_padding(const wekws_model* m);
 /* name: reference state_dict key, e.g. "backbone.blocks.0.res_blocks.1.bn1.running_var".
  * Data is copied.  num_batches_tracked entries may be skipped.                      */
 WEKWS_API int wekws_model_set_tensor(wekws_model* m, const char* name, const float* h_data, int64_t numel);
+/* head: wekws_head.  Called between create and pack / finalize (default WEKWS_HEAD_LINEAR).  GLOBAL / LAST need an
+ * MDTC, TCN or DS-TCN backbone (else WEKWS_ERR_INVALID); the MLP width is 64.  The streaming cache is unchanged. */
+WEKWS_API int wekws_model_set_head(wekws_model* m, int head);
 /* Host half of finalize: folds every eval-mode BatchNorm into its producer and packs the
  * weight stream.  No CUDA call -- usable (and tested) on a machine without a GPU.        */
 WEKWS_API int wekws_model_pack(wekws_model* m);
@@ -171,7 +181,8 @@ WEKWS_API int64_t wekws_model_packed_floats(const wekws_model* m, int which /*0 
 WEKWS_API int wekws_model_packed_copy(const wekws_model* m, int which, float* h_dst, int64_t capacity);
 
 /* d_feats (B,T,idim); d_in_cache NULL (start of stream == zeros) or
- * conv: (B,hdim,padding)  GRU: (num_layers,B,hdim)  FSMN: (B,proj_dim,padding,num_layers); d_out (B,T,odim);
+ * conv: (B,hdim,padding)  GRU: (num_layers,B,hdim)  FSMN: (B,proj_dim,padding,num_layers); d_out (B,T,odim), or
+ * (B,odim) with a GLOBAL / LAST head (pooled over the T frames of this call);
  * d_out_cache same shape as the cache; it may be the SAME buffer as d_in_cache (in-place
  * streaming update: every slice is read before it is overwritten) or a disjoint one, not a
  * partially overlapping one.                                                       */
@@ -229,7 +240,8 @@ WEKWS_API int wekws_context_expand(const float* d_feats, const int32_t* d_lens, 
                          int right, int skip, float* d_out, int64_t out_frames, void* stream);
 
 /* Raw PCM -> posteriors: Fbank(+CMVN from the model's global_cmvn.* if set) -> model.
- * d_feat_scratch: (B, frames, idim) floats of workspace owned by the caller.        */
+ * d_feat_scratch: (B, frames, idim) floats of workspace owned by the caller.  d_out as wekws_model_forward:
+ * (B, frames, odim), or (B, odim) with a GLOBAL / LAST head.                          */
 WEKWS_API int wekws_pipeline_forward(wekws_fbank* fb, wekws_model* m, const void* d_pcm, int pcm_dtype,
                            int64_t B, int64_t num_samples, int64_t pcm_stride,
                            float* d_feat_scratch, const float* d_in_cache, float* d_out,

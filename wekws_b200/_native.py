@@ -17,8 +17,9 @@ LIB_PATH = os.environ.get("WEKWS_B200_LIB") or os.path.join(_HERE, "libwekws_b20
 BACKBONE_MDTC, BACKBONE_TCN, BACKBONE_DSTCN, BACKBONE_GRU, BACKBONE_FSMN = 0, 1, 2, 3, 4
 ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
+HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 class FbankConfig(C.Structure):
@@ -53,6 +54,7 @@ SIGNATURES = {
     "wekws_model_destroy": (None, [C.c_void_p]),
     "wekws_model_padding": (C.c_int, [C.c_void_p]),
     "wekws_model_set_tensor": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
+    "wekws_model_set_head": (C.c_int, [C.c_void_p, C.c_int]),
     "wekws_model_pack": (C.c_int, [C.c_void_p]),
     "wekws_model_finalize": (C.c_int, [C.c_void_p]),
     "wekws_model_set_precision": (C.c_int, [C.c_void_p, C.c_int]),

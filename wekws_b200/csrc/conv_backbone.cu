@@ -390,7 +390,25 @@ __global__ void __launch_bounds__(NT, 1) conv_backbone_kernel(const ConvArgs a) 
       cls_in = abuf;
     }
     __syncthreads();
-    {
+    if (a.pool != nullptr) {
+      // utterance-level head (cls_head.cu): per-stream sum of the classifier input over frames [pool_t0, pool_t1), one
+      // warp per (stream, channel): lane-strided frames, then a butterfly in a fixed order; the first time-chunk of the
+      // call stores, later ones add
+      if (a.pool_t1 > a.pool_t0) {
+        for (int idx = warp; idx < Sv * C; idx += NT / 32) {
+          const int s = idx / C, c = idx - s * C;
+          const float* src = cls_in + c * RP + s * T;
+          float v = 0.f;
+          for (int t = a.pool_t0 + lane; t < a.pool_t1; t += 32) v += src[t];
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+          if (lane == 0) {
+            float* g = a.pool + (size_t)(b0 + s) * C + c;
+            *g = a.pool_add ? *g + v : v;
+          }
+        }
+      }
+    } else {
       const int odim = a.odim;
       const float* wc = vec + a.v_wc;          // [C][odim]  (transposed classifier weight)
       for (int idx = tid; idx < ROWS * odim; idx += NT) {

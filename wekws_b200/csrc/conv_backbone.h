@@ -27,6 +27,10 @@ struct ConvArgs {
   long long feat_bstride, out_bstride;   // floats between consecutive streams in feats / out
   // derived by conv_backbone_launch
   int S, RP, PADMAX, KP, ah_floats, n_tiles;
+  // utterance-level head (cls_head.cu): pool != nullptr replaces the per-frame classifier by the per-stream sum of the
+  // classifier input over frames [pool_t0, pool_t1) of this chunk, stored to pool (B, C) (pool_add = 0) or added to it
+  float* pool;
+  int pool_t0, pool_t1, pool_add;
 };
 
 int conv_chunk_rows(int C);

@@ -57,8 +57,12 @@ constexpr int OFF_STG = OFF_X + X_BYTES;                   // 129024
 constexpr int OFF_W = OFF_STG + NSLOT * STG_FLOATS * 4;    // 186368 (1024-aligned: SWIZZLE_128B images)
 constexpr int OFF_END = OFF_W + 2 * W_SLOT;                // 219136
 constexpr int SMEM_TOTAL = OFF_END + 1024;                 // incl. alignment slack
+constexpr int POOL_SPT = 16;                               // streams per tile at the shortest chunk (T = 8)
+constexpr int OFF_POOL = OFF_END;                          // head variant: pooled sums [NG][POOL_SPT][64]
+constexpr int SMEM_TOTAL_HEAD = OFF_POOL + NG * POOL_SPT * C * 4 + 1024;
 static_assert(OFF_W % 1024 == 0, "weight images must be 1024-byte aligned");
 static_assert(SMEM_TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
+static_assert(SMEM_TOTAL_HEAD <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 
 __device__ __forceinline__ void group_barrier(int grp) { asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(32 * WPG) : "memory"); }
 __device__ __forceinline__ float2 lds_f2(uint32_t addr) {
@@ -231,7 +235,9 @@ __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B,
 }
 
 // KT: compile-time tap count (5 = every shipped mdtc config; 0 = read a.ktaps, taps guarded one by one)
-template <int KT>
+// HEAD: utterance-level head variant: instead of the per-frame classifier, every stream's stack-output sum is summed over
+// frames [a.pool_t0, a.pool_t1) into a.pool (B, 64); cls_head.cu applies the MLP
+template <int KT, bool HEAD>
 __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant__ TcArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);
@@ -307,10 +313,12 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
         const float* cwf = reinterpret_cast<const float*>(&a.cw[0][0]);
         constexpr int CWS = 7 * 64;                        // floats per block in cw
         float part[2][8];                                  // classifier partial sums of the two rows
+        if constexpr (!HEAD) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+          for (int h = 0; h < 2; ++h)
 #pragma unroll
-          for (int j = 0; j < 8; ++j) part[h][j] = 0.f;
+            for (int j = 0; j < 8; ++j) part[h][j] = 0.f;
+        }
         float acc[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) acc[i] = 0.f;
@@ -466,7 +474,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
               const float o0 = fmaxf(acc[4 * j + 2 * h] + cwb[6 * 64 + ch] + r.x, 0.f);
               const float o1 = fmaxf(acc[4 * j + 2 * h + 1] + cwb[6 * 64 + ch + 1] + r.y, 0.f);
               if (live[h]) sts_f2(ax, o0, o1);
-              if (stack_end) {
+              if (!HEAD && stack_end) {
                 // the classifier is linear: W_c (sum of stack outputs) = sum of W_c (stack output)
                 const float* wc = vec + a.v_wc + ch * a.odim;
 #pragma unroll
@@ -476,7 +484,43 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             }
           }
           group_barrier(grp);                // x' of every row of the tile complete before the next block's conv
+          if constexpr (HEAD) {
+            // X now holds the stack output of every frame of the tile, and stays so until the next block's second
+            // group barrier.  Warp wq sums channels 8 wq .. 8 wq + 7; lane = 8 q + channel, q = frame phase mod 4:
+            // strided frame sums, two shuffles in a fixed order, then the q = 0 lane keeps the stream's running sum
+            // over the stacks in the shared pool buffer (always the same thread: no barrier, no atomics)
+            if (stack_end && a.pool_t1 > a.pool_t0) {
+              const int c = 8 * wq + (lane & 7), q = lane >> 3;
+              const uint32_t cofs = 128u * (uint32_t)((c >> 2) & 1) + 4u * (uint32_t)(c & 3);
+              float* pl = reinterpret_cast<float*>(base + OFF_POOL) + grp * POOL_SPT * C;
+              for (int s2 = 0; s2 < nst; ++s2) {
+                const int colb = (grp * spt + s2) * Lw + PADR;
+                float v = 0.f;
+                for (int t = a.pool_t0 + q; t < a.pool_t1; t += 4) {
+                  const uint32_t cc = (uint32_t)(colb + t);
+                  float x;
+                  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
+                               : "r"(((xs + (cc << 8) + ((cc & 7u) << 4)) ^ ((uint32_t)(c >> 3) << 4)) + cofs));
+                  v += x;
+                }
+                v += __shfl_xor_sync(0xffffffffu, v, 8);
+                v += __shfl_xor_sync(0xffffffffu, v, 16);
+                if (q == 0) pl[s2 * C + c] = (blk == a.stack_size) ? v : pl[s2 * C + c] + v;
+              }
+            }
+          }
         }
+        if constexpr (HEAD) {
+          // the stream's pooled vector: the first time-chunk of the call stores, later ones add (stream-ordered launches)
+          if (a.pool_t1 > a.pool_t0 && lane < 8) {
+            const int c = 8 * wq + lane;
+            const float* pl = reinterpret_cast<const float*>(base + OFF_POOL) + grp * POOL_SPT * C;
+            for (int s2 = 0; s2 < nst; ++s2) {
+              float* g = a.pool + (size_t)(b0 + grp * spt + s2) * C + c;
+              *g = a.pool_add ? *g + pl[s2 * C + c] : pl[s2 * C + c];
+            }
+          }
+        } else {
         // ---- classifier bias + activation: the four lanes of a row hold disjoint channel pairs
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -497,6 +541,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             }
           }
         }
+        }  // !HEAD
       } else {
         // a group without streams in this pass still releases every weight slot use (w_free counts every compute
         // warp's arrival); all lanes keep the same phase bookkeeping
@@ -525,8 +570,9 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
 
 }  // namespace
 
-bool tc_eligible(const TcArgs& a, int padmax) {
-  if (a.idim % 8 != 0 || a.idim > 96 || a.odim > 8 || a.ktaps > 5) return false;   // first Linear: at most two A atoms, K <= 96
+bool tc_eligible(const TcArgs& a, int padmax, bool head) {
+  // first Linear: at most two A atoms, K <= 96; the per-frame classifier keeps odim <= 8 partial sums per row
+  if (a.idim % 8 != 0 || a.idim > 96 || (!head && a.odim > 8) || a.ktaps > 5) return false;
   if (a.nblocks > kTcMaxBlocks) return false;                                        // taps / biases travel in the parameter block
   if (padmax > 32 || a.P % 4 != 0) return false;
   for (int b = 0; b < a.nblocks; ++b)
@@ -558,12 +604,13 @@ EncodeTiledFn encode_tiled_fn() {
 }
 }  // namespace
 
-int mdtc_tc_launch(TcArgs a, int padmax, cudaStream_t st) {
+int mdtc_tc_launch(TcArgs a, int padmax, cudaStream_t st, bool head) {
   WEKWS_REQUIRE(a.T >= 1 && a.T <= 128 && a.B >= 1, "mdtc_tc_launch: bad shape");
   a.padr = (padmax + 3) & ~3;
   const int Lw = a.padr + a.T;
   a.spt = 128 / a.T;                                   // streams per 128-row tile
   WEKWS_REQUIRE(a.spt >= 1 && Lw <= XCOLS, "mdtc_tc_launch: tile does not fit");
+  WEKWS_REQUIRE(!head || (a.pool != nullptr && a.spt <= POOL_SPT), "mdtc_tc_launch: bad head call");
   int smax = NG * a.spt;                               // streams resident per pass
   if (smax > XCOLS / Lw) smax = XCOLS / Lw;
   a.smax = smax;
@@ -597,12 +644,19 @@ int mdtc_tc_launch(TcArgs a, int padmax, cudaStream_t st) {
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL_HEAD));
+    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL_HEAD));
     attr_set[dev] = true;
   }
-  if (a.ktaps == 5) mdtc_tc_kernel<5><<<grid, NT_TC, SMEM_TOTAL, st>>>(a);
-  else mdtc_tc_kernel<0><<<grid, NT_TC, SMEM_TOTAL, st>>>(a);
+  if (head) {
+    if (a.ktaps == 5) mdtc_tc_kernel<5, true><<<grid, NT_TC, SMEM_TOTAL_HEAD, st>>>(a);
+    else mdtc_tc_kernel<0, true><<<grid, NT_TC, SMEM_TOTAL_HEAD, st>>>(a);
+    return check_launch("mdtc_tc_kernel");
+  }
+  if (a.ktaps == 5) mdtc_tc_kernel<5, false><<<grid, NT_TC, SMEM_TOTAL, st>>>(a);
+  else mdtc_tc_kernel<0, false><<<grid, NT_TC, SMEM_TOTAL, st>>>(a);
   return check_launch("mdtc_tc_kernel");
 }
 

@@ -31,11 +31,16 @@ struct TcArgs {
   // they never touch the shared-memory load/store pipe.  [blk][0..4] = taps (zero beyond ktaps), [5] = b1, [6] = b2;
   // 64 each.
   alignas(16) float4 cw[kTcMaxBlocks][7 * 16];
+  // head variant of the kernel only (cls_head.cu): per-stream sum of the stack-output sum over frames
+  // [pool_t0, pool_t1) of this chunk, stored to pool (B, 64) (pool_add = 0) or added to it
+  float* pool;
+  int pool_t0, pool_t1, pool_add;
 };
 static_assert(sizeof(TcArgs) <= 32764, "kernel parameter block exceeds 32764 bytes");
 
-bool tc_eligible(const TcArgs& a, int padmax);
+// head: the utterance-level head variant (a.pool set; no per-frame output, so no limit on odim)
+bool tc_eligible(const TcArgs& a, int padmax, bool head = false);
 int tc_max_T();
-int mdtc_tc_launch(TcArgs a, int padmax, cudaStream_t st);
+int mdtc_tc_launch(TcArgs a, int padmax, cudaStream_t st, bool head = false);
 
 }  // namespace wekws

@@ -23,6 +23,7 @@
 #include "dstcn_tc.h"
 #include "fsmn.h"
 #include "linear_tc.h"
+#include "cls_head.h"
 
 namespace wekws {
 
@@ -112,6 +113,10 @@ struct wekws_model {
   size_t hidden_cap = 0;
   bool gru_tc_ok = false;                   // tensor-core GRU (gru_tc.cu): weight stream lives in h_wimg / d_wimg
   GruTcArgs grutc{};
+  int head = WEKWS_HEAD_LINEAR;             // wekws_head; GLOBAL / LAST: the backbone kernel pools, cls_head.cu classifies
+  int v_w0 = 0, v_b0 = 0, v_w1 = 0, v_b1 = 0;   // the head's MLP in h_vec (pack_head)
+  float* d_pool = nullptr;                  // (B, hdim) pooled backbone output between the two kernels; grows monotonically
+  size_t pool_cap = 0;
 };
 
 namespace {
@@ -198,6 +203,28 @@ int pack_classifier(wekws_model* m, int H, int* v_wc, int* v_bc) {
   return WEKWS_OK;
 }
 
+// Utterance-level head (classifier.py:19-40 around kws_model.py:180-182): W0^T [H][64], b0, W1^T [64][odim], b1
+int pack_head(wekws_model* m, int H) {
+  const int odim = m->cfg.odim, W = kHeadWidth;
+  GET(w0, "classifier.classifier.0.weight", (size_t)W * H);
+  GET(b0, "classifier.classifier.0.bias", (size_t)W);
+  GET(w1, "classifier.classifier.3.weight", (size_t)odim * W);
+  GET(b1, "classifier.classifier.3.bias", (size_t)odim);
+  m->v_w0 = (int)m->h_vec.size();
+  m->h_vec.resize(m->h_vec.size() + pad4((size_t)H * W), 0.f);
+  for (int c = 0; c < H; ++c)
+    for (int j = 0; j < W; ++j) m->h_vec[m->v_w0 + c * W + j] = w0[j * H + c];
+  m->v_b0 = (int)m->h_vec.size();
+  m->h_vec.insert(m->h_vec.end(), b0, b0 + W);
+  m->v_w1 = (int)m->h_vec.size();
+  m->h_vec.resize(m->h_vec.size() + pad4((size_t)W * odim), 0.f);
+  for (int k = 0; k < W; ++k)
+    for (int j = 0; j < odim; ++j) m->h_vec[m->v_w1 + k * odim + j] = w1[j * W + k];
+  m->v_b1 = (int)m->h_vec.size();
+  m->h_vec.resize(m->h_vec.size() + pad4(odim), 0.f);
+  for (int j = 0; j < odim; ++j) m->h_vec[m->v_b1 + j] = b1[j];
+  return WEKWS_OK;
+}
 
 // round-to-nearest-even fp32 -> bf16 (as __floats2bfloat162_rn does on the device)
 uint16_t bf16_rn(float x) {
@@ -251,6 +278,8 @@ void pack_tc(wekws_model* m) {
   m->h_wimg.clear();
   m->h_cimg.clear();
   const wekws_model_config& c = m->cfg;
+  const bool head = m->head != WEKWS_HEAD_LINEAR;
+  if (head && c.backbone != WEKWS_BACKBONE_MDTC) return;     // TCN / DS-TCN heads run on the FP32 conv kernel
   if (c.backbone == WEKWS_BACKBONE_DSTCN) {
     DsTcArgs& t = m->dsargs;
     memset(&t, 0, sizeof(t));
@@ -312,7 +341,7 @@ void pack_tc(wekws_model* m) {
   t.v_mean = a.v_mean; t.v_istd = a.v_istd; t.v_bp = a.v_bp; t.v_blocks = a.v_blocks;
   t.v_blk_stride = a.v_blk_stride; t.v_wc = a.v_wc; t.v_bc = a.v_bc;
   for (int b = 0; b < a.nblocks; ++b) { t.dil[b] = a.dil[b]; t.coff[b] = a.coff[b]; }
-  if (!tc_eligible(t, m->padmax)) return;
+  if (!tc_eligible(t, m->padmax, head)) return;
   if (m->folded.size() != (size_t)(1 + 2 * a.nblocks)) return;
   m->h_wimg.assign((size_t)(2 + 2 * a.nblocks) * 16384, 0);
   write_w_image(m->h_wimg.data(), m->folded[0], a.idim, 0);
@@ -430,7 +459,11 @@ int pack_conv(wekws_model* m) {
       return WEKWS_ERR_INVALID;
     }
   }
-  if ((rc = pack_classifier(m, C, &a.v_wc, &a.v_bc))) return rc;
+  if (m->head != WEKWS_HEAD_LINEAR) {
+    if ((rc = pack_head(m, C))) return rc;
+  } else if ((rc = pack_classifier(m, C, &a.v_wc, &a.v_bc))) {
+    return rc;
+  }
   m->h_chunk_off.push_back((int)m->h_stream.size());
   a.kind = c.backbone; a.C = C; a.idim = idim; a.odim = c.odim; a.nblocks = m->nblocks; a.ktaps = K;
   a.P = m->padding; a.stack_size = c.stack_size > 0 ? c.stack_size : 1; a.act = c.activation;
@@ -581,9 +614,10 @@ int pack_fsmn(wekws_model* m) {
 
 void free_device(wekws_model* m) {
   cudaFree(m->d_stream); cudaFree(m->d_vec); cudaFree(m->d_chunk_off); cudaFree(m->d_wimg);
-  cudaFree(m->d_cimg); cudaFree(m->d_cbias); cudaFree(m->d_hidden);
+  cudaFree(m->d_cimg); cudaFree(m->d_cbias); cudaFree(m->d_hidden); cudaFree(m->d_pool);
   m->d_stream = nullptr; m->d_vec = nullptr; m->d_chunk_off = nullptr; m->d_wimg = nullptr;
   m->d_cimg = nullptr; m->d_cbias = nullptr; m->d_hidden = nullptr; m->hidden_cap = 0;
+  m->d_pool = nullptr; m->pool_cap = 0;
 }
 
 }  // namespace
@@ -632,6 +666,18 @@ extern "C" int wekws_model_padding(const wekws_model* m) {
 extern "C" int wekws_model_set_tensor(wekws_model* m, const char* name, const float* h_data, int64_t numel) {
   WEKWS_REQUIRE(m && name && (h_data || numel == 0) && numel >= 0, "wekws_model_set_tensor: bad argument");
   m->tensors[name].assign(h_data, h_data + numel);
+  m->finalized = false;
+  return WEKWS_OK;
+}
+
+extern "C" int wekws_model_set_head(wekws_model* m, int head) {
+  WEKWS_REQUIRE(m, "wekws_model_set_head: null handle");
+  WEKWS_REQUIRE(head >= WEKWS_HEAD_LINEAR && head <= WEKWS_HEAD_LAST, "unknown head id %d", head);
+  WEKWS_REQUIRE(head == WEKWS_HEAD_LINEAR || m->cfg.backbone == WEKWS_BACKBONE_MDTC ||
+                m->cfg.backbone == WEKWS_BACKBONE_TCN || m->cfg.backbone == WEKWS_BACKBONE_DSTCN,
+                "the %s head is implemented behind the MDTC, TCN and DS-TCN backbones only",
+                head == WEKWS_HEAD_GLOBAL ? "global" : "last");
+  m->head = head;
   m->finalized = false;
   return WEKWS_OK;
 }
@@ -781,6 +827,17 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
     const bool use_tcn = m->tcn_ok && m->precision != 1 && T >= 8 && ((uintptr_t)d_feats & 15) == 0;
     const bool use_ds = m->ds_ok && m->precision != 1 && T >= 8 && ((uintptr_t)d_feats & 15) == 0;
     const int maxT = use_tc ? tc_max_T() : use_tcn ? tcn_tc_max_T() : use_ds ? dstcn_tc_max_T() : m->conv_max_T;
+    const bool head = m->head != WEKWS_HEAD_LINEAR;
+    if (head) {                     // pooled vector scratch between the backbone kernel(s) and the head kernel
+      const size_t need = (size_t)B * (size_t)m->cfg.hdim;
+      if (need > m->pool_cap) {
+        WEKWS_CUDA_OK(cudaStreamSynchronize(st));          // the old scratch may still be in use on this stream
+        cudaFree(m->d_pool);
+        m->d_pool = nullptr; m->pool_cap = 0;
+        WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_pool, need * sizeof(float)));
+        m->pool_cap = need;
+      }
+    }
     if (use_ds && m->cls_tc) {      // hidden scratch between the backbone kernel and the classifier GEMM
       const size_t need = (size_t)B * (size_t)T * (size_t)m->cfg.hdim;
       if (need > m->hidden_cap) {
@@ -794,6 +851,13 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
     const int nchunk = (int)((T + maxT - 1) / maxT);
     const int Tc = (int)((T + nchunk - 1) / nchunk);
     for (int64_t t0 = 0; t0 < T; t0 += Tc) {
+      // head: the frames of this chunk the pooled vector takes (every frame, or the call's last one) and whether the
+      // chunk stores the vector (the first chunk that contributes) or adds to it
+      const int Tk = (int)(T - t0 < Tc ? T - t0 : Tc);
+      int pool_t0 = 0, pool_t1 = 0, pool_add = 0;
+      if (m->head == WEKWS_HEAD_GLOBAL) { pool_t1 = Tk; pool_add = t0 > 0; }
+      else if (m->head == WEKWS_HEAD_LAST && t0 + Tk == T) { pool_t0 = Tk - 1; pool_t1 = Tk; }
+      float* pool = head ? m->d_pool : nullptr;
       if (use_tc) {
         TcArgs a = m->tcargs;
         a.feats = d_feats + t0 * m->cfg.idim;
@@ -804,7 +868,8 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
         a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
         a.feat_bstride = T * m->cfg.idim;
         a.out_bstride = T * m->cfg.odim;
-        int rc = mdtc_tc_launch(a, m->padmax, st);
+        a.pool = pool; a.pool_t0 = pool_t0; a.pool_t1 = pool_t1; a.pool_add = pool_add;
+        int rc = mdtc_tc_launch(a, m->padmax, st, head);
         if (rc) return rc;
         continue;
       }
@@ -846,6 +911,7 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
       a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
       a.feat_bstride = T * m->cfg.idim;
       a.out_bstride = T * m->cfg.odim;
+      a.pool = pool; a.pool_t0 = pool_t0; a.pool_t1 = pool_t1; a.pool_add = pool_add;
       int rc = conv_backbone_launch(a, m->padmax, st);
       if (rc) return rc;
     }
@@ -859,6 +925,16 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
     a.N = m->cfg.odim; a.K = m->cfg.hdim; a.act = m->cfg.activation; a.n_mtiles = 0;
     int rc = linear_tc_launch(a, st);
     if (rc) return rc;
+  }
+  if (m->head != WEKWS_HEAD_LINEAR) {
+    // MLP head (+ activation, + softmax) on the pooled vectors: (B, odim)
+    ClsHeadArgs a;
+    a.pool = m->d_pool; a.out = d_out; a.vec = m->d_vec;
+    a.B = (int)B; a.H = m->cfg.hdim; a.odim = m->cfg.odim; a.act = m->cfg.activation;
+    a.softmax = (flags & WEKWS_FWD_SOFTMAX) ? 1 : 0;
+    a.scale = m->head == WEKWS_HEAD_GLOBAL ? (float)(1.0 / (double)T) : 1.f;
+    a.v_w0 = m->v_w0; a.v_b0 = m->v_b0; a.v_w1 = m->v_w1; a.v_b1 = m->v_b1;
+    return cls_head_launch(a, st);
   }
   if (flags & WEKWS_FWD_SOFTMAX) {
     const long long rows = B * T;

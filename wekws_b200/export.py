@@ -20,6 +20,9 @@ MAGIC, VERSION = b"WKB1", 2
 def export_native(model, path: str) -> dict:
     """Writes ``model`` (a wekws_b200.KWSModel, e.g. after load_state_dict of a reference checkpoint) to ``path``.
     Returns the metadata the ONNX exporter would have attached (export_onnx.py:72-77)."""
+    if getattr(model, "head", None) is not None:
+        raise NotImplementedError(f"export_native: the '{model.head}' classifier head cannot be exported: the runtime "
+                                  "shim is frame-level and the .wkb configuration does not carry the head")
     cfg = model._native_config()
     fields = [getattr(cfg, name) for name, _ in cfg._fields_]
     tensors = [(k, v.detach().to(device="cpu", dtype=torch.float32).contiguous())

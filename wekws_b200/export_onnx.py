@@ -216,6 +216,9 @@ def export_onnx(model, path: str, softmax: bool = False) -> dict:
     wekws/bin/export_onnx.py.  Returns the metadata that was attached."""
     bb = model.backbone
     kind = getattr(bb, "kind", None)
+    if getattr(model, "head", None) is not None:
+        raise NotImplementedError(f"export_onnx: the '{model.head}' classifier head is not exported yet; the graph "
+                                  "here is the frame-level (input, cache) -> (output, r_cache) contract")
     if kind not in ("mdtc", "tcn", "ds_tcn", "fsmn"):
         raise NotImplementedError("export_onnx: the ONNX contract needs `backbone.padding` (mdtc / tcn / ds_tcn / fsmn); "
                                   "the reference's exporter fails for GRU models too (export_onnx.py:57)")

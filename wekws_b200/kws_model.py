@@ -143,6 +143,17 @@ def _linear_classifier(idim: int, odim: int) -> nn.Module:
     return _holder(linear=nn.Linear(idim, odim))
 
 
+def _head_classifier(idim: int, odim: int, dropout: float, head: str) -> nn.Module:
+    """GlobalClassifier / LastClassifier around Sequential(Linear(idim, 64), ReLU, Dropout, Linear(64, odim))
+    (classifier.py:19-40, kws_model.py:180-189): state_dict classifier.{0,3}.{weight,bias}."""
+    m = _holder(classifier=nn.Sequential(nn.Linear(idim, 64), nn.ReLU(), nn.Dropout(dropout), nn.Linear(64, odim)))
+    m.head = head
+    return m
+
+
+_HEADS = {"global": _native.HEAD_GLOBAL, "last": _native.HEAD_LAST}
+
+
 class KWSModel(nn.Module):
     """wekws/model/kws_model.py:33-95, executed by libwekws_b200.so."""
 
@@ -231,6 +242,12 @@ class KWSModel(nn.Module):
         cfg.norm_var = 1 if (self.global_cmvn is None or self.global_cmvn.norm_var) else 0
         return cfg
 
+    @property
+    def head(self) -> Optional[str]:
+        """'global' / 'last' for the utterance-level speech-command heads (output (B, odim)), None for the per-frame
+        linear classifier."""
+        return getattr(self.classifier, "head", None)
+
     def _build_handle(self, finalize: bool = True):
         """Creates the native model and feeds it the state_dict by its reference key names."""
         lib = _native.lib()
@@ -239,6 +256,8 @@ class KWSModel(nn.Module):
         h = C.c_void_p()
         _native.check(lib.wekws_model_create(C.byref(cfg), C.byref(h)), "wekws_model_create")
         self._handle = h
+        if self.head is not None:
+            _native.check(lib.wekws_model_set_head(h, _HEADS[self.head]), "wekws_model_set_head")
         for name, t in self.state_dict().items():
             if name.endswith("num_batches_tracked"):
                 continue
@@ -305,6 +324,9 @@ class KWSModel(nn.Module):
             raise ValueError(f"features must be (B, T, {self.idim}), got {tuple(x.shape)}")
         dev = x.device
         B, T = x.size(0), x.size(1)
+        head = self.head
+        if head is not None and T == 0:
+            raise ValueError(f"the '{head}' classifier head needs at least one frame per call")
         if not x.is_contiguous():
             x = x.contiguous()
         gru = isinstance(self.backbone, nn.GRU)
@@ -323,7 +345,7 @@ class KWSModel(nn.Module):
             cache_ptr = in_cache.data_ptr()
         h = self._ensure(dev)
         self._apply_precision(h)
-        out = torch.empty((B, T, self.odim), device=dev, dtype=torch.float32)
+        out = torch.empty((B, self.odim) if head is not None else (B, T, self.odim), device=dev, dtype=torch.float32)
         if T == 0 and cache_ptr is not None:
             out_cache = in_cache.clone()
         elif T == 0:
@@ -347,7 +369,11 @@ class KWSModel(nn.Module):
         return self._run(x, in_cache, 0)
 
     def forward_softmax(self, x: torch.Tensor, in_cache: torch.Tensor = _EMPTY) -> Tuple[torch.Tensor, torch.Tensor]:
-        """kws_model.py:78-90 -- softmax over the output dim after the activation."""
+        """kws_model.py:78-90 -- softmax over the output dim after the activation.  With a global / last head the
+        reference's softmax(2) of the 2-D output raises IndexError; so does this, before any launch."""
+        if self.head is not None:
+            raise IndexError("Dimension out of range (expected to be in range of [-2, 1], but got 2): "
+                             f"the '{self.head}' head outputs (B, odim)")
         return self._run(x, in_cache, _native.FWD_SOFTMAX)
 
     def fuse_modules(self):
@@ -382,6 +408,9 @@ def init_model(configs: dict) -> KWSModel:
         sys.exit(1)
 
     bb = configs["backbone"]
+    if "classifier" in configs and configs["classifier"]["type"] in ("global", "last") and bb["type"] in ("gru", "fsmn"):
+        raise NotImplementedError(f"wekws_b200: the '{configs['classifier']['type']}' classifier head is implemented "
+                                  "behind the MDTC, TCN and DS-TCN backbones, not behind " + bb["type"].upper())
     if bb["type"] == "gru":
         backbone = nn.GRU(hidden_dim, hidden_dim, num_layers=bb["num_layers"], batch_first=True)
     elif bb["type"] == "tcn":
@@ -403,13 +432,20 @@ def init_model(configs: dict) -> KWSModel:
     if "classifier" in configs:                                 # kws_model.py:175-195
         classifier_type = configs["classifier"]["type"]
         if classifier_type in ("global", "last"):
-            raise NotImplementedError("wekws_b200: the speech-command 'classifier' heads (global/last) are "
-                                      "outside the streaming hot path (SURVEY.md section 2 row 8)")
+            dropout = configs["classifier"]["dropout"]          # read unconditionally, as the reference does
+            if output_dim < 2:
+                # the heads emit one logit per class for cross-entropy over the keywords plus the non-keyword class
+                # (loss.py:167-171, criterion 'ce' of the speech-command recipe); with a single output that
+                # classifier is degenerate (its softmax is identically 1).  Single-keyword detection is the per-frame
+                # linear head of the max-pooling recipes.
+                raise NotImplementedError(f"wekws_b200: the '{classifier_type}' classifier head needs output_dim >= 2 "
+                                          "(keywords + the non-keyword class), got %d" % output_dim)
+            classifier: nn.Module = _head_classifier(hidden_dim, output_dim, dropout, classifier_type)
         elif classifier_type == "identity":
             if bb["type"] != "fsmn":
                 raise NotImplementedError("wekws_b200: classifier 'identity' is implemented behind the FSMN backbone "
                                           "(the only shipped use, fsmn_ctc.yaml)")
-            classifier: nn.Module = nn.Identity()
+            classifier = nn.Identity()
         else:
             print("Unknown classifier type {}".format(classifier_type))
             sys.exit(1)

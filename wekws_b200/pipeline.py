@@ -53,6 +53,8 @@ class Pipeline:
                 raise ValueError(f"in_cache must be {cache_shape}, got {tuple(in_cache.shape)}")
             in_cache = in_cache.to(device=dev, dtype=torch.float32).contiguous()
             cache_ptr = in_cache.data_ptr()
+        if m.head is not None:
+            return self._run_head(pcm, in_cache, cache_ptr, cache_shape, softmax)
         out = torch.empty((B, T, m.odim), device=dev, dtype=torch.float32)
         if T == 0 or B == 0:
             return out, (in_cache.clone() if cache_ptr is not None else torch.zeros(cache_shape, device=dev))
@@ -66,6 +68,33 @@ class Pipeline:
                 _native.check(_native.lib().wekws_model_set_precision(h_model, 0 if m.precision == "auto" else 1),
                               "wekws_model_set_precision")
                 m._precision_applied = m.precision
+            rc = _native.lib().wekws_pipeline_forward(
+                fe._handle(dev), h_model, C.c_void_p(pcm.data_ptr()),
+                _native.PCM_S16 if pcm.dtype == torch.int16 else _native.PCM_F32, B, N, pcm.stride(0),
+                C.c_void_p(self._scratch.data_ptr()), cache_ptr, C.c_void_p(out.data_ptr()),
+                C.c_void_p(out_cache.data_ptr()), _native.FWD_SOFTMAX if softmax else 0,
+                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        _native.check(rc, "wekws_pipeline_forward")
+        return out, out_cache
+
+    def _run_head(self, pcm, in_cache, cache_ptr, cache_shape, softmax):
+        """Global / last classifier head: one (B, odim) row per clip, pooled over its frames (softmax: over each row)."""
+        m, fe = self.model, self.frontend
+        dev = pcm.device
+        B, N = pcm.shape
+        T = fe.num_frames(N)
+        if T == 0:
+            raise ValueError(f"the '{m.head}' classifier head needs at least one frame per call")
+        out = torch.empty((B, m.odim), device=dev, dtype=torch.float32)
+        if B == 0:
+            return out, (in_cache.clone() if cache_ptr is not None else torch.zeros(cache_shape, device=dev))
+        out_cache = torch.empty(cache_shape, device=dev, dtype=torch.float32)
+        need = B * T * m.idim
+        if self._scratch is None or self._scratch.numel() < need or self._scratch.device != dev:
+            self._scratch = torch.empty(need, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            h_model = m._ensure(dev)
+            m._apply_precision(h_model)
             rc = _native.lib().wekws_pipeline_forward(
                 fe._handle(dev), h_model, C.c_void_p(pcm.data_ptr()),
                 _native.PCM_S16 if pcm.dtype == torch.int16 else _native.PCM_F32, B, N, pcm.stride(0),
