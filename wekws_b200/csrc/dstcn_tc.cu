@@ -18,8 +18,6 @@
 //   * depthwise coefficients of the current block (9 KB) are staged by one bulk copy per block.
 // Warp roles: 16 compute warps (row = 32 * (warp % 4) + lane, channel group = warp / 4; warpgroup = warp / 4) + 1 weight
 // loader warp.
-#include <stdlib.h>
-
 #include <type_traits>
 
 #include "common.cuh"
@@ -100,22 +98,12 @@ __global__ void __launch_bounds__(NT_TC, 1) dstcn_tc_kernel(const DsTcArgs a) {
   int done = sb;
   uint32_t gu = 0;                                   // compute: weight images consumed so far (in pairs)
 
-  // the cache of the streams of a pass is pulled into L2 one pass ahead, so the depthwise taps that read it
-  // straight from global memory see L2 latency instead of HBM latency
-  auto prefetch_cache = [&](int first, int n) {
-    if (!a.prefetch_ok || lane != 0) return;
-    for (int i = 0; i < n; ++i)
-      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a.in_cache + (size_t)(first + i) * C * P),
-                   "r"(C * P * 4)
-                   : "memory");
-  };
   auto load_coef = [&](int blk) {                    // one thread
     fence_proxy_async();                             // the area was read/written through the generic proxy
     mbar_arrive_expect_tx(&coef_bar, COEF_FLOATS * 4);
     bulk_g2s(coef, vec + a.v_blocks + (size_t)blk * a.v_blk_stride, COEF_FLOATS * 4, &coef_bar);
   };
   uint32_t gl = 0;                                   // loader: weight images issued so far
-  if (is_loader) prefetch_cache(sb, min(spt, se - sb));
 
   while (done < se) {
     const int remaining = se - done;
@@ -135,7 +123,6 @@ __global__ void __launch_bounds__(NT_TC, 1) dstcn_tc_kernel(const DsTcArgs a) {
           bulk_g2s(Wring + slot * W_SLOT, a.wimg + (size_t)n * W_SLOT, W_SLOT, &w_bar[slot]);
         }
       }
-      if (done < se) prefetch_cache(done, min(spt, se - done));
     } else {
       // ================================================================== COMPUTE WARPS
       // Rows are ordered frame-major: row = t * ns + s, and X[c][row] likewise, so a tap is a column shift of
@@ -381,8 +368,8 @@ __global__ void __launch_bounds__(NT_TC, 1) dstcn_tc_kernel(const DsTcArgs a) {
 
 }  // namespace
 
-bool dstcn_tc_eligible(const DsTcArgs& a, int hdim) {
-  return hdim == C && a.ktaps == KT && a.idim % 8 == 0 && a.idim >= 8 && a.idim <= 128 && a.odim >= 1 && (a.odim <= 4 || a.hidden != nullptr) &&
+bool dstcn_tc_eligible(const DsTcArgs& a, int hdim, bool cls_gemm) {
+  return hdim == C && a.ktaps == KT && a.idim % 8 == 0 && a.idim >= 8 && a.idim <= 128 && a.odim >= 1 && (a.odim <= 4 || cls_gemm) &&
          a.v_blocks % 4 == 0 && a.v_blk_stride % 4 == 0;
 }
 
@@ -391,8 +378,6 @@ int dstcn_tc_max_T() { return RPX; }
 int dstcn_tc_launch(DsTcArgs a, cudaStream_t st) {
   WEKWS_REQUIRE(a.T >= 1 && a.T <= RPX && a.B >= 1, "dstcn_tc_launch: bad shape");
   a.spt = RPX / a.T;
-  a.prefetch_ok = a.in_cache != nullptr && ((uintptr_t)a.in_cache & 15) == 0 && (C * a.P * 4) % 16 == 0 &&
-                  getenv("WEKWS_DS_PREFETCH") != nullptr;      // off by default (opt-in L2 prefetch of the next pass's cache)
   {
     const size_t bytes = (size_t)a.B * C * a.P * sizeof(float);
     const char* i0 = reinterpret_cast<const char*>(a.in_cache);

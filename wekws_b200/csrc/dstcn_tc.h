@@ -26,10 +26,10 @@ struct DsTcArgs {
   int aliased;             // out_cache overlaps in_cache (set by dstcn_tc_launch)
   float* hidden;           // non-null: skip the classifier and write the final x as (B, T, 256) rows (stream stride
   long long hidden_bstride;  // hidden_bstride) for the tensor-core classifier (linear_tc.cu) that follows
-  int prefetch_ok;         // in_cache present and 16-byte aligned with 16-byte stream pitch (set by dstcn_tc_launch)
 };
 
-bool dstcn_tc_eligible(const DsTcArgs& a, int hdim);
+// cls_gemm: the classifier runs as its own GEMM (linear_tc.cu) on `hidden`, so odim is not limited
+bool dstcn_tc_eligible(const DsTcArgs& a, int hdim, bool cls_gemm);
 int dstcn_tc_max_T();
 int dstcn_tc_launch(DsTcArgs a, cudaStream_t st);
 

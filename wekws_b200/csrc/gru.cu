@@ -12,8 +12,6 @@
 // so every step streams them from L2 through a double-buffered shared-memory ring of 48 KB chunks
 // (16 k-rows of [W_ih | W_hh], one cp.async.bulk each, mbarrier-signalled): the TMA engine keeps
 // ~96 KB in flight per SM, which is what hides the L2 latency -- register-staged loads could not.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "gru.h"
 #include "tc_common.cuh"
@@ -29,13 +27,7 @@ constexpr int KCH = 16;                          // k-rows per weight chunk
 constexpr int CHUNK_FLOATS = KCH * 2 * GG;       // 12288 floats = 48 KB
 constexpr int NCHUNK = GH / KCH;                 // 8 chunks per layer
 
-// MC = true: the CTAs form clusters of CLUSTER; every weight chunk is fetched from L2 once per cluster -- CTA r loads
-// slice r and multicasts it into the ring slot of all CLUSTER CTAs -- instead of once per CTA.  At T = 1 the step is
-// bound by L2 egress (every SM ingests all 786 KB of weights), so this divides the dominant traffic by CLUSTER.
-constexpr int CLUSTER = 8;
-constexpr int SLICE_FLOATS = CHUNK_FLOATS / CLUSTER;
-
-template <int S, bool MC>
+template <int S>
 __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
   extern __shared__ __align__(128) float sm[];
   float* ring = sm;                               // [2][CHUNK_FLOATS]
@@ -45,44 +37,30 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
   float* gh = gi + S * GG;                        // [S][G]
   float* fin = gh + S * GG;                       // [S][idimP]
   __shared__ uint64_t full[2];
-  __shared__ uint64_t empty[2];                   // MC: all CLUSTER CTAs are done reading the slot
   const int tid = threadIdx.x;
   const int idim = a.idim, idimP = (idim + 3) & ~3;
   const float* vec = a.vec;
   if (tid == 0) {
     mbar_init(&full[0], 1); mbar_init(&full[1], 1);
-    mbar_init(&empty[0], CLUSTER); mbar_init(&empty[1], CLUSTER);
     mbar_fence_init();
   }
   __syncthreads();
-  const uint32_t crank = MC ? cluster_ctarank() : 0;
-  if (MC) cluster_sync_all();                     // peers must not signal barriers that are not initialised yet
   uint32_t seq_issued = 0, seq_used = 0;          // weight-chunk sequence numbers (slot = seq & 1)
   // chunk `c` of the per-step stream: layer l = c / NCHUNK, rows [KCH * (c % NCHUNK), +KCH)
   auto issue = [&](int c) {                       // thread 0
     const int l = c / NCHUNK, kc = c - l * NCHUNK;
     const float* src = vec + a.v_layers + (size_t)l * a.v_layer_stride + (size_t)kc * CHUNK_FLOATS;
     const uint32_t slot = seq_issued & 1;
-    if (MC && seq_issued >= 2) mbar_wait_cluster(&empty[slot], ((seq_issued >> 1) - 1) & 1);   // every CTA read chunk seq-2
     fence_proxy_async();                          // the slot was read through the generic proxy
     mbar_arrive_expect_tx(&full[slot], CHUNK_FLOATS * 4);
-    if (MC)
-      bulk_g2s_multicast(ring + slot * CHUNK_FLOATS + crank * SLICE_FLOATS, src + crank * SLICE_FLOATS, SLICE_FLOATS * 4,
-                         &full[slot], (uint16_t)((1u << CLUSTER) - 1));
-    else
-      bulk_g2s(ring + slot * CHUNK_FLOATS, src, CHUNK_FLOATS * 4, &full[slot]);
+    bulk_g2s(ring + slot * CHUNK_FLOATS, src, CHUNK_FLOATS * 4, &full[slot]);
     ++seq_issued;
   };
   const int chunks_per_step = a.L * NCHUNK;
 
-  // every CTA runs the same number of tiles (a cluster consumes one common weight-chunk sequence); tiles past the
-  // end are empty (Sv = 0): they keep the pipeline in step and touch no stream
-  const int tiles_per_cta = (a.n_tiles + (int)gridDim.x - 1) / (int)gridDim.x;
-  for (int it = 0; it < tiles_per_cta; ++it) {
-    const int tile = blockIdx.x + it * gridDim.x;
-    if (!MC && tile >= a.n_tiles) break;
+  for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
     const int b0 = tile * S;
-    const int Sv = max(0, min(S, a.B - b0));
+    const int Sv = min(S, a.B - b0);
     __syncthreads();
     for (int i = tid; i < a.L * S * GH; i += GG) {
       const int l = i / (S * GH), rem = i - l * S * GH, s = rem / GH, j = rem - s * GH;
@@ -143,8 +121,7 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
             if (c < chunks_per_step) issue(c);
             else if (t + 1 < a.T) issue(0);           // first chunk of the next time step
           }
-          if (MC) mbar_wait_bounded(&full[slot], (seq_used >> 1) & 1);
-          else mbar_wait(&full[slot], (seq_used >> 1) & 1);
+          mbar_wait(&full[slot], (seq_used >> 1) & 1);
           const float* w = ring + slot * CHUNK_FLOATS + tid;
 #pragma unroll
           for (int k4 = 0; k4 < KCH; k4 += 4) {
@@ -164,10 +141,6 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
           }
           ++seq_used;
           __syncthreads();                            // everyone done with this slot before it is refilled
-          if (MC && tid == 0) {
-#pragma unroll
-            for (uint32_t r = 0; r < CLUSTER; ++r) mbar_arrive_remote(&empty[slot], r);
-          }
         }
 #pragma unroll
         for (int s = 0; s < S; ++s) { gi[s * GG + tid] = ai[s]; gh[s * GG + tid] = ah[s]; }
@@ -210,7 +183,6 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
       a.out_cache[((size_t)l * a.B + b0 + s) * GH + j] = hst[(l * S + s) * GH + j];
     }
   }
-  if (MC) cluster_sync_all();                     // no CTA leaves while peers may still write to it or signal it
 }
 
 template <int S>
@@ -220,29 +192,9 @@ int launch_s(const GruArgs& a, cudaStream_t st) {
   const int idimP = (a.idim + 3) & ~3;
   const size_t smem = (size_t)(2 * CHUNK_FLOATS + S * GH + a.L * S * GH + 2 * S * GG + S * idimP) * sizeof(float);
   const int sms = device_sm_count();
-  // EXPERIMENTAL, off by default (not yet validated on hardware): WEKWS_GRU_CLUSTER=1 selects the multicast variant
-  const char* mc_env = getenv("WEKWS_GRU_CLUSTER");
-  const bool want_mc = mc_env != nullptr && atoi(mc_env) != 0;
-  if (want_mc && b.n_tiles >= CLUSTER) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_kernel<S, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchConfig_t cfg = {};
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CLUSTER; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.blockDim = dim3(GG); cfg.dynamicSmemBytes = smem; cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
-    cfg.gridDim = dim3(CLUSTER);
-    int max_clusters = 0;
-    WEKWS_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, gru_kernel<S, true>, &cfg));
-    if (max_clusters >= 1) {
-      const int want = (b.n_tiles + CLUSTER - 1) / CLUSTER;
-      cfg.gridDim = dim3((unsigned)((want < max_clusters ? want : max_clusters) * CLUSTER));
-      WEKWS_CUDA_OK(cudaLaunchKernelEx(&cfg, gru_kernel<S, true>, b));
-      return check_launch("gru_kernel");
-    }
-  }
-  WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_kernel<S, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = b.n_tiles < sms ? b.n_tiles : sms;
-  gru_kernel<S, false><<<grid, GG, smem, st>>>(b);
+  gru_kernel<S><<<grid, GG, smem, st>>>(b);
   return check_launch("gru_kernel");
 }
 
@@ -252,10 +204,8 @@ int gru_launch(const GruArgs& a, cudaStream_t st) {
   WEKWS_REQUIRE(a.H == 128, "GRU hidden_dim %d unsupported (128 only)", a.H);
   WEKWS_REQUIRE(a.L >= 1 && a.L <= 4, "GRU num_layers %d unsupported (1..4)", a.L);
   const int sms = device_sm_count();
-  // streams per CTA: keep the grid within one wave;
-  // WEKWS_GRU_S overrides for experiments
-  int S = a.B <= sms ? 1 : a.B <= 2 * sms ? 2 : a.B <= 4 * sms ? 4 : 8;
-  if (const char* e = getenv("WEKWS_GRU_S")) S = atoi(e);
+  // streams per CTA: keep the grid within one wave
+  const int S = a.B <= sms ? 1 : a.B <= 2 * sms ? 2 : a.B <= 4 * sms ? 4 : 8;
   switch (S) {
     case 1: return launch_s<1>(a, st);
     case 2: return launch_s<2>(a, st);

@@ -16,9 +16,6 @@
 //
 // Warps (352 threads): 0-7 unit owners (warpgroup = 64 hidden units): GEMMs, epilogues, gate math, classifier, cache
 // I/O; 8 weight ring (one lane); 9-10 feature rows -> operand image for the next step.
-#include <stdlib.h>
-#include <string.h>
-
 #include "common.cuh"
 #include "gru_tc.h"
 #include "tc_common.cuh"
@@ -390,20 +387,10 @@ bool gru_tc_eligible(int L, int H_, int idim) { return H_ == H && (L == 1 || L =
 // chunk c ^ (n & 7)); per K slab a hi chunk then a lo chunk.  Order: Linear; per layer the gates in the order the
 // kernel computes them: r (W_hr, W_ir), n (W_hn, then W_in), z (W_hz, W_iz).
 void gru_tc_pack(uint8_t* dst, const float* wp /*[H][idim]*/, int idim, const float* const* wih /*[L] of [3H][H]*/,
-                 const float* const* whh, int L, uint16_t (*bf16_rn)(float), float (*bf16_to_f)(uint16_t)) {
-  memset(dst, 0, gru_tc_image_bytes(L, idim));
+                 const float* const* whh, int L) {
   uint8_t* p = dst;
   auto slab = [&](const float* W, int ld, int row0, int k0, int kn) {    // rows row0..row0+127, K k0..k0+kn-1
-    uint8_t* hi_img = p;
-    uint8_t* lo_img = p + CHUNK;
-    for (int n = 0; n < H; ++n)
-      for (int kk = 0; kk < kn; ++kk) {
-        const float w = W[(size_t)(row0 + n) * ld + k0 + kk];
-        const uint16_t hi = bf16_rn(w), lo = bf16_rn(w - bf16_to_f(hi));
-        const size_t off = (size_t)n * 128 + (size_t)(((kk >> 3) ^ (n & 7)) << 4) + (size_t)(kk & 7) * 2;
-        memcpy(hi_img + off, &hi, 2);
-        memcpy(lo_img + off, &lo, 2);
-      }
+    tc::write_sw128_bf16x3(p, H, W + (size_t)row0 * ld + k0, ld, 1, H, kn);
     p += 2 * CHUNK;
   };
   for (int s = 0; s * 64 < idim; ++s) slab(wp, idim, 0, 64 * s, idim - 64 * s < 64 ? idim - 64 * s : 64);
@@ -424,7 +411,6 @@ int gru_tc_launch(GruTcArgs a, cudaStream_t st) {
   // ex2 / rcp per unit and stream), the weight stream per CTA and step is the same 786 KB whatever the tile holds
   const int sms0 = device_sm_count();
   a.ms = a.B > 32 * sms0 ? 64 : a.B > 16 * sms0 ? 32 : 16;
-  if (const char* e = getenv("WEKWS_GRU_MS")) { const int v = atoi(e); if (v == 16 || v == 32 || v == 64) a.ms = v; }
   a.n_tiles = (a.B + a.ms - 1) / a.ms;
   static bool attr_set[64] = {false};
   int dev = 0;

@@ -12,8 +12,6 @@
 //   * per output tile of 128 columns each of the two warpgroups runs K/64 slabs x 3 passes x 4 wgmma (M = 64, N = 128,
 //     K = 16) into a register accumulator, then its epilogue (bias, activation, stores to global).
 // Warps: 0-7 compute (two warpgroups of 64 rows), 8 weight loader.
-#include <string.h>
-
 #include "common.cuh"
 #include "linear_tc.h"
 #include "tc_common.cuh"
@@ -135,21 +133,12 @@ __global__ void __launch_bounds__(NT, 1) linear_tc_kernel(const LinearTcArgs a) 
 size_t linear_tc_image_bytes(int N, int K) { return (size_t)((N + NTILE - 1) / NTILE) * (size_t)(K / 64) * W_SLOT; }
 bool linear_tc_eligible(int N, int K) { return K >= 64 && K <= 256 && K % 64 == 0 && N >= 1; }
 
-void linear_tc_pack(uint8_t* dst, const float* wt, int ldn, int N, int K, uint16_t (*bf16_rn)(float), float (*bf16_to_f)(uint16_t)) {
+void linear_tc_pack(uint8_t* dst, const float* wt, int ldn, int N, int K) {
   const int ntn = (N + NTILE - 1) / NTILE, nslab = K / 64;
-  memset(dst, 0, (size_t)ntn * nslab * W_SLOT);
   for (int nt = 0; nt < ntn; ++nt)
-    for (int s = 0; s < nslab; ++s) {
-      uint8_t* img = dst + (size_t)(nt * nslab + s) * W_SLOT;      // hi at +0, lo at +16384
-      for (int n = 0; n < NTILE && nt * NTILE + n < N; ++n)
-        for (int kk = 0; kk < 64; ++kk) {
-          const float w = wt[(size_t)(64 * s + kk) * ldn + nt * NTILE + n];
-          const uint16_t hi = bf16_rn(w), lo = bf16_rn(w - bf16_to_f(hi));
-          const size_t off = (size_t)n * 128 + (size_t)(((kk >> 3) ^ (n & 7)) << 4) + (size_t)(kk & 7) * 2;
-          memcpy(img + off, &hi, 2);
-          memcpy(img + 16384 + off, &lo, 2);
-        }
-    }
+    for (int s = 0; s < nslab; ++s)
+      tc::write_sw128_bf16x3(dst + (size_t)(nt * nslab + s) * W_SLOT, NTILE, wt + (size_t)64 * s * ldn + nt * NTILE, 1,
+                             ldn, N - nt * NTILE, 64);
 }
 
 int linear_tc_launch(LinearTcArgs a, cudaStream_t st) {

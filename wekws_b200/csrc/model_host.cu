@@ -12,6 +12,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -24,6 +25,7 @@
 #include "fsmn.h"
 #include "linear_tc.h"
 #include "cls_head.h"
+#include "tc_common.cuh"
 
 namespace wekws {
 
@@ -71,6 +73,8 @@ struct Folded {           // BN as per-channel scale/shift
   std::vector<double> s, t;
 };
 
+enum class TcKernel { None, Mdtc, Tcn, DsTcn, Gru };   // the tensor-core kernel a model has, if any
+
 }  // namespace
 }  // namespace wekws
 
@@ -92,17 +96,15 @@ struct wekws_model {
   ConvArgs conv{};
   GruArgs gru{};
   int conv_max_T = 0;
-  // tensor-core path (mdtc, hidden 64)
-  std::vector<std::vector<float>> folded;   // folded GEMM weights W^T [K][64] in consumption order
+  // tensor-core path: the kernel the pack produced (None: the FP32 kernels only) and its pre-swizzled weight images
+  TcKernel tc = TcKernel::None;
+  std::vector<std::vector<float>> folded;   // folded GEMM weights W^T [K][C] in consumption order
   std::vector<uint8_t> h_wimg;
   uint8_t* d_wimg = nullptr;
-  bool tc_ok = false;
-  int precision = 0;                        // 0 auto (tensor cores where eligible), 1 fp32 FFMA only
-  TcArgs tcargs{};
-  bool tcn_ok = false;                      // tensor-core path for the dense TCN (hidden 64)
-  TcnTcArgs tcnargs{};
-  bool ds_ok = false;                       // tensor-core path for the depthwise-separable TCN (hidden 256)
-  DsTcArgs dsargs{};
+  int precision = 0;                        // 0 auto (tensor cores where eligible), 1 fp32 FFMA only, 2 tensor cores
+  TcArgs tcargs{};                          // MDTC, hidden 64
+  TcnTcArgs tcnargs{};                      // dense TCN, hidden 64
+  DsTcArgs dsargs{};                        // depthwise-separable TCN, hidden 256
   FsmnArgs fsmn{};                          // FSMN backbone (fsmn.cu): weights live in h_vec / d_vec
   bool cls_tc = false;                      // wide classifier head (odim > 4) as its own tensor-core GEMM (linear_tc.cu)
   std::vector<uint8_t> h_cimg;              //   behind the tensor-core DS-TCN backbone
@@ -111,8 +113,7 @@ struct wekws_model {
   float* d_cbias = nullptr;
   float* d_hidden = nullptr;                // (B, T, 256) scratch between the two kernels; grows monotonically
   size_t hidden_cap = 0;
-  bool gru_tc_ok = false;                   // tensor-core GRU (gru_tc.cu): weight stream lives in h_wimg / d_wimg
-  GruTcArgs grutc{};
+  GruTcArgs grutc{};                        // tensor-core GRU (gru_tc.cu): weight stream lives in h_wimg / d_wimg
   int head = WEKWS_HEAD_LINEAR;             // wekws_head; GLOBAL / LAST: the backbone kernel pools, cls_head.cu classifies
   int v_w0 = 0, v_b0 = 0, v_w1 = 0, v_b1 = 0;   // the head's MLP in h_vec (pack_head)
   float* d_pool = nullptr;                  // (B, hdim) pooled backbone output between the two kernels; grows monotonically
@@ -226,79 +227,55 @@ int pack_head(wekws_model* m, int H) {
   return WEKWS_OK;
 }
 
-// round-to-nearest-even fp32 -> bf16 (as __floats2bfloat162_rn does on the device)
-uint16_t bf16_rn(float x) {
-  uint32_t u;
-  memcpy(&u, &x, 4);
-  if ((u & 0x7F800000u) == 0x7F800000u) return (uint16_t)(u >> 16);      // inf / nan
-  u += 0x7FFFu + ((u >> 16) & 1u);
-  return (uint16_t)(u >> 16);
-}
-float bf16_to_f(uint16_t h) {
-  uint32_t u = (uint32_t)h << 16;
-  float f;
-  memcpy(&f, &u, 4);
-  return f;
+// 16 KB slot: the K-major SWIZZLE_128B bf16 hi|lo image (tc_common.cuh) of W[n][k0 .. k0+64), n < 64, from W^T [K][64]
+void write_w_image(uint8_t* dst, const std::vector<float>& wt, int K, int k0) {
+  tc::write_sw128_bf16x3(dst, 64, wt.data() + (size_t)k0 * 64, 1, 64, 64, K - k0);
 }
 
-// K-major SWIZZLE_128B image of W[n][k0 .. k0+64) (n < 64): hi at dst, lo at dst + 8192 (tc_common.cuh)
-void write_w_image(uint8_t* dst, const std::vector<float>& wt /*[K][64]*/, int K, int k0) {
-  memset(dst, 0, 16384);
-  for (int n = 0; n < 64; ++n)
-    for (int kk = 0; kk < 64 && k0 + kk < K; ++kk) {
-      const float w = wt[(size_t)(k0 + kk) * 64 + n];
-      const uint16_t hi = bf16_rn(w);
-      const uint16_t lo = bf16_rn(w - bf16_to_f(hi));
-      const size_t off = (size_t)n * 128 + (size_t)(((kk >> 3) ^ (n & 7)) << 4) + (size_t)(kk & 7) * 2;
-      memcpy(dst + off, &hi, 2);
-      memcpy(dst + 8192 + off, &lo, 2);
-    }
-}
-
-// Same layout for 128 output channels n0 .. n0+127 of a [K][ldn] matrix: hi at dst, lo at dst + 16384 (dstcn_tc.cu)
+// 32 KB slot: the same for the 128 output channels n0 .. n0+127 of W^T [K][ldn] (dstcn_tc.cu)
 void write_w_image128(uint8_t* dst, const std::vector<float>& wt, int ldn, int K, int k0, int n0) {
-  memset(dst, 0, 32768);
-  for (int n = 0; n < 128; ++n)
-    for (int kk = 0; kk < 64 && k0 + kk < K; ++kk) {
-      const float w = wt[(size_t)(k0 + kk) * ldn + n0 + n];
-      const uint16_t hi = bf16_rn(w);
-      const uint16_t lo = bf16_rn(w - bf16_to_f(hi));
-      const size_t off = (size_t)n * 128 + (size_t)(((kk >> 3) ^ (n & 7)) << 4) + (size_t)(kk & 7) * 2;
-      memcpy(dst + off, &hi, 2);
-      memcpy(dst + 16384 + off, &lo, 2);
-    }
+  tc::write_sw128_bf16x3(dst, 128, wt.data() + (size_t)k0 * ldn + n0, 1, ldn, 128, K - k0);
 }
 
-// Tensor-core eligibility + pre-swizzled bf16x3 weight images (mdtc_tc.cu, tcn_tc.cu, dstcn_tc.cu)
+// 16 KB slots of the hidden-64 kernels (mdtc_tc.h, tcn_tc.h): [Wp atom0][Wp atom1], then one per folded 64 x 64 GEMM
+void pack_images64(wekws_model* m) {
+  const int idim = m->conv.idim, ngemm = (int)m->folded.size() - 1;
+  m->h_wimg.assign((size_t)(2 + ngemm) * 16384, 0);
+  write_w_image(m->h_wimg.data(), m->folded[0], idim, 0);
+  if (idim > 64) write_w_image(m->h_wimg.data() + 16384, m->folded[0], idim, 64);
+  for (int g = 0; g < ngemm; ++g) write_w_image(m->h_wimg.data() + (size_t)(2 + g) * 16384, m->folded[1 + g], 64, 0);
+}
+
+// the ConvArgs fields every tensor-core conv argument block repeats (TcArgs, TcnTcArgs, DsTcArgs)
+template <class A>
+void init_tc_args(A* t, const ConvArgs& a) {
+  memset(t, 0, sizeof(*t));
+  t->idim = a.idim; t->odim = a.odim; t->nblocks = a.nblocks; t->ktaps = a.ktaps; t->P = a.P;
+  t->act = a.act; t->has_cmvn = a.has_cmvn;
+  t->v_mean = a.v_mean; t->v_istd = a.v_istd; t->v_bp = a.v_bp; t->v_blocks = a.v_blocks;
+  t->v_blk_stride = a.v_blk_stride; t->v_wc = a.v_wc; t->v_bc = a.v_bc;
+  for (int b = 0; b < a.nblocks; ++b) { t->dil[b] = a.dil[b]; t->coff[b] = a.coff[b]; }
+}
+
+// Tensor-core eligibility + pre-swizzled bf16x3 weight images (mdtc_tc.cu, tcn_tc.cu, dstcn_tc.cu); sets m->tc
 void pack_tc(wekws_model* m) {
-  m->tc_ok = false;
-  m->tcn_ok = false;
-  m->ds_ok = false;
+  m->tc = TcKernel::None;
   m->cls_tc = false;
   m->h_wimg.clear();
   m->h_cimg.clear();
   const wekws_model_config& c = m->cfg;
+  const ConvArgs& a = m->conv;
   const bool head = m->head != WEKWS_HEAD_LINEAR;
   if (head && c.backbone != WEKWS_BACKBONE_MDTC) return;     // TCN / DS-TCN heads run on the FP32 conv kernel
   if (c.backbone == WEKWS_BACKBONE_DSTCN) {
-    DsTcArgs& t = m->dsargs;
-    memset(&t, 0, sizeof(t));
-    const ConvArgs& a = m->conv;
-    t.idim = a.idim; t.odim = a.odim; t.nblocks = a.nblocks; t.ktaps = a.ktaps; t.P = a.P;
-    t.act = a.act; t.has_cmvn = a.has_cmvn;
-    t.v_mean = a.v_mean; t.v_istd = a.v_istd; t.v_bp = a.v_bp; t.v_blocks = a.v_blocks;
-    t.v_blk_stride = a.v_blk_stride; t.v_wc = a.v_wc; t.v_bc = a.v_bc;
-    for (int b = 0; b < a.nblocks; ++b) { t.dil[b] = a.dil[b]; t.coff[b] = a.coff[b]; }
+    init_tc_args(&m->dsargs, a);
     // output_dim > 4 (CTC vocabularies): the classifier becomes its own tensor-core GEMM fed from a hidden scratch
-    m->cls_tc = c.odim > 4 && linear_tc_eligible(c.odim, c.hdim);
-    t.hidden = m->cls_tc ? reinterpret_cast<float*>(1) : nullptr;      // placeholder for the eligibility test only
-    const bool ok = dstcn_tc_eligible(t, c.hdim);
-    t.hidden = nullptr;
-    if (!ok) { m->cls_tc = false; return; }
-    if (m->folded.size() != (size_t)(1 + a.nblocks)) { m->cls_tc = false; return; }
-    if (m->cls_tc) {        // W_c^T [256][odim] sits in h_vec at v_wc (pack_classifier), the bias at v_bc
+    const bool cls_tc = c.odim > 4 && linear_tc_eligible(c.odim, c.hdim);
+    if (!dstcn_tc_eligible(m->dsargs, c.hdim, cls_tc) || m->folded.size() != (size_t)(1 + a.nblocks)) return;
+    m->cls_tc = cls_tc;
+    if (cls_tc) {           // W_c^T [256][odim] sits in h_vec at v_wc (pack_classifier), the bias at v_bc
       m->h_cimg.assign(linear_tc_image_bytes(c.odim, c.hdim), 0);
-      linear_tc_pack(m->h_cimg.data(), m->h_vec.data() + a.v_wc, c.odim, c.odim, c.hdim, bf16_rn, bf16_to_f);
+      linear_tc_pack(m->h_cimg.data(), m->h_vec.data() + a.v_wc, c.odim, c.odim, c.hdim);
       m->h_cbias.assign((size_t)((c.odim + 127) / 128) * 128, 0.f);
       for (int j = 0; j < c.odim; ++j) m->h_cbias[j] = m->h_vec[a.v_bc + j];
     }
@@ -310,44 +287,22 @@ void pack_tc(wekws_model* m) {
     for (int b = 0; b < a.nblocks; ++b)
       for (int ks = 0; ks < 4; ++ks)
         for (int h = 0; h < 2; ++h, dst += 32768) write_w_image128(dst, m->folded[1 + b], 256, 256, 64 * ks, 128 * h);
-    m->ds_ok = true;
+    m->tc = TcKernel::DsTcn;
     return;
   }
   if (c.backbone == WEKWS_BACKBONE_TCN && c.hdim == 64) {
-    TcnTcArgs& t = m->tcnargs;
-    memset(&t, 0, sizeof(t));
-    const ConvArgs& a = m->conv;
-    t.idim = a.idim; t.odim = a.odim; t.nblocks = a.nblocks; t.ktaps = a.ktaps; t.P = a.P;
-    t.act = a.act; t.has_cmvn = a.has_cmvn;
-    t.v_mean = a.v_mean; t.v_istd = a.v_istd; t.v_bp = a.v_bp; t.v_blocks = a.v_blocks;
-    t.v_blk_stride = a.v_blk_stride; t.v_wc = a.v_wc; t.v_bc = a.v_bc;
-    for (int b = 0; b < a.nblocks; ++b) { t.dil[b] = a.dil[b]; t.coff[b] = a.coff[b]; }
-    if (!tcn_tc_eligible(t, m->padmax)) return;
-    if (m->folded.size() != (size_t)(1 + a.ktaps * a.nblocks)) return;
-    m->h_wimg.assign((size_t)(2 + a.ktaps * a.nblocks) * 16384, 0);
-    write_w_image(m->h_wimg.data(), m->folded[0], a.idim, 0);
-    if (a.idim > 64) write_w_image(m->h_wimg.data() + 16384, m->folded[0], a.idim, 64);
-    for (int g = 0; g < a.ktaps * a.nblocks; ++g)
-      write_w_image(m->h_wimg.data() + (size_t)(2 + g) * 16384, m->folded[1 + g], 64, 0);
-    m->tcn_ok = true;
+    init_tc_args(&m->tcnargs, a);
+    if (!tcn_tc_eligible(m->tcnargs, m->padmax) || m->folded.size() != (size_t)(1 + a.ktaps * a.nblocks)) return;
+    pack_images64(m);
+    m->tc = TcKernel::Tcn;
     return;
   }
   if (c.backbone != WEKWS_BACKBONE_MDTC || c.hdim != 64) return;
   TcArgs& t = m->tcargs;
-  memset(&t, 0, sizeof(t));
-  const ConvArgs& a = m->conv;
-  t.idim = a.idim; t.odim = a.odim; t.nblocks = a.nblocks; t.ktaps = a.ktaps; t.P = a.P;
-  t.stack_size = a.stack_size; t.act = a.act; t.has_cmvn = a.has_cmvn;
-  t.v_mean = a.v_mean; t.v_istd = a.v_istd; t.v_bp = a.v_bp; t.v_blocks = a.v_blocks;
-  t.v_blk_stride = a.v_blk_stride; t.v_wc = a.v_wc; t.v_bc = a.v_bc;
-  for (int b = 0; b < a.nblocks; ++b) { t.dil[b] = a.dil[b]; t.coff[b] = a.coff[b]; }
-  if (!tc_eligible(t, m->padmax, head)) return;
-  if (m->folded.size() != (size_t)(1 + 2 * a.nblocks)) return;
-  m->h_wimg.assign((size_t)(2 + 2 * a.nblocks) * 16384, 0);
-  write_w_image(m->h_wimg.data(), m->folded[0], a.idim, 0);
-  if (a.idim > 64) write_w_image(m->h_wimg.data() + 16384, m->folded[0], a.idim, 64);
-  for (int g = 0; g < 2 * a.nblocks; ++g)
-    write_w_image(m->h_wimg.data() + (size_t)(2 + g) * 16384, m->folded[1 + g], 64, 0);
+  init_tc_args(&t, a);
+  t.stack_size = a.stack_size;
+  if (!tc_eligible(t, m->padmax, head) || m->folded.size() != (size_t)(1 + 2 * a.nblocks)) return;
+  pack_images64(m);
   // depthwise taps + the two GEMM biases of every block, passed by value with the launch (mdtc_tc.h TcArgs::cw)
   for (int b = 0; b < a.nblocks; ++b) {
     const float* vb = m->h_vec.data() + a.v_blocks + (size_t)b * a.v_blk_stride;
@@ -365,7 +320,7 @@ void pack_tc(wekws_model* m) {
       dst[6 * 64 + ch] = vb[(a.ktaps + 2) * 64 + ch];
     }
   }
-  m->tc_ok = true;
+  m->tc = TcKernel::Mdtc;
 }
 
 int pack_conv(wekws_model* m) {
@@ -511,7 +466,7 @@ int pack_gru(wekws_model* m) {
   if ((rc = pack_classifier(m, H, &a.v_wc, &a.v_bc))) return rc;
   a.L = L; a.H = H; a.idim = idim; a.odim = c.odim; a.act = c.activation; a.has_cmvn = m->has_cmvn ? 1 : 0;
   // tensor-core variant: the per-step weight stream as pre-swizzled bf16 hi|lo operand chunks
-  m->gru_tc_ok = false;
+  m->tc = TcKernel::None;
   m->h_wimg.clear();
   if (gru_tc_eligible(L, H, idim)) {
     const float* wih[4];
@@ -522,13 +477,13 @@ int pack_gru(wekws_model* m) {
       if ((rc = get_tensor(m, "backbone.weight_hh" + sfx, (size_t)G * H, &whh[l]))) return rc;
     }
     m->h_wimg.assign(gru_tc_image_bytes(L, idim), 0);
-    gru_tc_pack(m->h_wimg.data(), wp, idim, wih, whh, L, bf16_rn, bf16_to_f);
+    gru_tc_pack(m->h_wimg.data(), wp, idim, wih, whh, L);
     GruTcArgs& t = m->grutc;
     memset(&t, 0, sizeof(t));
     t.L = L; t.idim = idim; t.odim = c.odim; t.act = c.activation; t.has_cmvn = a.has_cmvn;
     t.v_mean = a.v_mean; t.v_istd = a.v_istd; t.v_bp = a.v_bp; t.v_layers = a.v_layers;
     t.v_layer_stride = a.v_layer_stride; t.v_wc = a.v_wc; t.v_bc = a.v_bc;
-    m->gru_tc_ok = true;
+    m->tc = TcKernel::Gru;
   }
   return WEKWS_OK;
 }
@@ -620,6 +575,43 @@ void free_device(wekws_model* m) {
   m->d_pool = nullptr; m->pool_cap = 0;
 }
 
+template <class T>
+int upload(T** d_dst, const std::vector<T>& h_src) {
+  WEKWS_CUDA_OK(cudaMalloc((void**)d_dst, h_src.size() * sizeof(T)));
+  WEKWS_CUDA_OK(cudaMemcpy(*d_dst, h_src.data(), h_src.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return WEKWS_OK;
+}
+
+// grows a scratch buffer to at least `need` floats; contents are not kept
+int grow_scratch(float** buf, size_t* cap, size_t need, cudaStream_t st) {
+  if (need <= *cap) return WEKWS_OK;
+  WEKWS_CUDA_OK(cudaStreamSynchronize(st));          // the old scratch may still be in use on this stream
+  cudaFree(*buf);
+  *buf = nullptr; *cap = 0;
+  WEKWS_CUDA_OK(cudaMalloc((void**)buf, need * sizeof(float)));
+  *cap = need;
+  return WEKWS_OK;
+}
+
+bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// The kernel a forward call of B streams x T frames takes: the model's tensor-core kernel unless the precision mode,
+// the shape or the pointers rule it out, else TcKernel::None (the FP32 kernel).  feats_aligned: the features are
+// 16-byte aligned; caches_aligned: so are out_cache and in_cache (if given).
+TcKernel select_kernel(const wekws_model* m, int64_t B, int64_t T, bool feats_aligned, bool caches_aligned) {
+  if (m->tc == TcKernel::None || m->precision == 1) return TcKernel::None;
+  if (m->tc == TcKernel::Gru) {
+    // which GRU kernel is faster depends on the batch as well: the weight-streaming tensor-core kernel takes about the
+    // same time per step whatever the batch (up to one 64-stream tile per SM), the FP32 kernel scales with the streams
+    // per SM and has the shorter single-step latency at small batches
+    const bool tc = T >= 1 && (m->precision == 2 || B >= (T == 1 ? 640 : T < 8 ? 400 : 256));
+    return tc ? TcKernel::Gru : TcKernel::None;
+  }
+  // conv backbones: chunks of >= 8 frames; MDTC also reads and writes the cache rows with 16-byte accesses
+  const bool aligned = feats_aligned && (m->tc != TcKernel::Mdtc || caches_aligned);
+  return T >= 8 && aligned ? m->tc : TcKernel::None;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------- C ABI
@@ -694,38 +686,26 @@ extern "C" int wekws_model_finalize(wekws_model* m) {
   if (rc) return rc;
   free_device(m);
   WEKWS_CUDA_OK(cudaGetDevice(&m->device));
-  WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_vec, m->h_vec.size() * sizeof(float)));
-  WEKWS_CUDA_OK(cudaMemcpy(m->d_vec, m->h_vec.data(), m->h_vec.size() * sizeof(float), cudaMemcpyHostToDevice));
+  if ((rc = upload(&m->d_vec, m->h_vec))) return rc;
+  if (m->tc != TcKernel::None && (rc = upload(&m->d_wimg, m->h_wimg))) return rc;
   if (m->cfg.backbone == WEKWS_BACKBONE_FSMN) {
     m->fsmn.w = m->d_vec;
   } else if (m->cfg.backbone != WEKWS_BACKBONE_GRU) {
-    WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_stream, m->h_stream.size() * sizeof(float)));
-    WEKWS_CUDA_OK(cudaMemcpy(m->d_stream, m->h_stream.data(), m->h_stream.size() * sizeof(float), cudaMemcpyHostToDevice));
-    WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_chunk_off, m->h_chunk_off.size() * sizeof(int)));
-    WEKWS_CUDA_OK(cudaMemcpy(m->d_chunk_off, m->h_chunk_off.data(), m->h_chunk_off.size() * sizeof(int), cudaMemcpyHostToDevice));
+    if ((rc = upload(&m->d_stream, m->h_stream))) return rc;
+    if ((rc = upload(&m->d_chunk_off, m->h_chunk_off))) return rc;
     m->conv.wstream = m->d_stream; m->conv.chunk_off = m->d_chunk_off; m->conv.vec = m->d_vec;
-    if (m->tc_ok || m->tcn_ok || m->ds_ok) {
-      WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_wimg, m->h_wimg.size()));
-      WEKWS_CUDA_OK(cudaMemcpy(m->d_wimg, m->h_wimg.data(), m->h_wimg.size(), cudaMemcpyHostToDevice));
-      m->tcargs.wimg = m->d_wimg; m->tcargs.vec = m->d_vec;
-      m->tcnargs.wimg = m->d_wimg; m->tcnargs.vec = m->d_vec;
-      m->dsargs.wimg = m->d_wimg; m->dsargs.vec = m->d_vec;
-    }
+    m->tcargs.wimg = m->d_wimg; m->tcargs.vec = m->d_vec;
+    m->tcnargs.wimg = m->d_wimg; m->tcnargs.vec = m->d_vec;
+    m->dsargs.wimg = m->d_wimg; m->dsargs.vec = m->d_vec;
     if (m->cls_tc) {
-      WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_cimg, m->h_cimg.size()));
-      WEKWS_CUDA_OK(cudaMemcpy(m->d_cimg, m->h_cimg.data(), m->h_cimg.size(), cudaMemcpyHostToDevice));
-      WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_cbias, m->h_cbias.size() * sizeof(float)));
-      WEKWS_CUDA_OK(cudaMemcpy(m->d_cbias, m->h_cbias.data(), m->h_cbias.size() * sizeof(float), cudaMemcpyHostToDevice));
+      if ((rc = upload(&m->d_cimg, m->h_cimg))) return rc;
+      if ((rc = upload(&m->d_cbias, m->h_cbias))) return rc;
     }
     m->conv_max_T = conv_backbone_max_T(m->conv, m->padmax);
     WEKWS_REQUIRE(m->conv_max_T >= 1, "model does not fit the fused kernel's shared memory");
   } else {
     m->gru.vec = m->d_vec;
-    if (m->gru_tc_ok) {
-      WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_wimg, m->h_wimg.size()));
-      WEKWS_CUDA_OK(cudaMemcpy(m->d_wimg, m->h_wimg.data(), m->h_wimg.size(), cudaMemcpyHostToDevice));
-      m->grutc.vec = m->d_vec; m->grutc.wimg = m->d_wimg;
-    }
+    m->grutc.vec = m->d_vec; m->grutc.wimg = m->d_wimg;
   }
   m->finalized = true;
   return WEKWS_OK;
@@ -737,19 +717,9 @@ extern "C" int wekws_model_set_precision(wekws_model* m, int mode) {
   return WEKWS_OK;
 }
 
-// GRU: which kernel is faster depends on the batch as well: the weight-streaming tensor-core kernel takes about the same
-// time per step whatever the batch (up to one 64-stream tile per SM), the FP32 kernel scales with the streams per SM
-// and has the shorter single-step latency at small batches.
-static bool gru_takes_tc(const wekws_model* m, int64_t B, int64_t T) {
-  if (!m->gru_tc_ok || m->precision == 1 || T < 1) return false;
-  if (m->precision == 2) return true;
-  return B >= (T == 1 ? 640 : T < 8 ? 400 : 256);
-}
-
 extern "C" int wekws_model_uses_tensor_cores_bt(const wekws_model* m, int64_t B, int64_t T) {
   if (!m || !m->finalized) return 0;
-  if (m->cfg.backbone == WEKWS_BACKBONE_GRU) return gru_takes_tc(m, B, T) ? 1 : 0;
-  return ((m->tc_ok || m->tcn_ok || m->ds_ok) && m->precision != 1 && T >= 8) ? 1 : 0;
+  return select_kernel(m, B, T, true, true) != TcKernel::None ? 1 : 0;
 }
 
 extern "C" int wekws_model_uses_tensor_cores(const wekws_model* m, int64_t T) {
@@ -787,146 +757,79 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
   WEKWS_CUDA_OK(cudaGetDevice(&dev));
   WEKWS_REQUIRE(dev == m->device, "model was finalized on device %d but current device is %d", m->device, dev);
   cudaStream_t st = (cudaStream_t)stream;
-  if (m->cfg.backbone == WEKWS_BACKBONE_FSMN) {
-    // time-chunk to the tile height; the cache carries the memory-block state between chunks exactly as in streaming use
-    const int maxT = fsmn_tile_rows();
-    const int nchunk = (int)((T + maxT - 1) / maxT);
-    const int Tc = (int)((T + nchunk - 1) / nchunk);
-    for (int64_t t0 = 0; t0 < T; t0 += Tc) {
-      FsmnArgs a = m->fsmn;
-      a.feats = d_feats + t0 * m->cfg.idim;
-      a.out = d_out + t0 * m->cfg.odim;
-      a.in_cache = t0 == 0 ? d_in_cache : d_out_cache;
-      a.out_cache = d_out_cache;
-      a.B = (int)B;
-      a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
-      a.feat_bstride = T * m->cfg.idim;
-      a.out_bstride = T * m->cfg.odim;
-      int rc = fsmn_launch(a, st);
-      if (rc) return rc;
+  const bool head = m->head != WEKWS_HEAD_LINEAR;
+  const TcKernel k = select_kernel(m, B, T, aligned16(d_feats),
+                                   aligned16(d_out_cache) && (d_in_cache == nullptr || aligned16(d_in_cache)));
+  int rc = WEKWS_OK;
+  if (m->cfg.backbone == WEKWS_BACKBONE_GRU) {
+    if (k == TcKernel::Gru) {
+      GruTcArgs a = m->grutc;
+      a.feats = d_feats; a.in_cache = d_in_cache; a.out = d_out; a.out_cache = d_out_cache;
+      a.B = (int)B; a.T = (int)T;
+      rc = gru_tc_launch(a, st);
+    } else {
+      GruArgs a = m->gru;
+      a.feats = d_feats; a.in_cache = d_in_cache; a.out = d_out; a.out_cache = d_out_cache;
+      a.B = (int)B; a.T = (int)T;
+      rc = gru_launch(a, st);
     }
-  } else if (m->cfg.backbone == WEKWS_BACKBONE_GRU && gru_takes_tc(m, B, T)) {
-    GruTcArgs a = m->grutc;
-    a.feats = d_feats; a.in_cache = d_in_cache; a.out = d_out; a.out_cache = d_out_cache;
-    a.B = (int)B; a.T = (int)T;
-    int rc = gru_tc_launch(a, st);
-    if (rc) return rc;
-  } else if (m->cfg.backbone == WEKWS_BACKBONE_GRU) {
-    GruArgs a = m->gru;
-    a.feats = d_feats; a.in_cache = d_in_cache; a.out = d_out; a.out_cache = d_out_cache;
-    a.B = (int)B; a.T = (int)T;
-    int rc = gru_launch(a, st);
     if (rc) return rc;
   } else {
-    // time-chunk long inputs; the cache carries the state between chunks exactly as in
+    // time-chunk long inputs to the kernel's tile height; the cache carries the state between chunks exactly as in
     // streaming use (chunked == full utterance, SURVEY.md 8a "Numerical facts")
-    // tensor-core path: mdtc hidden 64, chunks of >= 8 frames, 16-byte aligned cache rows
-    const bool use_tc = m->tc_ok && m->precision != 1 && T >= 8 &&
-                        (d_in_cache == nullptr || ((uintptr_t)d_in_cache & 15) == 0) &&
-                        ((uintptr_t)d_feats & 15) == 0 && ((uintptr_t)d_out_cache & 15) == 0;
-    const bool use_tcn = m->tcn_ok && m->precision != 1 && T >= 8 && ((uintptr_t)d_feats & 15) == 0;
-    const bool use_ds = m->ds_ok && m->precision != 1 && T >= 8 && ((uintptr_t)d_feats & 15) == 0;
-    const int maxT = use_tc ? tc_max_T() : use_tcn ? tcn_tc_max_T() : use_ds ? dstcn_tc_max_T() : m->conv_max_T;
-    const bool head = m->head != WEKWS_HEAD_LINEAR;
-    if (head) {                     // pooled vector scratch between the backbone kernel(s) and the head kernel
-      const size_t need = (size_t)B * (size_t)m->cfg.hdim;
-      if (need > m->pool_cap) {
-        WEKWS_CUDA_OK(cudaStreamSynchronize(st));          // the old scratch may still be in use on this stream
-        cudaFree(m->d_pool);
-        m->d_pool = nullptr; m->pool_cap = 0;
-        WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_pool, need * sizeof(float)));
-        m->pool_cap = need;
-      }
-    }
-    if (use_ds && m->cls_tc) {      // hidden scratch between the backbone kernel and the classifier GEMM
-      const size_t need = (size_t)B * (size_t)T * (size_t)m->cfg.hdim;
-      if (need > m->hidden_cap) {
-        WEKWS_CUDA_OK(cudaStreamSynchronize(st));          // the old scratch may still be in use on this stream
-        cudaFree(m->d_hidden);
-        m->d_hidden = nullptr; m->hidden_cap = 0;
-        WEKWS_CUDA_OK(cudaMalloc((void**)&m->d_hidden, need * sizeof(float)));
-        m->hidden_cap = need;
-      }
-    }
+    const bool fsmn = m->cfg.backbone == WEKWS_BACKBONE_FSMN;
+    const int maxT = fsmn ? fsmn_tile_rows() : k == TcKernel::Mdtc ? tc_max_T() : k == TcKernel::Tcn ? tcn_tc_max_T()
+                   : k == TcKernel::DsTcn ? dstcn_tc_max_T() : m->conv_max_T;
+    const bool cls_gemm = k == TcKernel::DsTcn && m->cls_tc;      // the classifier runs after the backbone, on d_hidden
+    // scratch between the backbone kernel and the one that follows: pooled vectors (head), hidden rows (cls_gemm)
+    if (head && (rc = grow_scratch(&m->d_pool, &m->pool_cap, (size_t)B * m->cfg.hdim, st))) return rc;
+    if (cls_gemm && (rc = grow_scratch(&m->d_hidden, &m->hidden_cap, (size_t)B * T * m->cfg.hdim, st))) return rc;
     const int nchunk = (int)((T + maxT - 1) / maxT);
     const int Tc = (int)((T + nchunk - 1) / nchunk);
     for (int64_t t0 = 0; t0 < T; t0 += Tc) {
+      const int Tk = (int)(T - t0 < Tc ? T - t0 : Tc);
       // head: the frames of this chunk the pooled vector takes (every frame, or the call's last one) and whether the
       // chunk stores the vector (the first chunk that contributes) or adds to it
-      const int Tk = (int)(T - t0 < Tc ? T - t0 : Tc);
       int pool_t0 = 0, pool_t1 = 0, pool_add = 0;
       if (m->head == WEKWS_HEAD_GLOBAL) { pool_t1 = Tk; pool_add = t0 > 0; }
       else if (m->head == WEKWS_HEAD_LAST && t0 + Tk == T) { pool_t0 = Tk - 1; pool_t1 = Tk; }
-      float* pool = head ? m->d_pool : nullptr;
-      if (use_tc) {
-        TcArgs a = m->tcargs;
+      // the model's argument block with this chunk's call fields
+      auto chunk = [&](auto a) {
+        using A = decltype(a);
         a.feats = d_feats + t0 * m->cfg.idim;
         a.out = d_out + t0 * m->cfg.odim;
         a.in_cache = t0 == 0 ? d_in_cache : d_out_cache;
         a.out_cache = d_out_cache;
         a.B = (int)B;
-        a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
+        a.T = Tk;
         a.feat_bstride = T * m->cfg.idim;
         a.out_bstride = T * m->cfg.odim;
-        a.pool = pool; a.pool_t0 = pool_t0; a.pool_t1 = pool_t1; a.pool_add = pool_add;
-        int rc = mdtc_tc_launch(a, m->padmax, st, head);
-        if (rc) return rc;
-        continue;
+        if constexpr (std::is_same_v<A, TcArgs> || std::is_same_v<A, ConvArgs>) {
+          a.pool = head ? m->d_pool : nullptr; a.pool_t0 = pool_t0; a.pool_t1 = pool_t1; a.pool_add = pool_add;
+        }
+        if constexpr (std::is_same_v<A, DsTcArgs>) {
+          if (cls_gemm) { a.hidden = m->d_hidden + t0 * m->cfg.hdim; a.hidden_bstride = T * m->cfg.hdim; }
+        }
+        return a;
+      };
+      switch (k) {
+        case TcKernel::Mdtc: rc = mdtc_tc_launch(chunk(m->tcargs), m->padmax, st, head); break;
+        case TcKernel::Tcn: rc = tcn_tc_launch(chunk(m->tcnargs), m->padmax, st); break;
+        case TcKernel::DsTcn: rc = dstcn_tc_launch(chunk(m->dsargs), st); break;
+        default: rc = fsmn ? fsmn_launch(chunk(m->fsmn), st) : conv_backbone_launch(chunk(m->conv), m->padmax, st);
       }
-      if (use_ds) {
-        DsTcArgs a = m->dsargs;
-        a.feats = d_feats + t0 * m->cfg.idim;
-        a.out = d_out + t0 * m->cfg.odim;
-        a.in_cache = t0 == 0 ? d_in_cache : d_out_cache;
-        a.out_cache = d_out_cache;
-        a.B = (int)B;
-        a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
-        a.feat_bstride = T * m->cfg.idim;
-        a.out_bstride = T * m->cfg.odim;
-        if (m->cls_tc) { a.hidden = m->d_hidden + t0 * m->cfg.hdim; a.hidden_bstride = T * m->cfg.hdim; }
-        int rc = dstcn_tc_launch(a, st);
-        if (rc) return rc;
-        continue;
-      }
-      if (use_tcn) {
-        TcnTcArgs a = m->tcnargs;
-        a.feats = d_feats + t0 * m->cfg.idim;
-        a.out = d_out + t0 * m->cfg.odim;
-        a.in_cache = t0 == 0 ? d_in_cache : d_out_cache;
-        a.out_cache = d_out_cache;
-        a.B = (int)B;
-        a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
-        a.feat_bstride = T * m->cfg.idim;
-        a.out_bstride = T * m->cfg.odim;
-        int rc = tcn_tc_launch(a, m->padmax, st);
-        if (rc) return rc;
-        continue;
-      }
-      ConvArgs a = m->conv;
-      a.feats = d_feats + t0 * m->cfg.idim;
-      a.out = d_out + t0 * m->cfg.odim;
-      a.in_cache = t0 == 0 ? d_in_cache : d_out_cache;
-      a.out_cache = d_out_cache;
-      a.B = (int)B;
-      a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
-      a.feat_bstride = T * m->cfg.idim;
-      a.out_bstride = T * m->cfg.odim;
-      a.pool = pool; a.pool_t0 = pool_t0; a.pool_t1 = pool_t1; a.pool_add = pool_add;
-      int rc = conv_backbone_launch(a, m->padmax, st);
       if (rc) return rc;
     }
+    if (cls_gemm) {
+      // classifier (+ activation) of all B*T frames in one tensor-core GEMM over the hidden scratch (classifier.py:63-67)
+      LinearTcArgs a;
+      a.x = m->d_hidden; a.out = d_out; a.wimg = m->d_cimg; a.bias = m->d_cbias;
+      a.rows = B * T; a.x_stride = m->cfg.hdim; a.out_stride = m->cfg.odim;
+      a.N = m->cfg.odim; a.K = m->cfg.hdim; a.act = m->cfg.activation; a.n_mtiles = 0;
+      if ((rc = linear_tc_launch(a, st))) return rc;
+    }
   }
-  if (m->cfg.backbone == WEKWS_BACKBONE_DSTCN && m->cls_tc && m->ds_ok && m->precision != 1 && T >= 8 &&
-      ((uintptr_t)d_feats & 15) == 0) {
-    // classifier (+ activation) of all B*T frames in one tensor-core GEMM over the hidden scratch (classifier.py:63-67)
-    LinearTcArgs a;
-    a.x = m->d_hidden; a.out = d_out; a.wimg = m->d_cimg; a.bias = m->d_cbias;
-    a.rows = B * T; a.x_stride = m->cfg.hdim; a.out_stride = m->cfg.odim;
-    a.N = m->cfg.odim; a.K = m->cfg.hdim; a.act = m->cfg.activation; a.n_mtiles = 0;
-    int rc = linear_tc_launch(a, st);
-    if (rc) return rc;
-  }
-  if (m->head != WEKWS_HEAD_LINEAR) {
+  if (head) {
     // MLP head (+ activation, + softmax) on the pooled vectors: (B, odim)
     ClsHeadArgs a;
     a.pool = m->d_pool; a.out = d_out; a.vec = m->d_vec;
@@ -940,8 +843,7 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
     const long long rows = B * T;
     const int wpb = 8;
     softmax_rows_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, st>>>(d_out, rows, m->cfg.odim);
-    int rc = check_launch("softmax_rows_kernel");
-    if (rc) return rc;
+    if ((rc = check_launch("softmax_rows_kernel"))) return rc;
   }
   return WEKWS_OK;
 }

@@ -15,12 +15,47 @@
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 
 namespace wekws {
 namespace tc {
 
+// ------------------------------------------------------------------- host: pre-swizzled weight images
+// round-to-nearest-even fp32 -> bf16 (as __floats2bfloat162_rn does on the device)
+inline uint16_t bf16_rn(float x) {
+  uint32_t u;
+  memcpy(&u, &x, 4);
+  if ((u & 0x7F800000u) == 0x7F800000u) return (uint16_t)(u >> 16);      // inf / nan
+  u += 0x7FFFu + ((u >> 16) & 1u);
+  return (uint16_t)(u >> 16);
+}
+inline float bf16_to_f(uint16_t h) {
+  uint32_t u = (uint32_t)h << 16;
+  float f;
+  memcpy(&f, &u, 4);
+  return f;
+}
+// The hi and lo images of one `rows` x 64 K slab of a weight matrix in the layout above: element (n, k) of the slab is
+// w[n * n_stride + k * k_stride], split as hi = bf16(w), lo = bf16(w - hi).  hi goes to dst, lo to dst + rows * 128;
+// rows n >= n_valid and columns k >= k_valid are zero.
+inline void write_sw128_bf16x3(uint8_t* dst, int rows, const float* w, ptrdiff_t n_stride, ptrdiff_t k_stride,
+                               int n_valid, int k_valid) {
+  uint8_t* lo_img = dst + (size_t)rows * 128;
+  memset(dst, 0, (size_t)rows * 256);
+  for (int n = 0; n < rows && n < n_valid; ++n)
+    for (int kk = 0; kk < 64 && kk < k_valid; ++kk) {
+      const float v = w[n * n_stride + kk * k_stride];
+      const uint16_t hi = bf16_rn(v), lo = bf16_rn(v - bf16_to_f(hi));
+      const size_t off = (size_t)n * 128 + (size_t)(((kk >> 3) ^ (n & 7)) << 4) + (size_t)(kk & 7) * 2;
+      memcpy(dst + off, &hi, 2);
+      memcpy(lo_img + off, &lo, 2);
+    }
+}
+
+// ------------------------------------------------------------------------------ device
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
@@ -114,65 +149,6 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// ---------------------------------------------------------------------- thread-block clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// all threads of all CTAs of the cluster
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
-}
-// wait that traps instead of hanging the GPU if the phase never completes (experimental kernels)
-__device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
-  for (long long spin = 0; spin < (1ll << 26); ++spin) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (done) return;
-  }
-  __trap();
-}
-// wait with cluster-scope acquire (the arrivals come from other CTAs); bounded like the one above
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t done = 0;
-  for (long long spin = 0; !done; ++spin) {
-    if (spin > (1ll << 26)) __trap();
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  }
-}
-// global -> the same shared-memory offset of every CTA in cta_mask; each destination's mbarrier (same offset) gets
-// the bytes as complete_tx
-__device__ __forceinline__ void bulk_g2s_multicast(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar,
-                                                   uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
 // generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / bulk copies)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -187,20 +163,6 @@ __device__ __forceinline__ void wgmma_reg_fence(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// One lane of a converged warp (the single thread that issues a bulk copy or arrives on a barrier).
-__device__ __forceinline__ bool elect_one_sync() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}"
-      : "=r"(pred));
-  return pred != 0;
-}
-// warp-uniform copy of a value every lane holds
-__device__ __forceinline__ uint32_t uniform32(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
 
 // D (+)= A * B^T, bf16 x bf16 -> fp32, issued by a whole warpgroup; B is an [N][K] K-major SW128 image in shared
 // memory; A either four registers (_rs) or an [64][K] K-major SW128 image (_ss).  accumulate == 0 overwrites D.
@@ -210,16 +172,6 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], uint32_t a0, 
       "setp.ne.b32 p, %37, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(desc_b), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void wgmma_m64n32k16_rs(float (&d)[16], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t desc_b, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %21, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
@@ -244,7 +196,7 @@ __device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t des
       : "memory");
 }
 
-// ------------------------------------------------------------------- packed f32x2 math (FFMA2 / FADD2)
+// ------------------------------------------------------------------- packed f32x2 math (FFMA2)
 // Two fp32 values in one 64-bit register (lo = first); element-wise fp32 math on the pair.
 typedef unsigned long long f32x2;
 __device__ __forceinline__ f32x2 pack2(float lo, float hi) {
@@ -259,11 +211,6 @@ __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
   float a0, a1, b0, b1, c0, c1;
   unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
   return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  float a0, a1, b0, b1;
-  unpack2(a, a0, a1); unpack2(b, b0, b1);
-  return pack2(a0 + b0, a1 + b1);
 }
 // 16-byte shared-memory accesses as two packed pairs (shared-window addresses)
 __device__ __forceinline__ void lds_2x2(uint32_t addr, f32x2& a, f32x2& b) {
@@ -306,8 +253,6 @@ __device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;                                // layout type SWIZZLE_128B       [62,64)
   return d;
 }
-// advance a K-major SW128 descriptor by `ksteps` MMA K-steps (16 bf16 = 32 bytes each)
-__device__ __forceinline__ uint64_t sdesc_advance_k(uint64_t desc, int ksteps) { return desc + (uint64_t)(ksteps * 2); }
 
 // byte offset of the 16-byte chunk `chunk` (0..7) of row `row` inside a K-major SW128 operand image
 __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) {
