@@ -260,10 +260,11 @@ def _gru(x, cache, sd, bb, hdim):
     An empty cache raises in the reference (SURVEY: 'Expected hidden size ...');
     start-of-stream therefore means an explicit zero h0 here."""
     L = bb["num_layers"]
-    key = (id(sd), L, hdim)
+    dtype = sd["backbone.weight_ih_l0"].dtype                  # float64 state dicts give a float64 GRU
+    key = (id(sd), L, hdim, dtype)
     g = _GRU_CACHE.get(key)
     if g is None:
-        g = torch.nn.GRU(hdim, hdim, num_layers=L, batch_first=True)
+        g = torch.nn.GRU(hdim, hdim, num_layers=L, batch_first=True, dtype=dtype)
         with torch.no_grad():
             for n, p in g.named_parameters():
                 p.copy_(sd["backbone." + n])

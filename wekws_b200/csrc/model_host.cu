@@ -682,15 +682,25 @@ extern "C" int wekws_model_pack(wekws_model* m) {
 
 extern "C" int wekws_model_finalize(wekws_model* m) {
   WEKWS_REQUIRE(m, "wekws_model_finalize: null handle");
+  m->finalized = false;
   int rc = wekws_model_pack(m);
   if (rc) return rc;
+  const bool conv = m->cfg.backbone != WEKWS_BACKBONE_FSMN && m->cfg.backbone != WEKWS_BACKBONE_GRU;
+  if (conv) {
+    // every conv model keeps the FP32 kernel (T < 8, precision "fp32", misaligned inputs), so its one-frame tile with
+    // the widest cache slice must fit in shared memory, whatever tensor-core kernel the model also has
+    m->conv_max_T = conv_backbone_max_T(m->conv, m->padmax);
+    WEKWS_REQUIRE(m->conv_max_T >= 1, "model does not fit the FP32 conv kernel's shared memory: hidden %d with a "
+                  "widest cache slice of %d frames (dilation x (kernel_size - 1)) leaves no room for one frame",
+                  m->cfg.hdim, m->padmax);
+  }
   free_device(m);
   WEKWS_CUDA_OK(cudaGetDevice(&m->device));
   if ((rc = upload(&m->d_vec, m->h_vec))) return rc;
   if (m->tc != TcKernel::None && (rc = upload(&m->d_wimg, m->h_wimg))) return rc;
   if (m->cfg.backbone == WEKWS_BACKBONE_FSMN) {
     m->fsmn.w = m->d_vec;
-  } else if (m->cfg.backbone != WEKWS_BACKBONE_GRU) {
+  } else if (conv) {
     if ((rc = upload(&m->d_stream, m->h_stream))) return rc;
     if ((rc = upload(&m->d_chunk_off, m->h_chunk_off))) return rc;
     m->conv.wstream = m->d_stream; m->conv.chunk_off = m->d_chunk_off; m->conv.vec = m->d_vec;
@@ -701,8 +711,6 @@ extern "C" int wekws_model_finalize(wekws_model* m) {
       if ((rc = upload(&m->d_cimg, m->h_cimg))) return rc;
       if ((rc = upload(&m->d_cbias, m->h_cbias))) return rc;
     }
-    m->conv_max_T = conv_backbone_max_T(m->conv, m->padmax);
-    WEKWS_REQUIRE(m->conv_max_T >= 1, "model does not fit the fused kernel's shared memory");
   } else {
     m->gru.vec = m->d_vec;
     m->grutc.vec = m->d_vec; m->grutc.wimg = m->d_wimg;
@@ -778,7 +786,7 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
     // time-chunk long inputs to the kernel's tile height; the cache carries the state between chunks exactly as in
     // streaming use (chunked == full utterance, SURVEY.md 8a "Numerical facts")
     const bool fsmn = m->cfg.backbone == WEKWS_BACKBONE_FSMN;
-    const int maxT = fsmn ? fsmn_tile_rows() : k == TcKernel::Mdtc ? tc_max_T() : k == TcKernel::Tcn ? tcn_tc_max_T()
+    const int maxT = fsmn ? fsmn_tile_rows() : k == TcKernel::Mdtc ? tc_max_T() : k == TcKernel::Tcn ? tcn_tc_max_T(m->padmax)
                    : k == TcKernel::DsTcn ? dstcn_tc_max_T() : m->conv_max_T;
     const bool cls_gemm = k == TcKernel::DsTcn && m->cls_tc;      // the classifier runs after the backbone, on d_hidden
     // scratch between the backbone kernel and the one that follows: pooled vectors (head), hidden rows (cls_gemm)

@@ -268,7 +268,12 @@ bool tcn_tc_eligible(const TcnTcArgs& a, int padmax) {
   return true;
 }
 
-int tcn_tc_max_T() { return 128; }
+// a chunk of T frames takes roundup4(padmax) + roundup4(T) columns of X per stream: long receptive fields leave room
+// for fewer than 128 frames (XCOLS and the rounded pad are multiples of 4, so every chunk of this height fits)
+int tcn_tc_max_T(int padmax) {
+  const int room = XCOLS - ((padmax + 3) & ~3);
+  return room < 128 ? room : 128;
+}
 
 int tcn_tc_launch(TcnTcArgs a, int padmax, cudaStream_t st) {
   WEKWS_REQUIRE(a.T >= 1 && a.T <= 128 && a.B >= 1, "tcn_tc_launch: bad shape");

@@ -24,7 +24,7 @@ struct TcnTcArgs {
 };
 
 bool tcn_tc_eligible(const TcnTcArgs& a, int padmax);
-int tcn_tc_max_T();
+int tcn_tc_max_T(int padmax);   // chunk height: 128 frames, fewer when the pad leaves less room in the tile
 int tcn_tc_launch(TcnTcArgs a, int padmax, cudaStream_t st);
 
 }  // namespace wekws
