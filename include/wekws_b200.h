@@ -29,6 +29,10 @@
  *   wekws_pipeline_forward the composition the callers perform: Fbank -> model, i.e.
  *                          stream_kws_ctc.py:482-487 / score.py:117-127, raw PCM in,
  *                          posteriors out.
+ *   wekws_stream_pcm /     the per-stream state of KeyWordSpotter.accept_wave
+ *   wekws_stream_context / wekws/bin/stream_kws_ctc.py:335-398 (PCM remainder, context remainder,
+ *   wekws_ctc_spot         frame-skip offset) and the frame loop of KeyWordSpotter.forward :400-514
+ *                          (beam-search step, execute_detection, resets), for many streams per call.
  */
 #ifndef WEKWS_B200_H_
 #define WEKWS_B200_H_
@@ -40,7 +44,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 5   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head */
+#define WEKWS_B200_ABI_VERSION 6   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -230,6 +234,64 @@ WEKWS_API int wekws_ctc_keyword_hit(const int32_t* d_nhyp, const int32_t* d_hyp_
                           const int32_t* d_node_frame, const float* d_node_prob, int64_t B, int path_beam_size,
                           const int32_t* d_kw_tokens, const int32_t* d_kw_offsets, int num_keywords, int32_t* d_hit,
                           double* d_hit_score, int32_t* d_start, int32_t* d_end, void* stream);
+
+/* Streaming keyword spotter (wekws/bin/stream_kws_ctc.py:400-514, KeyWordSpotter.forward after the model call): for
+ * every stream with d_frames[b] > 0, frames t = 0 .. d_frames[b]-1 at rows d_rows[b] + t of d_probs (row width V), one
+ * step of the streaming prefix beam search (decode_keywords :400-409, hypotheses truncated to path_beam_size) and then
+ * execute_detection (:411-480: first hypothesis in beam order containing a keyword in keyword order, hit_score *=
+ * token probabilities then sqrt, carried across frames; activation needs hit_score >= threshold,
+ * min_frames <= end - start <= max_frames and last_active_pos == -1 or end - last_active_pos >= interval_frames).  On
+ * activation the result is recorded, reset() runs (hypotheses, hit_score) and the rest of the chunk is skipped
+ * (:495-501).  After the chunk total_frames += d_frames[b] * frame_stride and the max_frames reset of :509-512 runs.
+ * Frame numbers are total_frames + t * frame_stride.  Streams with d_frames[b] <= 0 are not touched.
+ *   d_keyword_tokens: {0} + every keyword token (set_keywords :304-333); d_kw_tokens / d_kw_offsets: the keywords'
+ *   token sequences back to back, keyword k = [d_kw_offsets[k], d_kw_offsets[k+1]), each <= WEKWS_CTC_MAX_PREFIX.
+ *   d_state: B x wekws_ctc_state_bytes() hypotheses in the layout of wekws_ctc_prefix_beam_search's d_state (so that
+ *   call with T = 0 and reset_state = 0 reads them out); d_det: B x wekws_ctc_spot_state_bytes() detection record
+ *   (hit_score, total_frames, last_active_pos, overflow).  A zero d_det row is a stream after reset_all() (:521-529):
+ *   its hypotheses are (re)initialised on its first frame, whatever d_state holds.
+ *   d_result[b] (written only for streams with frames) is self.result after the last frame processed: state 1 with
+ *   keyword index, start / end frames and score on activation, else state 0; overflow != 0 if any prefix of the
+ *   stream ever outgrew WEKWS_CTC_MAX_PREFIX tokens.                                                              */
+typedef struct {
+  double score;            /* hit_score at activation                                   */
+  int32_t state;           /* 1 = activated in this chunk                               */
+  int32_t keyword;         /* index into the keyword list, -1 if not activated          */
+  int32_t start, end;      /* frames of the keyword's first / last token                */
+  int32_t overflow;
+  int32_t reserved;
+} wekws_ctc_spot_result;
+WEKWS_API int64_t wekws_ctc_spot_state_bytes(void);
+WEKWS_API int wekws_ctc_spot(const float* d_probs, int V, const int32_t* d_rows, const int32_t* d_frames, int64_t B,
+                   const int32_t* d_keyword_tokens, int n_keyword_tokens, const int32_t* d_kw_tokens,
+                   const int32_t* d_kw_offsets, int num_keywords, int score_beam_size, int path_beam_size,
+                   int frame_stride, double threshold, int min_frames, int max_frames, int interval_frames,
+                   void* d_state, void* d_det, wekws_ctc_spot_result* d_result, void* stream);
+
+/* Streaming front-end state of KeyWordSpotter.accept_wave (wekws/bin/stream_kws_ctc.py:335-398), B streams.
+ *
+ * wekws_stream_pcm (:346-364, the wave_remained bookkeeping): stream b appends d_chunk_len[b] int16 samples of row b
+ * of d_chunk (0 = no new audio) to its remainder of d_rem_len[b] samples (row b of d_remainder, rem_stride samples per
+ * row), writes remainder || chunk to row b of d_stage (stage_stride samples per row; the input of wekws_fbank_forward
+ * with per-stream lengths) and keeps stage[d_consumed[b] .. d_rem_len[b] + d_chunk_len[b]) as its new remainder
+ * (d_consumed = frames * frame_shift, or 0 while the stream holds its audio).  The caller tracks the lengths.
+ *
+ * wekws_stream_context (:366-397, context expansion with the carried feature remainder and frame skip): stream b has
+ * d_nfeat[b] raw feature rows (row width D) at row b of d_feats (feat_stride rows per stream); 0 = no new features,
+ * the stream is not touched.  Its padded sequence is [first row x left] || feats when d_rem_rows[b] == 0 (first chunk)
+ * and remainder[0 .. d_rem_rows[b]) || feats otherwise; context row c is the concatenation of padded rows
+ * c .. c + left + right.  Output row j (j < d_nout[b]) is context row d_skip_off[b] + j * skip, written to row
+ * d_dst_row[b] + j of d_out (row width D * (left + right + 1)).  Then the last min(left + right, nfeat) raw rows become
+ * the stream's remainder (row b of d_remainder, (left + right) x D floats per stream).  left = right = 0: no context
+ * expansion, the rows are copied (frame skip only).  Values are copied, never computed.  d_out may be NULL only
+ * if every d_nout[b] is 0.                                                                                        */
+WEKWS_API int wekws_stream_pcm(const int16_t* d_chunk, int64_t chunk_stride, int64_t B, const int32_t* d_chunk_len,
+                     const int32_t* d_rem_len, const int32_t* d_consumed, int16_t* d_remainder, int64_t rem_stride,
+                     int16_t* d_stage, int64_t stage_stride, void* stream);
+WEKWS_API int wekws_stream_context(const float* d_feats, int64_t feat_stride, int64_t B, int D, const int32_t* d_nfeat,
+                         const int32_t* d_rem_rows, const int32_t* d_skip_off, const int32_t* d_nout,
+                         const int32_t* d_dst_row, int left, int right, int skip, float* d_remainder, float* d_out,
+                         void* stream);
 
 /* Context expansion + frame skipping of the FSMN / CTC recipes (SURVEY 8f-4): wekws/dataset/processor.py:267-312
  * (batched twin wekws/dataset/init_dataset.py:24-68).  d_feats (B,T,D); d_lens NULL = all T frames valid;

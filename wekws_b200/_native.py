@@ -19,7 +19,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 class FbankConfig(C.Structure):
@@ -74,6 +74,15 @@ SIGNATURES = {
     "wekws_ctc_keyword_hit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p]),
+    "wekws_ctc_spot_state_bytes": (C.c_int64, []),
+    "wekws_ctc_spot": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
+                                 C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_int,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_stream_pcm": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
+    "wekws_stream_context": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
     "wekws_context_expand_frames": (C.c_int64, [C.c_int64, C.c_int, C.c_int]),
     "wekws_context_expand": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_void_p, C.c_int64, C.c_void_p]),

@@ -167,6 +167,82 @@ __device__ void advance(Work& w, int t, const int* s_idx, const float* s_prob, i
   w.ncur = keep;
 }
 
+// keyword-token bitmap over V in shared memory (n_allowed = 0: every token allowed)
+__device__ __forceinline__ void build_allow(uint32_t* allow, int V, const int32_t* allowed, int n_allowed, int lane) {
+  const int nwords = (V + 31) / 32;
+  for (int i = lane; i < nwords; i += 32) allow[i] = n_allowed > 0 ? 0u : 0xffffffffu;
+  __syncwarp();
+  if (lane == 0) {
+    for (int i = 0; i < n_allowed; ++i) {
+      const int tkn = allowed[i];
+      if (tkn >= 0 && tkn < V) allow[tkn >> 5] |= 1u << (tkn & 31);
+    }
+  }
+}
+
+// the initial hypothesis list [(tuple(), (1.0, 0.0, []))]
+__device__ __forceinline__ void reset_hyps(Work& w) {
+  w.ncur = 1; w.npool = 0; w.overflow = 0;
+  w.cur[0].pb = 1.0; w.cur[0].pnb = 0.0; w.cur[0].len = 0; w.cur[0].nlen = 0;
+}
+
+__device__ __forceinline__ void load_hyps(Work& w, const Work* st) {
+  w.ncur = st->ncur; w.npool = st->npool; w.overflow = st->overflow;
+  for (int h = 0; h < st->ncur; ++h) w.cur[h] = st->cur[h];
+  for (int i = 0; i < st->npool; ++i) { w.ntok[i] = st->ntok[i]; w.nframe[i] = st->nframe[i]; w.nprob[i] = st->nprob[i]; }
+}
+
+__device__ __forceinline__ void store_hyps(Work* st, const Work& w) {
+  st->ncur = w.ncur; st->npool = w.npool; st->overflow = w.overflow;
+  for (int h = 0; h < w.ncur; ++h) st->cur[h] = w.cur[h];
+  for (int i = 0; i < w.npool; ++i) { st->ntok[i] = w.ntok[i]; st->nframe[i] = w.nframe[i]; st->nprob[i] = w.nprob[i]; }
+}
+
+// probs.topk(score_beam) of one frame p[0..V) followed by the prob > 0.05 / keyword-set filter (loss.py:244-255,
+// stream_kws_ctc.py:144-161): per-lane candidates, then SB rounds of warp arg-max (ties: lower index first).  Every
+// lane returns the same filtered tokens s_idx / s_prob[0..ns) in top-k order.
+__device__ __forceinline__ int topk_filter(const float* p, int V, int SB, const uint32_t* allow, int lane, int* s_idx,
+                                           float* s_prob) {
+  float bv[SBM];
+  int bi[SBM];
+#pragma unroll
+  for (int k = 0; k < SBM; ++k) { bv[k] = -INFINITY; bi[k] = 0x7fffffff; }
+  for (int i = lane; i < V; i += 32) {
+    const float v = __ldg(p + i);
+    if (v > bv[SBM - 1]) {                     // strictly greater: an equal later index never displaces an earlier one
+      bv[SBM - 1] = v; bi[SBM - 1] = i;
+#pragma unroll
+      for (int k = SBM - 1; k > 0; --k) {
+        if (bv[k] > bv[k - 1]) {
+          const float tv = bv[k]; bv[k] = bv[k - 1]; bv[k - 1] = tv;
+          const int ti = bi[k]; bi[k] = bi[k - 1]; bi[k - 1] = ti;
+        }
+      }
+    }
+  }
+  int ns = 0;
+  for (int k = 0; k < SB; ++k) {
+    float mv = bv[0];
+    int mi = bi[0];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, mv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, mi, o);
+      if (ov > mv || (ov == mv && oi < mi)) { mv = ov; mi = oi; }
+    }
+    if (bi[0] == mi && mi != 0x7fffffff) {     // the winning lane pops its head
+#pragma unroll
+      for (int q = 0; q < SBM - 1; ++q) { bv[q] = bv[q + 1]; bi[q] = bi[q + 1]; }
+      bv[SBM - 1] = -INFINITY; bi[SBM - 1] = 0x7fffffff;
+    }
+    // filter: prob > 0.05 (Python float compare of the float32 value) and token in the keyword set
+    if (mi != 0x7fffffff && (double)mv > 0.05 && ((allow[mi >> 5] >> (mi & 31)) & 1u)) {
+      s_idx[ns] = mi; s_prob[ns] = mv; ++ns;
+    }
+  }
+  return ns;
+}
+
 __global__ void __launch_bounds__(32) ctc_prefix_beam_kernel(const CtcArgs a) {
   extern __shared__ __align__(16) uint8_t smem[];
   Work& w = *reinterpret_cast<Work*>(smem);
@@ -177,70 +253,20 @@ __global__ void __launch_bounds__(32) ctc_prefix_beam_kernel(const CtcArgs a) {
   long long n = a.lens ? (long long)a.lens[b] : a.T;
   n = n < 0 ? 0 : (n > a.T ? a.T : n);
 
-  const int nwords = (V + 31) / 32;
-  for (int i = lane; i < nwords; i += 32) allow[i] = a.n_allowed > 0 ? 0u : 0xffffffffu;
-  __syncwarp();
+  build_allow(allow, V, a.allowed, a.n_allowed, lane);
   if (lane == 0) {
-    for (int i = 0; i < a.n_allowed; ++i) {
-      const int tkn = a.allowed[i];
-      if (tkn >= 0 && tkn < V) allow[tkn >> 5] |= 1u << (tkn & 31);
-    }
     // hypotheses: carried state or the initial [(tuple(), (1.0, 0.0, []))]
     Work* st = a.state ? reinterpret_cast<Work*>(a.state + (size_t)b * sizeof(Work)) : nullptr;
-    if (st && !a.reset_state) {
-      w.ncur = st->ncur; w.npool = st->npool; w.overflow = st->overflow;
-      for (int h = 0; h < st->ncur; ++h) w.cur[h] = st->cur[h];
-      for (int i = 0; i < st->npool; ++i) { w.ntok[i] = st->ntok[i]; w.nframe[i] = st->nframe[i]; w.nprob[i] = st->nprob[i]; }
-    } else {
-      w.ncur = 1; w.npool = 0; w.overflow = 0;
-      w.cur[0].pb = 1.0; w.cur[0].pnb = 0.0; w.cur[0].len = 0; w.cur[0].nlen = 0;
-    }
+    if (st && !a.reset_state) load_hyps(w, st);
+    else reset_hyps(w);
   }
   __syncwarp();
 
   const float* P = a.probs + b * a.T * (long long)V;
   for (long long t = 0; t < n; ++t) {
-    const float* p = P + t * V;
-    // ---- probs.topk(score_beam): per-lane candidates, then SB rounds of warp arg-max (ties: lower index first)
-    float bv[SBM];
-    int bi[SBM];
-#pragma unroll
-    for (int k = 0; k < SBM; ++k) { bv[k] = -INFINITY; bi[k] = 0x7fffffff; }
-    for (int i = lane; i < V; i += 32) {
-      const float v = __ldg(p + i);
-      if (v > bv[SBM - 1]) {                     // strictly greater: an equal later index never displaces an earlier one
-        bv[SBM - 1] = v; bi[SBM - 1] = i;
-#pragma unroll
-        for (int k = SBM - 1; k > 0; --k) {
-          if (bv[k] > bv[k - 1]) {
-            const float tv = bv[k]; bv[k] = bv[k - 1]; bv[k - 1] = tv;
-            const int ti = bi[k]; bi[k] = bi[k - 1]; bi[k - 1] = ti;
-          }
-        }
-      }
-    }
     int s_idx[SBM];
     float s_prob[SBM];
-    int ns = 0;
-    for (int k = 0; k < SB; ++k) {
-      float mv = bv[0];
-      int mi = bi[0];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, mv, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, mi, o);
-        if (ov > mv || (ov == mv && oi < mi)) { mv = ov; mi = oi; }
-      }
-      if (bi[0] == mi && mi != 0x7fffffff) {     // the winning lane pops its head
-#pragma unroll
-        for (int q = 0; q < SBM - 1; ++q) { bv[q] = bv[q + 1]; bi[q] = bi[q + 1]; }
-        bv[SBM - 1] = -INFINITY; bi[SBM - 1] = 0x7fffffff;
-      }
-      // filter: prob > 0.05 (Python float compare of the float32 value) and token in the keyword set
-      if (mi != 0x7fffffff && (double)mv > 0.05 && ((allow[mi >> 5] >> (mi & 31)) & 1u)) {
-        s_idx[ns] = mi; s_prob[ns] = mv; ++ns;
-      }
-    }
+    const int ns = topk_filter(P + t * V, V, SB, allow, lane, s_idx, s_prob);
     if (ns == 0) continue;                       // loss.py:254-255: the frame is skipped entirely
     if (lane == 0) advance(w, (int)(a.frame_offset + t * a.frame_stride), s_idx, s_prob, ns, a.path_beam);
     __syncwarp();
@@ -266,18 +292,14 @@ __global__ void __launch_bounds__(32) ctc_prefix_beam_kernel(const CtcArgs a) {
         a.hyp_score[o] = 0.0;
       }
     }
-    if (a.state) {
-      Work* st = reinterpret_cast<Work*>(a.state + (size_t)b * sizeof(Work));
-      st->ncur = w.ncur; st->npool = w.npool; st->overflow = w.overflow;
-      for (int h = 0; h < w.ncur; ++h) st->cur[h] = w.cur[h];
-      for (int i = 0; i < w.npool; ++i) { st->ntok[i] = w.ntok[i]; st->nframe[i] = w.nframe[i]; st->nprob[i] = w.nprob[i]; }
-    }
+    if (a.state) store_hyps(reinterpret_cast<Work*>(a.state + (size_t)b * sizeof(Work)), w);
   }
 }
 
 // score_ctc.py:88-103 (identical copy in stream_kws_ctc.py:105-120), quirk included: for a longer main list the loop
 // runs over range(len(main) - len(check)) and never tests the last offset
-__device__ int is_sublist(const int32_t* main_list, int nm, const int32_t* check, int nc) {
+template <typename Tok>
+__device__ int is_sublist(const Tok* main_list, int nm, const int32_t* check, int nc) {
   if (nm < nc) return -1;
   if (nm == nc) {
     for (int i = 0; i < nc; ++i)
@@ -325,22 +347,135 @@ __global__ void ctc_keyword_hit_kernel(const int32_t* __restrict__ nhyp, const i
   hit[b] = found; hit_score[b] = score; start[b] = st; end[b] = en;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Streaming keyword spotter (stream_kws_ctc.py:400-514, KeyWordSpotter.decode_keywords / execute_detection / the frame
+// loop of forward): per frame one beam-search step, then the detection rules on the carried hypotheses.
+
+// execute_detection (stream_kws_ctc.py:411-480) for the current hypotheses: the first one (beam order) containing a
+// keyword (dict order); hit_score is multiplied by the token probabilities and square-rooted IN PLACE -- it is only
+// ever reset with the hypotheses.  Returns 1 on activation and fills r.
+__device__ int detect(const Work& w, const SpotArgs& a, SpotDet& d, wekws_ctc_spot_result& r) {
+  int hit = -1, start = 0, end = 0;
+  for (int h = 0; h < w.ncur && hit < 0; ++h) {
+    const Hyp& c = w.cur[h];
+    for (int k = 0; k < a.nkw; ++k) {
+      const int32_t* lab = a.kw_tokens + a.kw_off[k];
+      const int nl = a.kw_off[k + 1] - a.kw_off[k];
+      const int off = is_sublist(c.tok, c.len, lab, nl);
+      if (off != -1) {
+        hit = k;
+        start = w.nframe[c.node[off]];
+        end = w.nframe[c.node[off + nl - 1]];
+        for (int i = off; i < off + nl; ++i) d.hit_score = __dmul_rn(d.hit_score, (double)w.nprob[c.node[i]]);
+        break;
+      }
+    }
+    if (hit >= 0) d.hit_score = sqrt(d.hit_score);
+  }
+  const int duration = end - start;
+  if (hit >= 0 && d.hit_score >= a.threshold && a.min_frames <= duration && duration <= a.max_frames &&
+      (d.last_active_pos == -1 || end - d.last_active_pos >= a.interval_frames)) {
+    d.last_active_pos = end;
+    r.score = d.hit_score; r.state = 1; r.keyword = hit; r.start = start; r.end = end;
+    return 1;
+  }
+  return 0;
+}
+
+// KeyWordSpotter.reset(): hypotheses, `activated` and hit_score (the overflow flag of the dropped hypotheses sticks)
+__device__ __forceinline__ void reset_detector(Work& w, SpotDet& d) {
+  d.overflow |= w.overflow;
+  reset_hyps(w);
+  d.hit_score = 1.0;
+}
+
+// one warp per stream; streams with no frames this call are not touched
+__global__ void __launch_bounds__(32) ctc_spot_kernel(const SpotArgs a) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  Work& w = *reinterpret_cast<Work*>(smem);
+  uint32_t* allow = reinterpret_cast<uint32_t*>(smem + sizeof(Work));
+  const int lane = threadIdx.x;
+  const long long b = blockIdx.x;
+  const int n = a.frames[b];
+  if (n <= 0) return;
+
+  build_allow(allow, a.V, a.allowed, a.n_allowed, lane);
+  Work* st = reinterpret_cast<Work*>(a.state + (size_t)b * sizeof(Work));
+  SpotDet* dp = reinterpret_cast<SpotDet*>(a.det + (size_t)b * sizeof(SpotDet));
+  SpotDet d = *dp;                               // lane 0's copy is the one that is used and written back
+  if (lane == 0) {
+    if (d.live) {
+      load_hyps(w, st);
+    } else {                                     // reset_all() (stream_kws_ctc.py:521-529) / a new stream
+      reset_hyps(w);
+      d.hit_score = 1.0; d.total_frames = 0; d.last_active_pos = -1; d.overflow = 0; d.live = 1;
+    }
+  }
+  __syncwarp();
+
+  wekws_ctc_spot_result r;                       // self.result of the last frame processed
+  r.score = 0.0; r.state = 0; r.keyword = -1; r.start = 0; r.end = 0; r.overflow = 0; r.reserved = 0;
+  const float* P = a.probs + (long long)a.rows[b] * a.V;
+  for (int t = 0; t < n; ++t) {
+    int s_idx[SBM];
+    float s_prob[SBM];
+    const int ns = topk_filter(P + (long long)t * a.V, a.V, a.score_beam, allow, lane, s_idx, s_prob);
+    int act = 0;
+    if (lane == 0) {
+      if (ns > 0) advance(w, (int)(d.total_frames + (long long)t * a.frame_stride), s_idx, s_prob, ns, a.path_beam);
+      act = detect(w, a, d, r);
+      if (act) reset_detector(w, d);             // ... and skip the rest of the chunk (stream_kws_ctc.py:495-501)
+    }
+    if (__shfl_sync(0xffffffffu, act, 0)) break;
+  }
+
+  if (lane == 0) {
+    d.total_frames += (long long)n * a.frame_stride;          // every frame of the chunk, even after a break
+    // stream_kws_ctc.py:509-512: drop a hypothesis whose first token is more than max_frames old
+    if (w.ncur > 0 && w.cur[0].len > 0 && d.total_frames - w.nframe[w.cur[0].node[0]] > a.max_frames)
+      reset_detector(w, d);
+    d.overflow |= w.overflow;
+    store_hyps(st, w);
+    *dp = d;
+    r.overflow = d.overflow;
+    a.result[b] = r;
+  }
+}
+
+// the dynamic shared-memory opt-in of a kernel, once per device and size
+int opt_in_smem(const void* kern, size_t smem, size_t* attr_bytes /* [64] */) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev >= 0 && dev < 64 && attr_bytes[dev] < smem) {
+    WEKWS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_bytes[dev] = smem;
+  }
+  return WEKWS_OK;
+}
+
 }  // namespace
 
 size_t ctc_state_bytes() { return sizeof(Work); }
+size_t ctc_spot_state_bytes() { return sizeof(SpotDet); }
 
 int ctc_launch(const CtcArgs& a, cudaStream_t st) {
   const size_t smem = sizeof(Work) + (size_t)((a.V + 31) / 32) * 4;
   WEKWS_REQUIRE(smem <= 227 * 1024, "ctc decode: vocabulary %d too large for the shared-memory token bitmap", a.V);
   static size_t attr_bytes[64] = {0};                  // per device: the largest dynamic size opted into so far
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_bytes[dev] < smem) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(ctc_prefix_beam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_bytes[dev] = smem;
-  }
+  const int rc = opt_in_smem((const void*)ctc_prefix_beam_kernel, smem, attr_bytes);
+  if (rc != WEKWS_OK) return rc;
   ctc_prefix_beam_kernel<<<(unsigned)a.B, 32, smem, st>>>(a);
   return check_launch("ctc_prefix_beam_kernel");
+}
+
+int ctc_spot_launch(const SpotArgs& a, cudaStream_t st) {
+  const size_t smem = sizeof(Work) + (size_t)((a.V + 31) / 32) * 4;
+  WEKWS_REQUIRE(smem <= 227 * 1024, "ctc spot: vocabulary %d too large for the shared-memory token bitmap", a.V);
+  static size_t attr_bytes[64] = {0};
+  const int rc = opt_in_smem((const void*)ctc_spot_kernel, smem, attr_bytes);
+  if (rc != WEKWS_OK) return rc;
+  ctc_spot_kernel<<<(unsigned)a.B, 32, smem, st>>>(a);
+  return check_launch("ctc_spot_kernel");
 }
 
 int ctc_hit_launch(const int32_t* nhyp, const int32_t* hyp_len, const int32_t* hyp_tokens, const int32_t* node_frame,
@@ -398,4 +533,31 @@ extern "C" int wekws_ctc_keyword_hit(const int32_t* d_nhyp, const int32_t* d_hyp
                 "wekws_ctc_keyword_hit: null argument");
   return ctc_hit_launch(d_nhyp, d_hyp_len, d_hyp_tokens, d_node_frame, d_node_prob, B, path_beam_size, d_kw_tokens,
                         d_kw_offsets, num_keywords, d_hit, d_hit_score, d_start, d_end, (cudaStream_t)stream);
+}
+
+extern "C" int64_t wekws_ctc_spot_state_bytes(void) { return (int64_t)ctc_spot_state_bytes(); }
+
+extern "C" int wekws_ctc_spot(const float* d_probs, int V, const int32_t* d_rows, const int32_t* d_frames, int64_t B,
+                              const int32_t* d_keyword_tokens, int n_keyword_tokens, const int32_t* d_kw_tokens,
+                              const int32_t* d_kw_offsets, int num_keywords, int score_beam_size, int path_beam_size,
+                              int frame_stride, double threshold, int min_frames, int max_frames, int interval_frames,
+                              void* d_state, void* d_det, wekws_ctc_spot_result* d_result, void* stream) {
+  WEKWS_REQUIRE(B >= 0 && B < (1ll << 31) && V >= 1 && V <= 32767, "wekws_ctc_spot: bad sizes (vocabulary <= 32767)");
+  WEKWS_REQUIRE(score_beam_size >= 1 && score_beam_size <= WEKWS_CTC_MAX_SCORE_BEAM && score_beam_size <= V,
+                "score_beam_size %d out of range (1..%d)", score_beam_size, WEKWS_CTC_MAX_SCORE_BEAM);
+  WEKWS_REQUIRE(path_beam_size >= 1 && path_beam_size <= WEKWS_CTC_MAX_PATH_BEAM, "path_beam_size %d out of range (1..%d)",
+                path_beam_size, WEKWS_CTC_MAX_PATH_BEAM);
+  WEKWS_REQUIRE(n_keyword_tokens >= 0 && (n_keyword_tokens == 0 || d_keyword_tokens), "keyword token set is null");
+  WEKWS_REQUIRE(num_keywords >= 1 && d_kw_tokens && d_kw_offsets, "wekws_ctc_spot: no keywords");
+  WEKWS_REQUIRE(frame_stride >= 1, "frame_stride must be >= 1");
+  if (B == 0) return WEKWS_OK;
+  WEKWS_REQUIRE(d_probs && d_rows && d_frames && d_state && d_det && d_result, "wekws_ctc_spot: null argument");
+  SpotArgs a;
+  a.probs = d_probs; a.rows = d_rows; a.frames = d_frames; a.B = B; a.V = V;
+  a.allowed = d_keyword_tokens; a.n_allowed = n_keyword_tokens;
+  a.kw_tokens = d_kw_tokens; a.kw_off = d_kw_offsets; a.nkw = num_keywords;
+  a.score_beam = score_beam_size; a.path_beam = path_beam_size; a.frame_stride = frame_stride;
+  a.threshold = threshold; a.min_frames = min_frames; a.max_frames = max_frames; a.interval_frames = interval_frames;
+  a.state = (uint8_t*)d_state; a.det = (uint8_t*)d_det; a.result = d_result;
+  return ctc_spot_launch(a, (cudaStream_t)stream);
 }

@@ -29,7 +29,40 @@ struct CtcArgs {
   float* node_prob;          // (B, path_beam, WEKWS_CTC_MAX_PREFIX)
 };
 
+// Per-stream detection record of the streaming spotter (wekws_ctc_spot_state_bytes).  All zero = a stream that has
+// not decoded a frame since reset_all(); the kernel initialises it on the stream's first frame.
+struct SpotDet {
+  double hit_score;          // KeyWordSpotter.hit_score
+  long long total_frames;    // KeyWordSpotter.total_frames
+  int32_t last_active_pos;   // KeyWordSpotter.last_active_pos
+  int32_t overflow;          // sticky: some prefix outgrew WEKWS_CTC_MAX_PREFIX
+  int32_t live;
+  int32_t pad;
+};
+
+struct SpotArgs {
+  const float* probs;        // softmax posteriors; stream b's frames are rows rows[b] .. rows[b] + frames[b] - 1
+  const int32_t* rows;       // (B)
+  const int32_t* frames;     // (B) frames this call, 0 = stream not touched
+  long long B;
+  int V;
+  const int32_t* allowed;    // keyword token set ({0} + every keyword token)
+  int n_allowed;
+  const int32_t* kw_tokens;  // keyword k = kw_tokens[kw_off[k] .. kw_off[k + 1])
+  const int32_t* kw_off;
+  int nkw;
+  int score_beam, path_beam;
+  int frame_stride;          // downsampling: row t is frame total_frames + t * frame_stride
+  double threshold;
+  int min_frames, max_frames, interval_frames;
+  uint8_t* state;            // B x ctc_state_bytes() hypotheses (the layout ctc_prefix_beam_kernel carries)
+  uint8_t* det;              // B x sizeof(SpotDet)
+  wekws_ctc_spot_result* result;   // (B)
+};
+
 size_t ctc_state_bytes();
+size_t ctc_spot_state_bytes();
+int ctc_spot_launch(const SpotArgs& a, cudaStream_t st);
 int ctc_launch(const CtcArgs& a, cudaStream_t st);
 int ctc_hit_launch(const int32_t* nhyp, const int32_t* hyp_len, const int32_t* hyp_tokens, const int32_t* node_frame,
                    const float* node_prob, long long B, int path_beam, const int32_t* kw_tokens, const int32_t* kw_off,

@@ -128,3 +128,106 @@ def write_ctc_scores(fout, keys: Sequence[str], hits) -> None:
             fout.write('{} detected {} {:.3f}\n'.format(key, word, hit_score))
         else:
             fout.write('{} rejected\n'.format(key))
+
+
+# one wekws_ctc_spot_result per stream (include/wekws_b200.h)
+SPOT_RESULT_DTYPE = [("score", "<f8"), ("state", "<i4"), ("keyword", "<i4"), ("start", "<i4"), ("end", "<i4"),
+                     ("overflow", "<i4"), ("reserved", "<i4")]
+SPOT_RESULT_BYTES = 32
+
+
+def check_spot_args(keywords: Dict[str, Sequence[int]], score_beam_size: int, path_beam_size: int,
+                    frame_stride: int = 1):
+    """Validates the spotter's decoding arguments; returns (keyword names, token-id lists)."""
+    if not keywords:
+        raise ValueError("at least one keyword is needed")
+    if not 1 <= int(score_beam_size) <= MAX_SCORE_BEAM:
+        raise ValueError(f"score_beam_size must be in 1..{MAX_SCORE_BEAM}, got {score_beam_size}")
+    if not 1 <= int(path_beam_size) <= MAX_PATH_BEAM:
+        raise ValueError(f"path_beam_size must be in 1..{MAX_PATH_BEAM}, got {path_beam_size}")
+    if int(frame_stride) < 1:
+        raise ValueError("frame_stride must be >= 1")
+    words = list(keywords)
+    seqs = [[int(t) for t in keywords[w]] for w in words]
+    for w, s in zip(words, seqs):
+        if not 1 <= len(s) <= MAX_PREFIX or min(s) < 0:
+            raise ValueError(f"keyword {w!r}: 1..{MAX_PREFIX} non-negative token ids are needed, got {s}")
+    return words, seqs
+
+
+class CtcSpotDecoder:
+    """The decoding and detection half of the reference's streaming spotter (stream_kws_ctc.py:400-514) for
+    `num_streams` streams, with every piece of state on the device: the hypotheses (ctc_state layout), hit_score,
+    total_frames and last_active_pos.  ``__call__`` runs ctc_spot_kernel once over every stream with frames."""
+
+    def __init__(self, num_streams: int, keywords: Dict[str, Sequence[int]], score_beam_size: int = 3,
+                 path_beam_size: int = 20, frame_stride: int = 1, threshold: float = 0.0, min_frames: int = 5,
+                 max_frames: int = 250, interval_frames: int = 50, device="cuda"):
+        self.words, seqs = check_spot_args(keywords, score_beam_size, path_beam_size, frame_stride)
+        self.B = int(num_streams)
+        self.dev = torch.device(device)
+        self.score_beam, self.path_beam, self.frame_stride = int(score_beam_size), int(path_beam_size), int(frame_stride)
+        self.threshold, self.min_frames = float(threshold), int(min_frames)
+        self.max_frames, self.interval_frames = int(max_frames), int(interval_frames)
+        tokenset = {0}                                          # set_keywords: keywords_idxset = {0} | every token
+        for s in seqs:
+            tokenset.update(s)
+        self.tokenset = tokenset
+        self.max_token = max(tokenset)
+        offs = [0]
+        for s in seqs:
+            offs.append(offs[-1] + len(s))
+        self._set = torch.tensor(sorted(tokenset), dtype=torch.int32, device=self.dev)
+        self._kw = torch.tensor([t for s in seqs for t in s], dtype=torch.int32, device=self.dev)
+        self._off = torch.tensor(offs, dtype=torch.int32, device=self.dev)
+        self.state = ctc_state(self.B, self.dev)
+        self.det = torch.zeros(self.B, int(_native.lib().wekws_ctc_spot_state_bytes()), dtype=torch.uint8,
+                               device=self.dev)
+        self.result = torch.zeros(self.B, SPOT_RESULT_BYTES, dtype=torch.uint8, device=self.dev)
+        self._live = [False] * self.B
+
+    def reset(self, streams: Optional[Iterable[int]] = None) -> None:
+        """KeyWordSpotter.reset_all() for these streams (None = all): a zero detection record restarts the stream."""
+        if streams is None:
+            self.det.zero_()
+            self._live = [False] * self.B
+            return
+        idx = [int(b) for b in streams]
+        if idx:
+            self.det.index_fill_(0, torch.tensor(idx, dtype=torch.int64, device=self.dev), 0)
+        for b in idx:
+            self._live[b] = False
+
+    def __call__(self, probs: torch.Tensor, rows: torch.Tensor, frames: torch.Tensor,
+                 live: Optional[Sequence[bool]] = None) -> torch.Tensor:
+        """probs (R, V) float32 CUDA softmax rows; stream b decodes rows rows[b] .. rows[b] + frames[b] - 1 (int32 CUDA
+        (B,) tensors; frames 0 = stream untouched).  `live`: host copy of frames > 0, if the caller has it.  Returns
+        the (B, 32) byte result buffer (decode with SPOT_RESULT_DTYPE); only streams with frames are written."""
+        if not probs.is_cuda or probs.dtype != torch.float32 or probs.dim() != 2 or not probs.is_contiguous():
+            raise ValueError("probs must be a contiguous (rows, V) float32 CUDA tensor")
+        V = probs.size(1)
+        if self.max_token >= V:
+            raise ValueError(f"keyword token {self.max_token} is outside the vocabulary of {V} outputs")
+        if live is None:
+            live = (frames.cpu() > 0).tolist()
+        for b, x in enumerate(live):
+            if x:
+                self._live[b] = True
+
+        def p(t):
+            return C.c_void_p(t.data_ptr())
+
+        with torch.cuda.device(self.dev):
+            rc = _native.lib().wekws_ctc_spot(
+                p(probs), V, p(rows), p(frames), self.B, p(self._set), self._set.numel(), p(self._kw), p(self._off),
+                len(self.words), self.score_beam, self.path_beam, self.frame_stride, self.threshold, self.min_frames,
+                self.max_frames, self.interval_frames, p(self.state), p(self.det), p(self.result),
+                C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream))
+        _native.check(rc, "wekws_ctc_spot")
+        return self.result
+
+    def hypotheses(self) -> List[list]:
+        """Each stream's carried hypotheses as [(prefix, pb + pnb, nodes)] (hyps_of(cur_hyps))."""
+        out = ctc_prefix_beam_search(torch.empty(self.B, 0, 1, device=self.dev), None, None, 1, self.path_beam,
+                                     state=self.state, reset_state=False).to_python()
+        return [out[b] if self._live[b] else [(tuple(), 1.0, [])] for b in range(self.B)]
