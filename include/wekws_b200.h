@@ -33,6 +33,8 @@
  *   wekws_stream_context / wekws/bin/stream_kws_ctc.py:335-398 (PCM remainder, context remainder,
  *   wekws_ctc_spot         frame-skip offset) and the frame loop of KeyWordSpotter.forward :400-514
  *                          (beam-search step, execute_detection, resets), for many streams per call.
+ *   wekws_ctc_stream_score the per-utterance frame loop of wekws/bin/stream_score_ctc.py:221-377 (streaming
+ *                          decode with its own detection rule over whole utterances of a test set).
  */
 #ifndef WEKWS_B200_H_
 #define WEKWS_B200_H_
@@ -44,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 6   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes */
+#define WEKWS_B200_ABI_VERSION 7   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -267,6 +269,37 @@ WEKWS_API int wekws_ctc_spot(const float* d_probs, int V, const int32_t* d_rows,
                    const int32_t* d_kw_offsets, int num_keywords, int score_beam_size, int path_beam_size,
                    int frame_stride, double threshold, int min_frames, int max_frames, int interval_frames,
                    void* d_state, void* d_det, wekws_ctc_spot_result* d_result, void* stream);
+
+/* Streaming scoring of a CTC test set (wekws/bin/stream_score_ctc.py:221-377): every utterance b decodes its first
+ * d_lens[b] rows of d_probs (B,T,V) frame by frame from the empty hypothesis, with the detection rule of that script
+ * (:236-374), quirks included:
+ *   - a frame whose top-score_beam_size tokens all fail the filter (prob > 0.05 and in d_keyword_tokens) is skipped
+ *     entirely, detection included;
+ *   - hit keyword, start, end and hit_score persist across frames and are reset (with the hypotheses) only on
+ *     activation, so once a keyword has been seen only the first hypothesis is searched and hit_score = sqrt(hit_score)
+ *     runs on every later decoded frame; the stale start / end are tested again;
+ *   - activation needs hit_score >= threshold and min_frames <= end - start <= max_frames (no interval rule) and does
+ *     not end the utterance; decoding goes on and can activate again.
+ * Frame numbers are t * frame_stride (frame_skip), from 0 in each utterance.
+ *   d_keyword_tokens: {0} + every keyword token; d_kw_tokens / d_kw_offsets: the keywords in --keywords order, as in
+ *   wekws_ctc_spot.
+ * Outputs: d_count[b] = activations of utterance b (all of them, even past capacity); d_detections[b * max_detections
+ * + i], i < min(count, max_detections), the activations in firing order; d_overflow[b] != 0 if a prefix outgrew
+ * WEKWS_CTC_MAX_PREFIX tokens.  A caller that finds a count above max_detections launches again with more room:
+ * decoding is deterministic, so the second launch gives the same records.  d_detections may be NULL when
+ * max_detections is 0.                                                                                          */
+typedef struct {
+  double score;            /* hit_score at activation                                   */
+  int32_t keyword;         /* index into the keyword list                               */
+  int32_t start, end;      /* frames of the keyword's first / last token                */
+  int32_t frame;           /* t * frame_stride of the frame that activated              */
+} wekws_ctc_stream_detection;
+WEKWS_API int wekws_ctc_stream_score(const float* d_probs, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                           const int32_t* d_keyword_tokens, int n_keyword_tokens, const int32_t* d_kw_tokens,
+                           const int32_t* d_kw_offsets, int num_keywords, int score_beam_size, int path_beam_size,
+                           int frame_stride, double threshold, int min_frames, int max_frames, int max_detections,
+                           int32_t* d_count, wekws_ctc_stream_detection* d_detections, int32_t* d_overflow,
+                           void* stream);
 
 /* Streaming front-end state of KeyWordSpotter.accept_wave (wekws/bin/stream_kws_ctc.py:335-398), B streams.
  *

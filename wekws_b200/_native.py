@@ -19,7 +19,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 
 class FbankConfig(C.Structure):
@@ -78,6 +78,9 @@ SIGNATURES = {
     "wekws_ctc_spot": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
                                  C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_int,
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_ctc_stream_score": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int,
+                                         C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wekws_stream_pcm": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "wekws_stream_context": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

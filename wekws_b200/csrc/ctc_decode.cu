@@ -3,7 +3,7 @@
 //   wekws/model/loss.py:206-312 ctc_prefix_beam_search (whole utterance, wekws/bin/score_ctc.py:198-200) and its
 //   streaming twin wekws/bin/stream_kws_ctc.py:124-215 (one frame per call, hypotheses carried), followed by the
 //   keyword look-up of score_ctc.py:201-220 / stream_kws_ctc.py:411-434 (is_sublist, sqrt of the product of the
-//   token probabilities).
+//   token probabilities), and the per-utterance streaming scorer of wekws/bin/stream_score_ctc.py:221-377.
 // Bit-exact restatement, including the parts that only exist because of Python object semantics:
 //   * probabilities are float32 values promoted to double, every update is the same sequence of double multiplies and
 //     adds (no FMA contraction), `math.isclose(p, 0.0, abs_tol=1e-6)` is |p| <= 1e-6;
@@ -442,6 +442,90 @@ __global__ void __launch_bounds__(32) ctc_spot_kernel(const SpotArgs a) {
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Streaming scoring of a test set (stream_score_ctc.py:221-377): each utterance decoded frame by frame from the empty
+// hypothesis, with that script's own detection rule.
+
+// The detection variables of stream_score_ctc.py:230-234; they live for the whole utterance.
+struct ScoreDet {
+  double hit_score;
+  int32_t hit, start, end;   // hit_keyword (-1 = None), start, end
+};
+
+// stream_score_ctc.py:321-347 on a decoded frame.  hit / start / end / hit_score are NOT reset per frame: once a keyword
+// has been seen, the loop breaks after the first hypothesis whatever it holds, and hit_score = sqrt(hit_score) runs
+// again.  Returns 1 if the (possibly stale) hit activates.
+__device__ int stream_detect(const Work& w, const StreamScoreArgs& a, ScoreDet& d) {
+  for (int h = 0; h < w.ncur; ++h) {
+    const Hyp& c = w.cur[h];
+    for (int k = 0; k < a.nkw; ++k) {
+      const int32_t* lab = a.kw_tokens + a.kw_off[k];
+      const int nl = a.kw_off[k + 1] - a.kw_off[k];
+      const int off = is_sublist(c.tok, c.len, lab, nl);
+      if (off != -1) {
+        d.hit = k;
+        d.start = w.nframe[c.node[off]];
+        d.end = w.nframe[c.node[off + nl - 1]];
+        for (int i = off; i < off + nl; ++i) d.hit_score = __dmul_rn(d.hit_score, (double)w.nprob[c.node[i]]);
+        break;
+      }
+    }
+    if (d.hit >= 0) {
+      d.hit_score = sqrt(d.hit_score);
+      break;
+    }
+  }
+  const int duration = d.end - d.start;
+  return d.hit >= 0 && d.hit_score >= a.threshold && a.min_frames <= duration && duration <= a.max_frames;
+}
+
+// one warp per utterance, as ctc_prefix_beam_kernel
+__global__ void __launch_bounds__(32) ctc_stream_score_kernel(const StreamScoreArgs a) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  Work& w = *reinterpret_cast<Work*>(smem);
+  uint32_t* allow = reinterpret_cast<uint32_t*>(smem + sizeof(Work));
+  const int lane = threadIdx.x;
+  const long long b = blockIdx.x;
+  long long n = a.lens[b];
+  n = n < 0 ? 0 : (n > a.T ? a.T : n);
+
+  build_allow(allow, a.V, a.allowed, a.n_allowed, lane);
+  ScoreDet d;                                    // lane 0's copy is the one that is used
+  d.hit_score = 1.0; d.hit = -1; d.start = 0; d.end = 0;
+  int count = 0, overflow = 0;
+  if (lane == 0) reset_hyps(w);
+  __syncwarp();
+
+  const float* P = a.probs + b * a.T * (long long)a.V;
+  wekws_ctc_stream_detection* out = a.det + b * (long long)a.max_detections;
+  for (long long t = 0; t < n; ++t) {
+    int s_idx[SBM];
+    float s_prob[SBM];
+    const int ns = topk_filter(P + t * a.V, a.V, a.score_beam, allow, lane, s_idx, s_prob);
+    if (ns == 0) continue;                       // stream_score_ctc.py:260-261: no update and no detection
+    if (lane == 0) {
+      const int frame = (int)(t * a.frame_stride);
+      advance(w, frame, s_idx, s_prob, ns, a.path_beam);
+      if (stream_detect(w, a, d)) {
+        if (count < a.max_detections) {
+          wekws_ctc_stream_detection& r = out[count];
+          r.score = d.hit_score; r.keyword = d.hit; r.start = d.start; r.end = d.end; r.frame = frame;
+        }
+        ++count;
+        overflow |= w.overflow;                  // :357-360: hypotheses, hit_keyword and hit_score start over
+        reset_hyps(w);
+        d.hit = -1; d.hit_score = 1.0;
+      }
+    }
+    __syncwarp();
+  }
+
+  if (lane == 0) {
+    a.count[b] = count;
+    a.overflow[b] = overflow | w.overflow;
+  }
+}
+
 // the dynamic shared-memory opt-in of a kernel, once per device and size
 int opt_in_smem(const void* kern, size_t smem, size_t* attr_bytes /* [64] */) {
   int dev = 0;
@@ -476,6 +560,16 @@ int ctc_spot_launch(const SpotArgs& a, cudaStream_t st) {
   if (rc != WEKWS_OK) return rc;
   ctc_spot_kernel<<<(unsigned)a.B, 32, smem, st>>>(a);
   return check_launch("ctc_spot_kernel");
+}
+
+int ctc_stream_score_launch(const StreamScoreArgs& a, cudaStream_t st) {
+  const size_t smem = sizeof(Work) + (size_t)((a.V + 31) / 32) * 4;
+  WEKWS_REQUIRE(smem <= 227 * 1024, "ctc stream score: vocabulary %d too large for the shared-memory token bitmap", a.V);
+  static size_t attr_bytes[64] = {0};
+  const int rc = opt_in_smem((const void*)ctc_stream_score_kernel, smem, attr_bytes);
+  if (rc != WEKWS_OK) return rc;
+  ctc_stream_score_kernel<<<(unsigned)a.B, 32, smem, st>>>(a);
+  return check_launch("ctc_stream_score_kernel");
 }
 
 int ctc_hit_launch(const int32_t* nhyp, const int32_t* hyp_len, const int32_t* hyp_tokens, const int32_t* node_frame,
@@ -560,4 +654,36 @@ extern "C" int wekws_ctc_spot(const float* d_probs, int V, const int32_t* d_rows
   a.threshold = threshold; a.min_frames = min_frames; a.max_frames = max_frames; a.interval_frames = interval_frames;
   a.state = (uint8_t*)d_state; a.det = (uint8_t*)d_det; a.result = d_result;
   return ctc_spot_launch(a, (cudaStream_t)stream);
+}
+
+static_assert(sizeof(wekws_ctc_stream_detection) == 24, "wekws_ctc_stream_detection layout is part of the C ABI");
+
+extern "C" int wekws_ctc_stream_score(const float* d_probs, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                                      const int32_t* d_keyword_tokens, int n_keyword_tokens, const int32_t* d_kw_tokens,
+                                      const int32_t* d_kw_offsets, int num_keywords, int score_beam_size,
+                                      int path_beam_size, int frame_stride, double threshold, int min_frames,
+                                      int max_frames, int max_detections, int32_t* d_count,
+                                      wekws_ctc_stream_detection* d_detections, int32_t* d_overflow, void* stream) {
+  WEKWS_REQUIRE(B >= 0 && B < (1ll << 31) && T >= 0 && V >= 1 && V <= 32767,
+                "wekws_ctc_stream_score: bad sizes (vocabulary <= 32767)");
+  WEKWS_REQUIRE(T * (int64_t)frame_stride <= INT32_MAX, "wekws_ctc_stream_score: frame numbers overflow int32");
+  WEKWS_REQUIRE(score_beam_size >= 1 && score_beam_size <= WEKWS_CTC_MAX_SCORE_BEAM && score_beam_size <= V,
+                "score_beam_size %d out of range (1..%d)", score_beam_size, WEKWS_CTC_MAX_SCORE_BEAM);
+  WEKWS_REQUIRE(path_beam_size >= 1 && path_beam_size <= WEKWS_CTC_MAX_PATH_BEAM, "path_beam_size %d out of range (1..%d)",
+                path_beam_size, WEKWS_CTC_MAX_PATH_BEAM);
+  WEKWS_REQUIRE(n_keyword_tokens >= 0 && (n_keyword_tokens == 0 || d_keyword_tokens), "keyword token set is null");
+  WEKWS_REQUIRE(num_keywords >= 1 && d_kw_tokens && d_kw_offsets, "wekws_ctc_stream_score: no keywords");
+  WEKWS_REQUIRE(frame_stride >= 1, "frame_stride must be >= 1");
+  WEKWS_REQUIRE(max_detections >= 0, "max_detections must be >= 0");
+  if (B == 0) return WEKWS_OK;
+  WEKWS_REQUIRE((d_probs || T == 0) && d_lens && d_count && d_overflow && (d_detections || max_detections == 0),
+                "wekws_ctc_stream_score: null argument");
+  StreamScoreArgs a;
+  a.probs = d_probs; a.lens = d_lens; a.B = B; a.T = T; a.V = V;
+  a.allowed = d_keyword_tokens; a.n_allowed = n_keyword_tokens;
+  a.kw_tokens = d_kw_tokens; a.kw_off = d_kw_offsets; a.nkw = num_keywords;
+  a.score_beam = score_beam_size; a.path_beam = path_beam_size; a.frame_stride = frame_stride;
+  a.threshold = threshold; a.min_frames = min_frames; a.max_frames = max_frames;
+  a.max_detections = max_detections; a.count = d_count; a.det = d_detections; a.overflow = d_overflow;
+  return ctc_stream_score_launch(a, (cudaStream_t)stream);
 }

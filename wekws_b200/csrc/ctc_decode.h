@@ -60,8 +60,29 @@ struct SpotArgs {
   wekws_ctc_spot_result* result;   // (B)
 };
 
+struct StreamScoreArgs {
+  const float* probs;        // (B, T, V) softmax posteriors
+  const int32_t* lens;       // (B) valid frames
+  long long B, T;
+  int V;
+  const int32_t* allowed;    // keyword token set ({0} + every keyword token)
+  int n_allowed;
+  const int32_t* kw_tokens;  // keyword k = kw_tokens[kw_off[k] .. kw_off[k + 1])
+  const int32_t* kw_off;
+  int nkw;
+  int score_beam, path_beam;
+  int frame_stride;          // frame_skip: row t is frame t * frame_stride
+  double threshold;
+  int min_frames, max_frames;
+  int max_detections;        // records kept per utterance; the count goes on past it
+  int32_t* count;            // (B) activations
+  wekws_ctc_stream_detection* det;   // (B, max_detections)
+  int32_t* overflow;         // (B)
+};
+
 size_t ctc_state_bytes();
 size_t ctc_spot_state_bytes();
+int ctc_stream_score_launch(const StreamScoreArgs& a, cudaStream_t st);
 int ctc_spot_launch(const SpotArgs& a, cudaStream_t st);
 int ctc_launch(const CtcArgs& a, cudaStream_t st);
 int ctc_hit_launch(const int32_t* nhyp, const int32_t* hyp_len, const int32_t* hyp_tokens, const int32_t* node_frame,

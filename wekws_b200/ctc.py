@@ -2,7 +2,8 @@
 
 Replaces the per-utterance / per-frame pure-Python decoding of the reference -- ``wekws/model/loss.py:206-312``
 (``ctc_prefix_beam_search``) as called by ``wekws/bin/score_ctc.py:198-226`` and its streaming twin
-``wekws/bin/stream_kws_ctc.py:124-215,400-434`` -- with one kernel over all utterances, bit-exact (hypothesis
+``wekws/bin/stream_kws_ctc.py:124-215,400-434``, and the streaming scorer ``wekws/bin/stream_score_ctc.py:221-377``
+-- with one kernel over all utterances, bit-exact (hypothesis
 order, scores as doubles, node frames / probabilities; see csrc/ctc_decode.cu for the Python semantics it keeps).
 """
 from __future__ import annotations
@@ -153,6 +154,101 @@ def check_spot_args(keywords: Dict[str, Sequence[int]], score_beam_size: int, pa
         if not 1 <= len(s) <= MAX_PREFIX or min(s) < 0:
             raise ValueError(f"keyword {w!r}: 1..{MAX_PREFIX} non-negative token ids are needed, got {s}")
     return words, seqs
+
+
+# one wekws_ctc_stream_detection per activation (include/wekws_b200.h)
+STREAM_DETECTION_DTYPE = [("score", "<f8"), ("keyword", "<i4"), ("start", "<i4"), ("end", "<i4"), ("frame", "<i4")]
+STREAM_DETECTION_BYTES = 24
+STREAM_SCORE_CAPACITY = 32         # detection records per utterance of the first launch
+
+
+class StreamScores:
+    """Result of stream_score_ctc.  ``count`` (B,) int32: activations per utterance; ``detections`` (B, capacity, 24)
+    uint8: the records in firing order (decode with STREAM_DETECTION_DTYPE); ``overflow`` (B,) int32: != 0 if a
+    prefix outgrew MAX_PREFIX tokens (the decode of that utterance is then not the reference's); ``launches``: kernel
+    launches the call made (1, or 2 when some utterance activated more than STREAM_SCORE_CAPACITY times)."""
+
+    def __init__(self, words, count, detections, overflow, launches):
+        self.words, self.count, self.detections, self.overflow = words, count, detections, overflow
+        self.launches = launches
+
+    def to_python(self) -> List[List[tuple]]:
+        """Per utterance, its activations [(keyword, score, start, end, frame)] in firing order; frame is
+        t * frame_skip of the frame that activated, in the units of start and end."""
+        count = self.count.cpu().tolist()
+        rec = self.detections.cpu().numpy().view(STREAM_DETECTION_DTYPE)[..., 0]
+        return [[(self.words[int(r["keyword"])], float(r["score"]), int(r["start"]), int(r["end"]), int(r["frame"]))
+                 for r in rec[b, :n]] for b, n in enumerate(count)]
+
+
+def stream_score_ctc(probs: torch.Tensor, lengths, keywords: Dict[str, Sequence[int]], score_beam_size: int = 3,
+                     path_beam_size: int = 20, threshold: float = 0.0, min_frames: int = 5, max_frames: int = 250,
+                     frame_skip: int = 1) -> StreamScores:
+    """The frame loop of wekws/bin/stream_score_ctc.py:221-377 over a whole batch, one warp per utterance.
+
+    probs (B, T, V) float32 CUDA softmax posteriors (``model.forward_softmax(feats)`` or ``logits.softmax(2)``);
+    lengths (B,) valid frames (``feats_lengths`` after frame skip); keywords {word: token ids} in --keywords order.
+    Every activation is kept: a first launch stores STREAM_SCORE_CAPACITY records per utterance and counts them all;
+    if some utterance activated more often, one more launch with room for the largest count follows."""
+    words, seqs = check_spot_args(keywords, score_beam_size, path_beam_size, frame_skip)
+    if not torch.is_tensor(probs) or probs.dim() != 3 or probs.dtype != torch.float32:
+        raise ValueError("probs must be a (B, T, V) float32 tensor")
+    B, T, V = probs.shape
+    lens_host = torch.as_tensor(lengths).detach().cpu()
+    if lens_host.numel() == 0:
+        lens_host = lens_host.long()
+    if lens_host.dtype.is_floating_point or lens_host.dtype == torch.bool or tuple(lens_host.shape) != (B,):
+        raise ValueError(f"lengths must be ({B},) integer frame counts")
+    if B and (int(lens_host.min()) < 0 or int(lens_host.max()) > T):
+        raise ValueError(f"lengths must be in 0..{T} (the frames of probs)")
+    tokenset = {0}.union(*[set(s) for s in seqs])
+    if max(tokenset) >= V:
+        raise ValueError(f"keyword token {max(tokenset)} is outside the vocabulary of {V} outputs")
+    if not probs.is_cuda:
+        raise RuntimeError("wekws_b200.stream_score_ctc runs on CUDA only; got a CPU tensor (no CPU fallback)")
+    dev = probs.device
+    probs = probs.contiguous()
+    lens = lens_host.to(device=dev, dtype=torch.int32)
+    tset = torch.tensor(sorted(tokenset), dtype=torch.int32, device=dev)
+    kw = torch.tensor([t for s in seqs for t in s], dtype=torch.int32, device=dev)
+    offs = [0]
+    for s in seqs:
+        offs.append(offs[-1] + len(s))
+    off = torch.tensor(offs, dtype=torch.int32, device=dev)
+    count = torch.zeros(B, dtype=torch.int32, device=dev)
+    overflow = torch.zeros(B, dtype=torch.int32, device=dev)
+
+    def p(t):
+        return C.c_void_p(t.data_ptr())
+
+    def launch(cap):
+        det = torch.empty(B, cap, STREAM_DETECTION_BYTES, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            rc = _native.lib().wekws_ctc_stream_score(
+                p(probs), p(lens), B, T, V, p(tset), tset.numel(), p(kw), p(off), len(words), int(score_beam_size),
+                int(path_beam_size), int(frame_skip), float(threshold), int(min_frames), int(max_frames), cap, p(count),
+                p(det), p(overflow), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        _native.check(rc, "wekws_ctc_stream_score")
+        return det
+
+    cap = STREAM_SCORE_CAPACITY
+    det = launch(cap)
+    launches = 1
+    need = int(count.max()) if B else 0
+    if need > cap:
+        det = launch(need)
+        launches = 2
+    return StreamScores(words, count, det, overflow, launches)
+
+
+def write_stream_ctc_scores(fout, keys: Sequence[str], result: StreamScores) -> None:
+    """The score file of stream_score_ctc.py:349-376: '{key} detected {keyword} {score:.3f}' per activation, or
+    '{key} rejected' for an utterance that never activated."""
+    for key, dets in zip(keys, result.to_python()):
+        if not dets:
+            fout.write('{} rejected\n'.format(key))
+        for word, score, _, _, _ in dets:
+            fout.write('{} detected {} {:.3f}\n'.format(key, word, score))
 
 
 class CtcSpotDecoder:
