@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 7   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection */
+#define WEKWS_B200_ABI_VERSION 8   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_* */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -341,6 +341,40 @@ WEKWS_API int wekws_pipeline_forward(wekws_fbank* fb, wekws_model* m, const void
                            int64_t B, int64_t num_samples, int64_t pcm_stride,
                            float* d_feat_scratch, const float* d_in_cache, float* d_out,
                            float* d_out_cache, uint32_t flags, void* stream);
+
+/* Held-out loss and accuracy with the training criteria of wekws/model/loss.py criterion() (as
+ * wekws/utils/executor.py Executor.cv / Executor.test call it).  Each call writes d_loss (one float: the criterion's
+ * loss) and d_acc (one double: its accuracy) and, when the pointers are not NULL, per-term losses and per-utterance
+ * counts.  d_workspace: the bytes the matching *_workspace_bytes query returns, owned by the caller.
+ *
+ * wekws_criterion_max_pooling (loss.py:26-88): d_logits (B,T,D) posteriors, d_target (B) (< 0 = filler, >= D = no
+ *   keyword column), d_lens (B) with max(lens) == T (the caller checks).  Loss: sum of the B*D terms in (i, j) order
+ *   in float32, / B.  d_acc = correct / B.  d_term_loss (B,D); d_correct (B) 0/1.  2 launches.
+ * wekws_criterion_ce (loss.py:91-100,167-180): d_logits (B,C), d_target (B) in 0..C-1 or -100 (ignored: no term, not
+ *   counted; the caller checks the range).  Loss: mean over the counted rows; d_acc = 100 * (argmax == target) / B.
+ *   d_utt_loss (B); d_correct (B) 0/1.  2 launches.
+ * wekws_criterion_ctc (loss.py:102-164): d_logits (B,T,V) logits, d_lens (B) in 0..T.  Label b is
+ *   d_labels[b * label_stride ...] (padded layout) or, with label_stride == 0, the labels back to back (F.ctc_loss's
+ *   1-D layout); d_label_lens (B); every label <= max_label_len <= WEKWS_CRITERION_MAX_LABEL tokens, each in 0..V-1
+ *   (the caller checks).  Loss: sum of the per-utterance CTC losses (blank 0, +inf for an infeasible utterance) / B.
+ *   validation != 0: d_acc = 100 * sum_b (L_b - edit distance of the best prefix-beam hypothesis (score beam 3, path
+ *   beam 5) to label b) / sum_b L_b over non-empty labels (NaN when every label is empty), d_overflow (B) != 0 if
+ *   utterance b's decode outgrew WEKWS_CTC_MAX_PREFIX tokens (its count is then not the reference's), d_correct (B)
+ *   = L_b - distance, d_best (B, 1 + WEKWS_CTC_MAX_PREFIX) = the best hypothesis' length, then its tokens (-1
+ *   padded).  validation == 0: d_acc = 0.  d_utt_loss (B).  3 launches, 5 with validation.                      */
+#define WEKWS_CRITERION_MAX_LABEL 511
+WEKWS_API int64_t wekws_criterion_max_pooling_workspace_bytes(int64_t B, int D);
+WEKWS_API int wekws_criterion_max_pooling(const float* d_logits, const int32_t* d_target, const int32_t* d_lens,
+                                int64_t B, int64_t T, int D, int min_duration, void* d_workspace, float* d_loss,
+                                double* d_acc, float* d_term_loss, int32_t* d_correct, void* stream);
+WEKWS_API int64_t wekws_criterion_ce_workspace_bytes(int64_t B);
+WEKWS_API int wekws_criterion_ce(const float* d_logits, const int32_t* d_target, int64_t B, int C, void* d_workspace,
+                       float* d_loss, double* d_acc, float* d_utt_loss, int32_t* d_correct, void* stream);
+WEKWS_API int64_t wekws_criterion_ctc_workspace_bytes(int64_t B, int64_t T, int validation);
+WEKWS_API int wekws_criterion_ctc(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                        const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len,
+                        int validation, void* d_workspace, float* d_loss, double* d_acc, float* d_utt_loss,
+                        int32_t* d_correct, int32_t* d_overflow, int32_t* d_best, void* stream);
 
 #ifdef __cplusplus
 }

@@ -12,6 +12,7 @@ Public surface mirrors the reference (wenet-e2e/wekws):
     KeywordSpotter           <- wekws/bin/stream_kws_ctc.py KeyWordSpotter: online CTC keyword spotting, B streams per call
     stream_score_ctc, write_stream_ctc_scores <- wekws/bin/stream_score_ctc.py: streaming decode of a CTC test set
     ctc_det_stats, write_ctc_det_stats <- wekws/bin/compute_det_ctc.py: DET statistics of a CTC score file
+    criterion                <- wekws/model/loss.py criterion(): held-out loss / accuracy (max_pooling, ce, ctc)
     context_expansion        <- wekws/dataset/processor.py context_expansion + frame_skip (FSMN / CTC recipes)
     export_native()          -> weight file for the C++ runtime shim (the role of wekws/bin/export_onnx.py)
     export_onnx()            <- wekws/bin/export_onnx.py: the ONNX file (input, cache -> output, r_cache) for the ORT runtime
@@ -22,6 +23,7 @@ from .frontend import Fbank, Mfcc, fbank, mfcc
 from .kws_model import GlobalCMVN, KWSModel, init_model
 from .ctc import (ctc_keyword_hits, ctc_prefix_beam_search, ctc_state, stream_score_ctc, write_ctc_scores,
                   write_stream_ctc_scores)
+from .criterion import criterion
 from .export import export_native
 from .export_onnx import export_onnx
 from .overlay import patch_reference
@@ -34,5 +36,5 @@ __all__ = ["init_model", "KWSModel", "GlobalCMVN", "Fbank", "fbank", "Mfcc", "mf
            "model_config", "MODEL_NAMES", "patch_reference", "export_native", "export_onnx", "det_stats", "det_curve", "det_thresholds", "context_expansion",
            "Pipeline", "ctc_prefix_beam_search", "ctc_keyword_hits", "ctc_state", "write_ctc_scores",
            "KeywordSpotter", "SpotResult", "stream_score_ctc", "write_stream_ctc_scores", "ctc_det_stats",
-           "write_ctc_det_stats", "space_mixed_label"]
+           "write_ctc_det_stats", "space_mixed_label", "criterion"]
 __version__ = "0.1.0"

@@ -19,7 +19,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 class FbankConfig(C.Structure):
@@ -89,6 +89,16 @@ SIGNATURES = {
     "wekws_context_expand_frames": (C.c_int64, [C.c_int64, C.c_int, C.c_int]),
     "wekws_context_expand": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_void_p, C.c_int64, C.c_void_p]),
+    "wekws_criterion_max_pooling_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int]),
+    "wekws_criterion_max_pooling": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_criterion_ce_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "wekws_criterion_ce": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_criterion_ctc_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64, C.c_int]),
+    "wekws_criterion_ctc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
+                                      C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wekws_pipeline_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64,
                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_uint32, C.c_void_p]),

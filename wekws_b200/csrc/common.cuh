@@ -66,6 +66,18 @@ __device__ __forceinline__ void cp_async_wait_pending(int pending) {
   }
 }
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+// Softmax normaliser of the row p[0..n) across one warp: every lane gets m = max p and s = sum expf(p[i] - m), and
+// the row's softmax is expf(p[i] - m) / s.  The model's softmax and the CTC criterion (log-softmax, and the
+// posteriors its accuracy decodes) share this code, so their probabilities are bit-identical.
+__device__ __forceinline__ void warp_row_max_sum(const float* p, int n, int lane, float& m, float& s) {
+  m = -INFINITY;
+  for (int i = lane; i < n; i += 32) m = fmaxf(m, p[i]);
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  s = 0.f;
+  for (int i = lane; i < n; i += 32) s += expf(p[i] - m);
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+}
 #endif
 
 }  // namespace wekws

@@ -198,17 +198,30 @@ __device__ __forceinline__ void store_hyps(Work* st, const Work& w) {
   for (int i = 0; i < w.npool; ++i) { st->ntok[i] = w.ntok[i]; st->nframe[i] = w.nframe[i]; st->nprob[i] = w.nprob[i]; }
 }
 
+// One frame's posteriors, as stored ...
+struct ProbRow {
+  const float* p;
+  __device__ __forceinline__ float operator()(int i) const { return __ldg(p + i); }
+};
+// ... or formed from the logits and the row's softmax normaliser with softmax_rows_kernel's arithmetic
+struct LogitRow {
+  const float* x;
+  float m, s;
+  __device__ __forceinline__ float operator()(int i) const { return expf(__ldg(x + i) - m) / s; }
+};
+
 // probs.topk(score_beam) of one frame p[0..V) followed by the prob > 0.05 / keyword-set filter (loss.py:244-255,
 // stream_kws_ctc.py:144-161): per-lane candidates, then SB rounds of warp arg-max (ties: lower index first).  Every
 // lane returns the same filtered tokens s_idx / s_prob[0..ns) in top-k order.
-__device__ __forceinline__ int topk_filter(const float* p, int V, int SB, const uint32_t* allow, int lane, int* s_idx,
+template <class Row>
+__device__ __forceinline__ int topk_filter(const Row& p, int V, int SB, const uint32_t* allow, int lane, int* s_idx,
                                            float* s_prob) {
   float bv[SBM];
   int bi[SBM];
 #pragma unroll
   for (int k = 0; k < SBM; ++k) { bv[k] = -INFINITY; bi[k] = 0x7fffffff; }
   for (int i = lane; i < V; i += 32) {
-    const float v = __ldg(p + i);
+    const float v = p(i);
     if (v > bv[SBM - 1]) {                     // strictly greater: an equal later index never displaces an earlier one
       bv[SBM - 1] = v; bi[SBM - 1] = i;
 #pragma unroll
@@ -243,6 +256,7 @@ __device__ __forceinline__ int topk_filter(const float* p, int V, int SB, const 
   return ns;
 }
 
+template <bool kFromLogits>
 __global__ void __launch_bounds__(32) ctc_prefix_beam_kernel(const CtcArgs a) {
   extern __shared__ __align__(16) uint8_t smem[];
   Work& w = *reinterpret_cast<Work*>(smem);
@@ -266,7 +280,14 @@ __global__ void __launch_bounds__(32) ctc_prefix_beam_kernel(const CtcArgs a) {
   for (long long t = 0; t < n; ++t) {
     int s_idx[SBM];
     float s_prob[SBM];
-    const int ns = topk_filter(P + t * V, V, SB, allow, lane, s_idx, s_prob);
+    int ns;
+    if constexpr (kFromLogits) {
+      const long long row = b * a.T + t;
+      ns = topk_filter(LogitRow{P + t * V, __ldg(a.row_max + row), __ldg(a.row_sum + row)}, V, SB, allow, lane, s_idx,
+                       s_prob);
+    } else {
+      ns = topk_filter(ProbRow{P + t * V}, V, SB, allow, lane, s_idx, s_prob);
+    }
     if (ns == 0) continue;                       // loss.py:254-255: the frame is skipped entirely
     if (lane == 0) advance(w, (int)(a.frame_offset + t * a.frame_stride), s_idx, s_prob, ns, a.path_beam);
     __syncwarp();
@@ -419,7 +440,7 @@ __global__ void __launch_bounds__(32) ctc_spot_kernel(const SpotArgs a) {
   for (int t = 0; t < n; ++t) {
     int s_idx[SBM];
     float s_prob[SBM];
-    const int ns = topk_filter(P + (long long)t * a.V, a.V, a.score_beam, allow, lane, s_idx, s_prob);
+    const int ns = topk_filter(ProbRow{P + (long long)t * a.V}, a.V, a.score_beam, allow, lane, s_idx, s_prob);
     int act = 0;
     if (lane == 0) {
       if (ns > 0) advance(w, (int)(d.total_frames + (long long)t * a.frame_stride), s_idx, s_prob, ns, a.path_beam);
@@ -501,7 +522,7 @@ __global__ void __launch_bounds__(32) ctc_stream_score_kernel(const StreamScoreA
   for (long long t = 0; t < n; ++t) {
     int s_idx[SBM];
     float s_prob[SBM];
-    const int ns = topk_filter(P + t * a.V, a.V, a.score_beam, allow, lane, s_idx, s_prob);
+    const int ns = topk_filter(ProbRow{P + t * a.V}, a.V, a.score_beam, allow, lane, s_idx, s_prob);
     if (ns == 0) continue;                       // stream_score_ctc.py:260-261: no update and no detection
     if (lane == 0) {
       const int frame = (int)(t * a.frame_stride);
@@ -542,14 +563,19 @@ int opt_in_smem(const void* kern, size_t smem, size_t* attr_bytes /* [64] */) {
 size_t ctc_state_bytes() { return sizeof(Work); }
 size_t ctc_spot_state_bytes() { return sizeof(SpotDet); }
 
-int ctc_launch(const CtcArgs& a, cudaStream_t st) {
+template <bool kFromLogits>
+int prefix_beam_launch(const CtcArgs& a, cudaStream_t st) {
   const size_t smem = sizeof(Work) + (size_t)((a.V + 31) / 32) * 4;
   WEKWS_REQUIRE(smem <= 227 * 1024, "ctc decode: vocabulary %d too large for the shared-memory token bitmap", a.V);
   static size_t attr_bytes[64] = {0};                  // per device: the largest dynamic size opted into so far
-  const int rc = opt_in_smem((const void*)ctc_prefix_beam_kernel, smem, attr_bytes);
+  const int rc = opt_in_smem((const void*)ctc_prefix_beam_kernel<kFromLogits>, smem, attr_bytes);
   if (rc != WEKWS_OK) return rc;
-  ctc_prefix_beam_kernel<<<(unsigned)a.B, 32, smem, st>>>(a);
+  ctc_prefix_beam_kernel<kFromLogits><<<(unsigned)a.B, 32, smem, st>>>(a);
   return check_launch("ctc_prefix_beam_kernel");
+}
+
+int ctc_launch(const CtcArgs& a, cudaStream_t st) {
+  return a.row_max ? prefix_beam_launch<true>(a, st) : prefix_beam_launch<false>(a, st);
 }
 
 int ctc_spot_launch(const SpotArgs& a, cudaStream_t st) {
@@ -613,6 +639,7 @@ extern "C" int wekws_ctc_prefix_beam_search(const float* d_probs, const int32_t*
   a.state = (uint8_t*)d_state; a.reset_state = reset_state;
   a.nhyp = d_nhyp; a.overflow = d_overflow; a.hyp_len = d_hyp_len; a.hyp_tokens = d_hyp_tokens; a.hyp_score = d_hyp_score;
   a.node_frame = d_node_frame; a.node_prob = d_node_prob;
+  a.row_max = nullptr; a.row_sum = nullptr;
   return ctc_launch(a, (cudaStream_t)stream);
 }
 

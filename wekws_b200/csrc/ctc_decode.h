@@ -27,6 +27,10 @@ struct CtcArgs {
   double* hyp_score;         // (B, path_beam)      pb + pnb
   int32_t* node_frame;       // (B, path_beam, WEKWS_CTC_MAX_PREFIX)
   float* node_prob;          // (B, path_beam, WEKWS_CTC_MAX_PREFIX)
+  // nullptr: `probs` are posteriors.  Otherwise `probs` are logits and row (b, t) of the posteriors is
+  // expf(x - row_max[b * T + t]) / row_sum[b * T + t], formed on load (the criterion's accuracy decode).
+  const float* row_max;
+  const float* row_sum;
 };
 
 // Per-stream detection record of the streaming spotter (wekws_ctc_spot_state_bytes).  All zero = a stream that has

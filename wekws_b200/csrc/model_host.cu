@@ -60,12 +60,8 @@ __global__ void softmax_rows_kernel(float* x, long long rows, int n) {
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
   float* p = x + row * n;
-  float m = -INFINITY;
-  for (int i = lane; i < n; i += 32) m = fmaxf(m, p[i]);
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  float s = 0.f;
-  for (int i = lane; i < n; i += 32) s += expf(p[i] - m);
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  float m, s;
+  warp_row_max_sum(p, n, lane, m, s);
   for (int i = lane; i < n; i += 32) p[i] = expf(p[i] - m) / s;
 }
 
