@@ -9,8 +9,9 @@
 //     pointwise-2 GEMM; B (weights) is a pre-swizzled K-major SWIZZLE_128B image in shared memory, streamed by
 //     cp.async.bulk into a 2-slot ring;
 //   * a 128-row tile is one GROUP of two warpgroups (64 rows each, accumulator 64 x 64 fp32 in registers), and the
-//     groups run the network independently of each other (a 256-thread named barrier per group), so the CUDA-core
-//     phases of one tile overlap the tensor-core phases of the other.
+//     groups run the network independently of each other (a named barrier per group over its live warps), so the
+//     CUDA-core phases of one tile overlap the tensor-core phases of the other; a warpgroup with no row in the pass
+//     only keeps the weight ring and the loader's barriers in step.
 //
 // One CTA per SM holds ALL of its streams (up to 7 x 40 frames) resident for the whole network.  The residual stream is
 // CHANNEL-MINOR: X[col][64 ch] (256 B per frame column, every stream's cache slice in the columns directly in front of
@@ -64,7 +65,10 @@ static_assert(OFF_W % 1024 == 0, "weight images must be 1024-byte aligned");
 static_assert(SMEM_TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 static_assert(SMEM_TOTAL_HEAD <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 
-__device__ __forceinline__ void group_barrier(int grp) { asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(32 * WPG) : "memory"); }
+// named barrier of tile grp's nlw live compute warps
+__device__ __forceinline__ void group_barrier(int grp, int nlw) {
+  asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "r"(32 * nlw) : "memory");
+}
 __device__ __forceinline__ float2 lds_f2(uint32_t addr) {
   float2 v;
   asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
@@ -84,9 +88,10 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, in
 }
 
 
-// The service roles are separate NON-INLINED functions on purpose: compiled on their own they do not compete with the
-// compute groups for uniform registers, which is what lets ptxas keep the per-block tap / bias constants of the
-// compute code in the uniform datapath (LDCU + FFMA2 / FADD2 with UR operands) instead of vector LDC loads.
+// The service roles are separate NON-INLINED functions: compiled on their own, their state does not add to the register
+// pressure of the compute code.  (Under the wgmma fragment layout the per-block tap / bias constants are read with
+// lane-indexed LDC from the parameter bank, four distinct addresses per warp.  Reading them instead from a
+// fragment-ordered global array with __ldg was measured 11 % slower on H100: see DESIGN.md section 3.)
 struct Bars {
   uint64_t *halo_bar, *h_free, *w_bar, *w_free, *stg_bar;
 };
@@ -293,7 +298,12 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
       // warp = grp * WPG + 4 wg + w: warpgroup wg of the tile owns rows [64 wg, 64 wg + 64) and runs their GEMMs; a thread
       // holds the wgmma fragment of rows r0 and r0 + 8 (r0 = 64 wg + 16 w + lane / 4), channel pairs 8 m + 2 (lane % 4)
       const int grp = warp / WPG, wq = warp % WPG;
-      if (grp < ntile) {
+      // live warps of the group: a tile of <= 64 rows leaves warpgroup 1 without a row (the flagship 1024 x 40 shape
+      // runs its 8-stream CTAs as two passes of 3 + 1 streams, so every pass has one), and that warpgroup skips the
+      // depthwise conv, the GEMMs and the epilogues.  The head variant keeps all eight: its pooling splits the
+      // channels over the group's warps.
+      const int nlw = (grp < ntile && !HEAD && tile_streams(grp) * T <= 64) ? WPG / 2 : WPG;
+      if (grp < ntile && wq < nlw) {
         const int nst = tile_streams(grp), rows = nst * T;
         const int q4 = lane & 3, r0 = 64 * (wq >> 2) + 16 * (wq & 3) + (lane >> 2);
         const uint32_t qoff = 128u * (uint32_t)(q4 >> 1) + 8u * (uint32_t)(q4 & 1);   // channel pair 2 q4 inside a chunk
@@ -382,7 +392,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             if (live[h])
               sts_f2(((t_own[h] ^ ((uint32_t)j << 4)) + qoff), fmaxf(acc[4 * j + 2 * h] + b.x, 0.f), fmaxf(acc[4 * j + 2 * h + 1] + b.y, 0.f));
         }
-        group_barrier(grp);                  // X of the tile complete before the first depthwise conv reads across rows
+        group_barrier(grp, nlw);                // X of the tile complete before the first depthwise conv reads across rows
 
         // ---- blocks
         for (int blk = 0; blk < a.nblocks; ++blk) {
@@ -434,7 +444,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             const int jpl = pad < 32 ? pad : 32, lgj = 31 - __clz(jpl), qstep = 32 >> lgj;
             const int j = lane & (jpl - 1), qs = lane >> lgj, per = 16 >> (5 - lgj);      // quads passes per stream
             const int nitem = nst * per;
-            for (int it = wq; it < nitem; it += WPG) {
+            for (int it = wq; it < nitem; it += nlw) {
               const int s2 = it / per, cq = (it - s2 * per) * qstep + qs;
               const int sg2 = grp * spt + s2;
               const uint32_t cc = (uint32_t)(sg2 * Lw + PADR + T - pad + j);
@@ -463,7 +473,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             }
           // ---------------- pointwise-2 GEMM; x' = relu(D + b2 + x) -> X; classifier partial sums at the end of a stack
           gemm(1, 4, true);                                                    // (mdtc.py:116-118, 266-273)
-          group_barrier(grp);                // every row's depthwise taps and cache stores have read x
+          group_barrier(grp, nlw);              // every row's depthwise taps and cache stores have read x
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int ch = 8 * j + 2 * q4;
@@ -483,7 +493,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
               }
             }
           }
-          group_barrier(grp);                // x' of every row of the tile complete before the next block's conv
+          group_barrier(grp, nlw);              // x' of every row of the tile complete before the next block's conv
           if constexpr (HEAD) {
             // X now holds the stack output of every frame of the tile, and stays so until the next block's second
             // group barrier.  Warp wq sums channels 8 wq .. 8 wq + 7; lane = 8 q + channel, q = frame phase mod 4:
@@ -543,8 +553,9 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
         }
         }  // !HEAD
       } else {
-        // a group without streams in this pass still releases every weight slot use (w_free counts every compute
-        // warp's arrival); all lanes keep the same phase bookkeeping
+        // a group without streams in this pass, or a warpgroup without rows in a live tile, still releases every
+        // weight slot use (w_free counts every compute warp's arrival); all lanes keep the same phase bookkeeping
+        const bool in_tile = grp < ntile;
         mbar_wait(&w_bar[0], w_par & 1);
         if (lane == 0) mbar_arrive(&w_free[0]);
         if (natoms > 1) {
@@ -557,7 +568,12 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             mbar_wait(&w_bar[job], (w_par >> job) & 1);
             w_par ^= 1u << job;
             if (lane == 0) mbar_arrive(&w_free[job]);
+            // in a live tile it also stands in for its share of h_free (WPG arrivals per block).  Arriving only once
+            // W1 of the block has landed keeps it in step: W1(blk + 1) is loaded only after every live warp's
+            // pointwise-1 GEMM of blk, and each live warp arrives on h_free(blk) before that GEMM.
+            if (job == 0 && in_tile && lane == 0) mbar_arrive(&h_free[grp]);
           }
+        if (in_tile) halo_par ^= (uint32_t)a.nblocks & 1u;   // the tile's halo_bar went through nblocks phases
       }
     } else if (warp == W_WGT) {
       if (lane == 0) weights_role(a, base, bars, K, natoms, wf_par, b0 == sb);
