@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 8   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_* */
+#define WEKWS_B200_ABI_VERSION 9   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_* */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -375,6 +375,37 @@ WEKWS_API int wekws_criterion_ctc(const float* d_logits, const int32_t* d_lens, 
                         const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len,
                         int validation, void* d_workspace, float* d_loss, double* d_acc, float* d_utt_loss,
                         int32_t* d_correct, int32_t* d_overflow, int32_t* d_best, void* stream);
+
+/* Resampling: torchaudio.transforms.Resample(orig_freq, new_freq) with sinc_interp_hann (the resampling of
+ * wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py:50-53), for B waveforms of their own lengths.
+ * h_kernel: the (new/g, 2*width + orig/g) float32 table of torchaudio's _get_sinc_resample_kernel (g = gcd of the
+ * rates) and its width.  The handle keeps each phase's non-zero span in shared memory; create refuses a rate pair
+ * whose compact table does not fit (WEKWS_ERR_INVALID, the message states the size).  Equal rates are refused too:
+ * the transform returns its input unchanged.
+ * wekws_resample_output_length = ceil(new * n / orig) (0 for n = 0).
+ * wekws_resample_forward: d_pcm as wekws_fbank_forward (int16 or float32 at int16 scale, row b at b * pcm_stride
+ * elements); d_lens optional (NULL = num_samples each; samples at or past lens[b] count as zeros, they are never
+ * read as data).  Row b of d_out (out_stride floats per row) gets the resampling of its first lens[b] samples,
+ * accumulated in double and rounded once to float32, then zeros up to max_out, which must be at least
+ * wekws_resample_output_length(num_samples).  One launch.                                                      */
+typedef struct wekws_resample wekws_resample;
+WEKWS_API int wekws_resample_create(int orig_freq, int new_freq, const float* h_kernel, int width,
+                                    wekws_resample** out);
+WEKWS_API void wekws_resample_destroy(wekws_resample* h);
+WEKWS_API int64_t wekws_resample_output_length(const wekws_resample* h, int64_t num_samples);
+WEKWS_API int wekws_resample_forward(wekws_resample* h, const void* d_pcm, int pcm_dtype, int64_t B,
+                                     int64_t num_samples, int64_t pcm_stride, const int32_t* d_lens, float* d_out,
+                                     int64_t out_stride, int64_t max_out, void* stream);
+
+/* Global CMVN statistics (tools/compute_cmvn_stats.py): adds the first d_frames[b] rows of every utterance of
+ * d_feats (B, max_frames, D) to d_acc = double[2][D] (sum x, then sum x^2, per dimension) and their count to
+ * *d_frame_num.  Per-utterance sums are formed in double in a fixed order and folded into d_acc in utterance order,
+ * so the result depends on the order of the utterances only, not on how they are split into calls.
+ * d_workspace: wekws_cmvn_stats_workspace_bytes(B, D) bytes owned by the caller.  Two launches.                 */
+WEKWS_API int64_t wekws_cmvn_stats_workspace_bytes(int64_t B, int D);
+WEKWS_API int wekws_cmvn_stats_accumulate(const float* d_feats, int64_t B, int64_t max_frames, int D,
+                                          const int32_t* d_frames, double* d_acc, int64_t* d_frame_num,
+                                          void* d_workspace, void* stream);
 
 #ifdef __cplusplus
 }

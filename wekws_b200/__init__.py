@@ -4,6 +4,8 @@ Public surface mirrors the reference (wenet-e2e/wekws):
     init_model, KWSModel     <- wekws/model/kws_model.py
     Fbank, fbank             <- torchaudio.compliance.kaldi.fbank as the reference calls it
     Mfcc, mfcc               <- torchaudio.compliance.kaldi.mfcc  (processor.py:157-166, the mdtc configs' front-end)
+    Resample, resample       <- torchaudio.transforms.Resample (processor.py resample(), compute_cmvn_stats.py:50-53)
+    CmvnStats, scp_segment   <- tools/compute_cmvn_stats.py: global CMVN statistics and its global_cmvn JSON
     load_cmvn, load_kaldi_cmvn <- wekws/utils/cmvn.py
     Pipeline(frontend, model) <- raw PCM -> posteriors in one native call (stream_kws_ctc.py:482-487 composition)
     patch_reference()        -> makes `wekws.model.kws_model` resolve to this implementation
@@ -18,8 +20,9 @@ Public surface mirrors the reference (wenet-e2e/wekws):
     export_onnx()            <- wekws/bin/export_onnx.py: the ONNX file (input, cache -> output, r_cache) for the ORT runtime
 """
 from .cmvn import load_cmvn, load_kaldi_cmvn
+from .cmvn_stats import CmvnStats, scp_segment
 from .configs import MODEL_NAMES, model_config
-from .frontend import Fbank, Mfcc, fbank, mfcc
+from .frontend import Fbank, Mfcc, Resample, fbank, mfcc, resample
 from .kws_model import GlobalCMVN, KWSModel, init_model
 from .ctc import (ctc_keyword_hits, ctc_prefix_beam_search, ctc_state, stream_score_ctc, write_ctc_scores,
                   write_stream_ctc_scores)
@@ -36,5 +39,5 @@ __all__ = ["init_model", "KWSModel", "GlobalCMVN", "Fbank", "fbank", "Mfcc", "mf
            "model_config", "MODEL_NAMES", "patch_reference", "export_native", "export_onnx", "det_stats", "det_curve", "det_thresholds", "context_expansion",
            "Pipeline", "ctc_prefix_beam_search", "ctc_keyword_hits", "ctc_state", "write_ctc_scores",
            "KeywordSpotter", "SpotResult", "stream_score_ctc", "write_stream_ctc_scores", "ctc_det_stats",
-           "write_ctc_det_stats", "space_mixed_label", "criterion"]
+           "write_ctc_det_stats", "space_mixed_label", "criterion", "Resample", "resample", "CmvnStats", "scp_segment"]
 __version__ = "0.1.0"

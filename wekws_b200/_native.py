@@ -19,7 +19,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 
 class FbankConfig(C.Structure):
@@ -102,6 +102,14 @@ SIGNATURES = {
     "wekws_pipeline_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64,
                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_uint32, C.c_void_p]),
+    "wekws_resample_create": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]),
+    "wekws_resample_destroy": (None, [C.c_void_p]),
+    "wekws_resample_output_length": (C.c_int64, [C.c_void_p, C.c_int64]),
+    "wekws_resample_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
+                                         C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    "wekws_cmvn_stats_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int]),
+    "wekws_cmvn_stats_accumulate": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

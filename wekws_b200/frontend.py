@@ -14,6 +14,7 @@ import ctypes as C
 import math
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import _native
@@ -185,6 +186,139 @@ class Mfcc(Fbank):
         _native.check(_native.lib().wekws_fbank_set_mfcc(
             handle, self.num_ceps, C.c_void_p(self.dct.data_ptr()),
             C.c_void_p(self.lifter.data_ptr()) if self.lifter is not None else None), "wekws_fbank_set_mfcc")
+
+
+def sinc_resample_kernel(orig_freq: int, new_freq: int, lowpass_filter_width: int = 6, rolloff: float = 0.99,
+                         resampling_method: str = "sinc_interp_hann"):
+    """torchaudio 2.11 functional `_get_sinc_resample_kernel` with dtype None: the same float64 ops in the same order,
+    then a cast to float32.  Returns the (new / g, 2 width + orig / g) table and width (g = gcd of the rates).
+    Only the Hann window is implemented: it is the only one the reference uses."""
+    if resampling_method != "sinc_interp_hann":
+        raise NotImplementedError(f"resampling_method {resampling_method!r}: only 'sinc_interp_hann' is implemented")
+    if int(orig_freq) != orig_freq or int(new_freq) != new_freq:
+        raise ValueError("resample rates must be integers")
+    if lowpass_filter_width <= 0:
+        raise ValueError("Low pass filter width should be positive.")
+    g = math.gcd(int(orig_freq), int(new_freq))
+    orig, new = int(orig_freq) // g, int(new_freq) // g
+    base_freq = min(orig, new) * rolloff
+    width = math.ceil(lowpass_filter_width * orig / base_freq)
+    if new * (2 * width + orig) > _RESAMPLE_DENSE_MAX:
+        raise ValueError(f"resample {orig_freq} -> {new_freq}: the filter table is {new} x {2 * width + orig} floats; "
+                         f"its non-zero taps (about {new * math.ceil(2 * lowpass_filter_width * orig / base_freq) * 4} "
+                         "bytes) do not fit the kernel's shared memory")
+    idx = torch.arange(-width, width + orig, dtype=torch.float64)[None, None] / orig
+    t = torch.arange(0, -new, -1, dtype=None)[:, None, None] / new + idx
+    t *= base_freq
+    t = t.clamp_(-lowpass_filter_width, lowpass_filter_width)
+    window = torch.cos(t * math.pi / lowpass_filter_width / 2) ** 2
+    t *= math.pi
+    scale = base_freq / orig
+    kernels = torch.where(t == 0, torch.tensor(1.0).to(t), t.sin() / t)
+    kernels *= window * scale
+    return kernels.to(dtype=torch.float32), width
+
+
+_RESAMPLE_DENSE_MAX = 1 << 24        # dense table entries; far past any pair whose compact table fits on chip
+
+
+class Resample:
+    """Batched GPU twin of ``torchaudio.transforms.Resample(orig_freq, new_freq)`` (sinc_interp_hann,
+    lowpass_filter_width 6, rolloff 0.99), as wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py
+    call it.  ``__call__(pcm, lengths=None)``: pcm (B, N) or (N,) int16 / float32 CUDA tensor at int16 scale ->
+    (B, output_length(N)) float32; row b is the resampling of its first lengths[b] samples (the rest count as zeros
+    and are never read), zero-filled past output_length(lengths[b]).  The output is not rounded back to int16:
+    kaldi.fbank receives the float waveform.  Each output is accumulated in double and rounded once to float32."""
+
+    def __init__(self, orig_freq: int, new_freq: int, resampling_method: str = "sinc_interp_hann",
+                 lowpass_filter_width: int = 6, rolloff: float = 0.99):
+        self.orig_freq, self.new_freq = int(orig_freq), int(new_freq)
+        if self.orig_freq <= 0 or self.new_freq <= 0:
+            raise ValueError(f"resample rates must be positive, got {orig_freq} -> {new_freq}")
+        self.gcd = math.gcd(self.orig_freq, self.new_freq)
+        self.kernel, self.width = None, 0
+        if self.orig_freq != self.new_freq:
+            self.kernel, self.width = sinc_resample_kernel(self.orig_freq, self.new_freq, lowpass_filter_width,
+                                                           rolloff, resampling_method)
+            self.kernel = self.kernel.reshape(self.kernel.shape[0], -1).contiguous()
+        self._handles = {}
+
+    def output_length(self, num_samples: int) -> int:
+        """torchaudio's target length ceil(torch.as_tensor(new * n / orig)): the quotient passes through float32, so
+        for very long rows it can be one short of the exact ceiling; n itself when the rates are equal."""
+        if self.orig_freq == self.new_freq:
+            return int(num_samples)
+        o, n = self.orig_freq // self.gcd, self.new_freq // self.gcd
+        if num_samples <= 0:
+            return 0
+        target = math.ceil(float(np.float32(n * int(num_samples) / o)))
+        return min(target, (int(num_samples) // o + 1) * n)
+
+    def _handle(self, dev: torch.device):
+        h = self._handles.get(dev)
+        if h is None:
+            h = C.c_void_p()
+            with torch.cuda.device(dev):
+                _native.check(_native.lib().wekws_resample_create(
+                    self.orig_freq, self.new_freq, C.c_void_p(self.kernel.data_ptr()), self.width, C.byref(h)),
+                    "wekws_resample_create")
+            self._handles[dev] = h
+        return h
+
+    def __del__(self):
+        for h in getattr(self, "_handles", {}).values():
+            try:
+                _native.lib().wekws_resample_destroy(h)
+            except Exception:
+                pass
+
+    def __call__(self, pcm: torch.Tensor, lengths=None) -> torch.Tensor:
+        if self.orig_freq == self.new_freq:
+            return pcm                       # as the transform does
+        if not pcm.is_cuda:
+            raise RuntimeError("wekws_b200.Resample runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
+        squeeze = pcm.dim() == 1
+        if squeeze:
+            pcm = pcm.unsqueeze(0)
+        if pcm.dim() != 2:
+            raise ValueError("pcm must be (N,) or (B, N)")
+        if pcm.dtype == torch.int16:
+            dtype = _native.PCM_S16
+        elif pcm.dtype == torch.float32:
+            dtype = _native.PCM_F32
+        else:
+            raise TypeError(f"pcm must be int16 or float32, got {pcm.dtype}")
+        if pcm.stride(1) != 1:
+            pcm = pcm.contiguous()
+        dev = pcm.device
+        B, N = pcm.shape
+        max_out = self.output_length(N)
+        out = torch.empty(B, max_out, device=dev, dtype=torch.float32)
+        lens = None
+        if lengths is not None:
+            lens = torch.as_tensor(lengths).to(device=dev, dtype=torch.int32).contiguous()
+            if lens.shape != (B,):
+                raise ValueError(f"lengths must have shape ({B},), got {tuple(lens.shape)}")
+        if B > 0 and max_out > 0:
+            h = self._handle(dev)
+            with torch.cuda.device(dev):
+                stream = torch.cuda.current_stream(dev).cuda_stream
+                rc = _native.lib().wekws_resample_forward(
+                    h, C.c_void_p(pcm.data_ptr()), dtype, B, N, pcm.stride(0),
+                    C.c_void_p(lens.data_ptr()) if lens is not None else None, C.c_void_p(out.data_ptr()),
+                    out.stride(0), max_out, C.c_void_p(stream))
+            _native.check(rc, "wekws_resample_forward")
+        return out[0] if squeeze else out
+
+
+def resample(waveform: torch.Tensor, orig_freq: int, new_freq: int) -> torch.Tensor:
+    """Functional form: the waveform unchanged when the rates are equal (as the transform does), else
+    Resample(orig_freq, new_freq)(waveform) with the handle cached per rate pair."""
+    key = ("resample", int(orig_freq), int(new_freq))
+    rs = _DEFAULT.get(key)
+    if rs is None:
+        rs = _DEFAULT[key] = Resample(orig_freq, new_freq)
+    return rs(waveform)
 
 
 _DEFAULT = {}
