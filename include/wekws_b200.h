@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 9   /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_* */
+#define WEKWS_B200_ABI_VERSION 10  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -135,6 +135,27 @@ WEKWS_API int wekws_fbank_forward(wekws_fbank* fb, const void* d_pcm, int pcm_dt
                         int64_t num_samples, int64_t pcm_stride, const int32_t* d_lens,
                         const float* d_mean, const float* d_istd, float* d_out,
                         int64_t max_frames, void* stream);
+
+/* Training front-end (the dither of kaldi.fbank / kaldi.mfcc as wekws/dataset/processor.py compute_fbank /
+ * compute_mfcc pass it): wekws_fbank_forward with Gaussian noise of standard deviation `dither` added to every
+ * frame after framing, before DC removal, pre-emphasis and the window (torchaudio kaldi.py _get_window).  The
+ * noise is not torch.randn's but a pure function of (seed, row b, frame f, sample j): normals from
+ * Philox4x32-10 (Random123 constants) with counter (j / 4, f, b, 0) and key (seed lo, seed hi), two Box-Muller
+ * pairs per call, u = ((word >> 8) + 0.5) 2^-24, r = sqrt(-2 ln u_a), (r cos 2 pi u_b, r sin 2 pi u_b); each
+ * within 1e-6 of the float64 formula.  Log-mel or MFCC by the handle's mode.  One launch.
+ * wekws_dither_noise (test hook) writes those normals, d_out (B, frames, frame_length) floats, 16-byte aligned. */
+WEKWS_API int wekws_fbank_forward_dither(wekws_fbank* fb, const void* d_pcm, int pcm_dtype, int64_t B,
+                                         int64_t num_samples, int64_t pcm_stride, const int32_t* d_lens,
+                                         const float* d_mean, const float* d_istd, float* d_out,
+                                         int64_t max_frames, float dither, uint64_t seed, void* stream);
+WEKWS_API int wekws_dither_noise(uint64_t seed, int64_t B, int64_t frames, float* d_out, void* stream);
+
+/* SpecAugment (wekws/dataset/processor.py spec_aug) on d_feats (B, T, D) in place: for row b, frames t <
+ * d_frames[b] that fall in one of its num_t_mask frame ranges, and every column of those frames in one of its
+ * num_f_mask column ranges, are set to 0.  d_masks: per row, num_t_mask (start, end) frame pairs then num_f_mask
+ * (start, end) column pairs, ends exclusive.  No other element is read or written.  One launch.                */
+WEKWS_API int wekws_spec_aug(float* d_feats, const int32_t* d_frames, int64_t B, int64_t T, int D,
+                             const int32_t* d_masks, int num_t_mask, int num_f_mask, void* stream);
 
 /* ----------------------------------------------------------------------------- model */
 typedef struct wekws_model wekws_model;

@@ -16,6 +16,8 @@ Public surface mirrors the reference (wenet-e2e/wekws):
     ctc_det_stats, write_ctc_det_stats <- wekws/bin/compute_det_ctc.py: DET statistics of a CTC score file
     criterion                <- wekws/model/loss.py criterion(): held-out loss / accuracy (max_pooling, ce, ctc)
     context_expansion        <- wekws/dataset/processor.py context_expansion + frame_skip (FSMN / CTC recipes)
+    TrainFeatures, spec_aug  <- the training data chain of wekws/dataset/dataset.py / init_dataset.py: dithered
+                                Fbank / MFCC, SpecAugment, context expansion, frame skip and padding() on the device
     export_native()          -> weight file for the C++ runtime shim (the role of wekws/bin/export_onnx.py)
     export_onnx()            <- wekws/bin/export_onnx.py: the ONNX file (input, cache -> output, r_cache) for the ORT runtime
 """
@@ -34,10 +36,12 @@ from .pipeline import Pipeline
 from .postproc import (context_expansion, ctc_det_stats, det_curve, det_stats, det_thresholds, space_mixed_label,
                        write_ctc_det_stats)
 from .spotter import KeywordSpotter, SpotResult
+from .train_features import TrainFeatures, spec_aug
 
 __all__ = ["init_model", "KWSModel", "GlobalCMVN", "Fbank", "fbank", "Mfcc", "mfcc", "load_cmvn", "load_kaldi_cmvn",
            "model_config", "MODEL_NAMES", "patch_reference", "export_native", "export_onnx", "det_stats", "det_curve", "det_thresholds", "context_expansion",
            "Pipeline", "ctc_prefix_beam_search", "ctc_keyword_hits", "ctc_state", "write_ctc_scores",
            "KeywordSpotter", "SpotResult", "stream_score_ctc", "write_stream_ctc_scores", "ctc_det_stats",
-           "write_ctc_det_stats", "space_mixed_label", "criterion", "Resample", "resample", "CmvnStats", "scp_segment"]
+           "write_ctc_det_stats", "space_mixed_label", "criterion", "Resample", "resample", "CmvnStats", "scp_segment",
+           "TrainFeatures", "spec_aug"]
 __version__ = "0.1.0"

@@ -110,8 +110,17 @@ __device__ __forceinline__ float log_floored(float e, float floor_v, float log_o
 // MFCC = true adds the cepstral epilogue: the log-mel rows of the warp's FB_FPW frames stay in registers
 // (lane owns bins lane + 32 k) and are multiplied with the DCT matrix together, so every matrix element is
 // loaded once per FB_FPW frames and 12-16 accumulators run in parallel.
-template <typename PCM, bool MFCC>
-__global__ void __launch_bounds__(FB_NT, MFCC ? 2 : 3) fbank_kernel(const FbankArgs a, const __grid_constant__ MelTable mt) {
+// Training front-end (DITHER, wekws_fbank_forward_dither): Gaussian dither noise enters each frame as it is read from
+// the PCM stage (fbcore::frame_power_spectrum, dither.cuh).  Its own parameter block comes after the mel table, so the
+// parameter layout, and the code, of the undithered instantiations is what it was before the dithered ones existed.
+struct DitherArgs {
+  float scale;              // the `dither` of kaldi.fbank
+  uint32_t key0, key1;      // 64-bit seed (lo, hi)
+};
+
+template <typename PCM, bool MFCC, bool DITHER>
+__global__ void __launch_bounds__(FB_NT, (MFCC || DITHER) ? 2 : 3)
+fbank_kernel(const FbankArgs a, const __grid_constant__ MelTable mt, const DitherArgs dz) {
   extern __shared__ __align__(16) float fb_smem[];
   float* s_stage = fb_smem;                                              // [STAGE]
   float2* s_ex = reinterpret_cast<float2*>(s_stage + STAGE);              // [FB_WARPS][E_SZ] exchange buffers
@@ -222,8 +231,8 @@ __global__ void __launch_bounds__(FB_NT, MFCC ? 2 : 3) fbank_kernel(const FbankA
       for (int fi = 0; fi < FB_FPW; ++fi) {
         const int fl = warp + FB_WARPS * fi;
         if (f0 + fl < mb) {
-          fbcore::frame_power_spectrum(s_stage + fl * SHIFT, s_win, s_tw512, tw, E, s_pow + fl * P_ST, a.preemph,
-                                       a.remove_dc, lane);
+          fbcore::frame_power_spectrum<DITHER>(s_stage + fl * SHIFT, s_win, s_tw512, tw, E, s_pow + fl * P_ST,
+                                               a.preemph, a.remove_dc, lane, dz.scale, dz.key0, dz.key1, b, f0 + fl);
         }
       }
       __syncthreads();                              // spectra complete; the PCM stage is dead and becomes the output tile
@@ -291,7 +300,8 @@ __global__ void __launch_bounds__(FB_NT, MFCC ? 2 : 3) fbank_kernel(const FbankA
       continue;
     }
 
-    fbcore::frame_power_spectrum(s_stage + fl * SHIFT, s_win, s_tw512, tw, E, Br, a.preemph, a.remove_dc, lane);
+    fbcore::frame_power_spectrum<DITHER>(s_stage + fl * SHIFT, s_win, s_tw512, tw, E, Br, a.preemph, a.remove_dc, lane,
+                                         dz.scale, dz.key0, dz.key1, b, f);
     __syncwarp();
     // ---- mel projection (sparse rows), log floor ----
     {
@@ -484,10 +494,10 @@ extern "C" int wekws_fbank_set_mfcc(wekws_fbank* fb, int num_ceps, const float* 
   return WEKWS_OK;
 }
 
-extern "C" int wekws_fbank_forward(wekws_fbank* fb, const void* d_pcm, int pcm_dtype, int64_t B,
-                                   int64_t num_samples, int64_t pcm_stride, const int32_t* d_lens,
-                                   const float* d_mean, const float* d_istd, float* d_out,
-                                   int64_t max_frames, void* stream) {
+// dz == nullptr: the undithered kernels; else the dithered ones with *dz
+static int fbank_launch(wekws_fbank* fb, const void* d_pcm, int pcm_dtype, int64_t B, int64_t num_samples,
+                        int64_t pcm_stride, const int32_t* d_lens, const float* d_mean, const float* d_istd, float* d_out,
+                        int64_t max_frames, void* stream, const DitherArgs* dz) {
   WEKWS_REQUIRE(fb && d_out, "wekws_fbank_forward: null handle or output");
   WEKWS_REQUIRE(B >= 0 && num_samples >= 0 && max_frames >= 0, "wekws_fbank_forward: negative size");
   WEKWS_REQUIRE(pcm_dtype == WEKWS_PCM_S16 || pcm_dtype == WEKWS_PCM_F32, "wekws_fbank_forward: bad pcm_dtype %d", pcm_dtype);
@@ -520,11 +530,15 @@ extern "C" int wekws_fbank_forward(wekws_fbank* fb, const void* d_pcm, int pcm_d
   WEKWS_CUDA_OK(cudaGetDevice(&dev));
   WEKWS_REQUIRE(dev == fb->device, "fbank handle was created on device %d but the current device is %d", fb->device, dev);
   WEKWS_REQUIRE(dev >= 0 && dev < 64, "fbank: device index %d out of range", dev);
-  static int occ_dev[64][4] = {};        // the shared-memory attribute and the occupancy are per device
+  static int occ_dev[64][8] = {};        // the shared-memory attribute and the occupancy are per device
   int* occ = occ_dev[dev];
-  const int ti = (pcm_dtype == WEKWS_PCM_S16 ? 0 : 1) + (mf ? 2 : 0);
-  const void* kern = ti == 0 ? (const void*)fbank_kernel<int16_t, false> : ti == 1 ? (const void*)fbank_kernel<float, false>
-                   : ti == 2 ? (const void*)fbank_kernel<int16_t, true> : (const void*)fbank_kernel<float, true>;
+  const int ti = (pcm_dtype == WEKWS_PCM_S16 ? 0 : 1) + (mf ? 2 : 0) + (dz ? 4 : 0);
+  static const void* const kernels[8] = {
+      (const void*)fbank_kernel<int16_t, false, false>, (const void*)fbank_kernel<float, false, false>,
+      (const void*)fbank_kernel<int16_t, true, false>,  (const void*)fbank_kernel<float, true, false>,
+      (const void*)fbank_kernel<int16_t, false, true>,  (const void*)fbank_kernel<float, false, true>,
+      (const void*)fbank_kernel<int16_t, true, true>,   (const void*)fbank_kernel<float, true, true>};
+  const void* kern = kernels[ti];
   if (occ[ti] == 0) {
     WEKWS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     WEKWS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[ti], kern, FB_NT, smem));
@@ -533,11 +547,61 @@ extern "C" int wekws_fbank_forward(wekws_fbank* fb, const void* d_pcm, int pcm_d
   const long long cap = (long long)device_sm_count() * occ[ti];
   const int grid = (int)(items < cap ? items : cap);
   cudaStream_t st = (cudaStream_t)stream;
+  const DitherArgs d = dz ? *dz : DitherArgs{0.f, 0u, 0u};
   switch (ti) {
-    case 0: fbank_kernel<int16_t, false><<<grid, FB_NT, smem, st>>>(a, fb->mt); break;
-    case 1: fbank_kernel<float, false><<<grid, FB_NT, smem, st>>>(a, fb->mt); break;
-    case 2: fbank_kernel<int16_t, true><<<grid, FB_NT, smem, st>>>(a, fb->mt); break;
-    default: fbank_kernel<float, true><<<grid, FB_NT, smem, st>>>(a, fb->mt); break;
+    case 0: fbank_kernel<int16_t, false, false><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
+    case 1: fbank_kernel<float, false, false><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
+    case 2: fbank_kernel<int16_t, true, false><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
+    case 3: fbank_kernel<float, true, false><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
+    case 4: fbank_kernel<int16_t, false, true><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
+    case 5: fbank_kernel<float, false, true><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
+    case 6: fbank_kernel<int16_t, true, true><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
+    default: fbank_kernel<float, true, true><<<grid, FB_NT, smem, st>>>(a, fb->mt, d); break;
   }
-  return check_launch("fbank_kernel");
+  return check_launch(dz ? "fbank_kernel (dither)" : "fbank_kernel");
+}
+
+extern "C" int wekws_fbank_forward(wekws_fbank* fb, const void* d_pcm, int pcm_dtype, int64_t B,
+                                   int64_t num_samples, int64_t pcm_stride, const int32_t* d_lens,
+                                   const float* d_mean, const float* d_istd, float* d_out,
+                                   int64_t max_frames, void* stream) {
+  return fbank_launch(fb, d_pcm, pcm_dtype, B, num_samples, pcm_stride, d_lens, d_mean, d_istd, d_out, max_frames,
+                      stream, nullptr);
+}
+
+extern "C" int wekws_fbank_forward_dither(wekws_fbank* fb, const void* d_pcm, int pcm_dtype, int64_t B,
+                                          int64_t num_samples, int64_t pcm_stride, const int32_t* d_lens,
+                                          const float* d_mean, const float* d_istd, float* d_out, int64_t max_frames,
+                                          float dither, uint64_t seed, void* stream) {
+  WEKWS_REQUIRE(dither == dither && fabsf(dither) <= 3.0e38f, "wekws_fbank_forward_dither: dither must be finite");
+  const DitherArgs dz{dither, (uint32_t)seed, (uint32_t)(seed >> 32)};
+  return fbank_launch(fb, d_pcm, pcm_dtype, B, num_samples, pcm_stride, d_lens, d_mean, d_istd, d_out, max_frames,
+                      stream, &dz);
+}
+
+// Test hook: the exact normals the dithered kernel adds, out[b][f][j] for j < 400 (one thread per Philox call)
+namespace wekws {
+namespace {
+__global__ void dither_noise_kernel(uint32_t k0, uint32_t k1, long long B, int frames, float* out) {
+  const long long calls = B * frames * (WIN / 4);
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < calls; i += (long long)gridDim.x * blockDim.x) {
+    const int q = (int)(i % (WIN / 4));
+    const long long bf = i / (WIN / 4);
+    const int f = (int)(bf % frames), b = (int)(bf / frames);
+    const float2 n0 = dither::normal_pair(k0, k1, b, f, 2 * q), n1 = dither::normal_pair(k0, k1, b, f, 2 * q + 1);
+    reinterpret_cast<float4*>(out)[i] = make_float4(n0.x, n0.y, n1.x, n1.y);
+  }
+}
+}  // namespace
+}  // namespace wekws
+
+extern "C" int wekws_dither_noise(uint64_t seed, int64_t B, int64_t frames, float* d_out, void* stream) {
+  WEKWS_REQUIRE(B >= 0 && frames >= 0 && B < (1ll << 31) && frames < (1ll << 31), "wekws_dither_noise: bad size");
+  if (B == 0 || frames == 0) return WEKWS_OK;
+  WEKWS_REQUIRE(d_out && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0, "wekws_dither_noise: output must be 16-byte aligned");
+  const long long calls = B * frames * (WIN / 4);
+  const int grid = (int)((calls + 255) / 256 < 65536 ? (calls + 255) / 256 : 65536);
+  dither_noise_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((uint32_t)seed, (uint32_t)(seed >> 32), B, (int)frames,
+                                                             d_out);
+  return check_launch("dither_noise_kernel");
 }

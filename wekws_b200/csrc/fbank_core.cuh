@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "dither.cuh"
+
 namespace wekws {
 namespace fbcore {
 
@@ -65,13 +67,44 @@ struct LaneTwiddles {
 // After the last radix-4 pass lane l holds Z[l + 32 i], i < 8, in registers; the untangle needs Z[256 - k]
 // next to Z[k], which is element 7 - i of lane 32 - l (lane 0: its own element (8 - i) & 7) -- 16 shuffles instead
 // of a third trip through shared memory.
+//
+// DITHER (training front-end, dither.cuh): the frame's samples get dither * normal_pair(key, b, f, m) in registers as
+// they are read; the staged PCM, which overlapping frames share, stays undithered.  The DC mean is then taken over the
+// dithered frame, and pre-emphasis needs the dithered sample 2m - 1: it is the odd sample of point m - 1, so it is
+// shuffled over from the lane that owns that point (lane 31 of the previous step for lane 0) rather than recomputed,
+// which would cost lane 0 a second Philox call and Box-Muller pair per step with the other 31 lanes idle.  Both lanes
+// then use the same float, as the reference's single dithered frame does.
+template <bool DITHER = false>
 __device__ __forceinline__ void frame_power_spectrum(const float* __restrict__ s, const float2* __restrict__ s_win,
                                                      const float2* __restrict__ s_tw512h, const LaneTwiddles& tw, float2* E,
-                                                     float* pw, float preemph, int remove_dc, int lane) {
+                                                     float* pw, float preemph, int remove_dc, int lane,
+                                                     float dither = 0.f, uint32_t key0 = 0, uint32_t key1 = 0,
+                                                     int row = 0, int frame = 0) {
   const float* t1r = tw.t1r; const float* t1i = tw.t1i; const float* t2r = tw.t2r; const float* t2i = tw.t2i;
   // ---- window: lane owns packed points m = lane + 32 i (even/odd sample pair 2m, 2m+1) ----
   float xa[7], xb[7], xc[7];
   float sum = 0.f;
+  if constexpr (DITHER) {
+#pragma unroll
+    for (int i = 0; i < 7; ++i) {
+      const int m = lane + 32 * i;
+      if (m < WIN / 2) {
+        const float2 v = *reinterpret_cast<const float2*>(s + 2 * m);
+        const float2 n = dither::normal_pair(key0, key1, row, frame, m);
+        xb[i] = __fadd_rn(v.x, __fmul_rn(n.x, dither));
+        xc[i] = __fadd_rn(v.y, __fmul_rn(n.y, dither));
+        sum += xb[i] + xc[i];
+      } else {
+        xb[i] = xc[i] = 0.f;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 7; ++i) {
+      const float up = __shfl_up_sync(0xffffffffu, xc[i], 1);
+      const float wrap = i > 0 ? __shfl_sync(0xffffffffu, xc[i > 0 ? i - 1 : 0], 31) : xb[0];
+      xa[i] = lane > 0 ? up : wrap;                   // point 0: replicate pad of the dithered x[0] (kaldi.py:195)
+    }
+  } else {
 #pragma unroll
   for (int i = 0; i < 7; ++i) {
     const int m = lane + 32 * i;
@@ -83,6 +116,7 @@ __device__ __forceinline__ void frame_power_spectrum(const float* __restrict__ s
     } else {
       xa[i] = xb[i] = xc[i] = 0.f;
     }
+  }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);

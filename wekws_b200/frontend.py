@@ -122,7 +122,12 @@ class Fbank:
 
     def __call__(self, pcm: torch.Tensor, lengths: Optional[torch.Tensor] = None,
                  mean: Optional[torch.Tensor] = None, istd: Optional[torch.Tensor] = None,
-                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 out: Optional[torch.Tensor] = None, dither: float = 0.0,
+                 generator: Optional[torch.Generator] = None) -> torch.Tensor:
+        """dither != 0: the training front-end of kaldi.fbank(dither=...): Gaussian noise of that standard deviation on
+        every framed sample.  One 64-bit seed is drawn per call from ``generator`` (torch's default CPU generator when
+        None, so torch.manual_seed governs it as it governs the reference's torch.randn); the noise is a documented
+        function of (seed, row, frame, sample) (include/wekws_b200.h), not torch.randn's values."""
         if not pcm.is_cuda:
             raise RuntimeError("wekws_b200.Fbank runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
         squeeze = pcm.dim() == 1
@@ -158,12 +163,22 @@ class Fbank:
             h = self._handle(dev)
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream(dev).cuda_stream
-                rc = _native.lib().wekws_fbank_forward(
-                    h, C.c_void_p(pcm.data_ptr()), dtype, B, N, pcm.stride(0), ptr(lengths, torch.int32),
-                    ptr(mean, torch.float32), ptr(istd, torch.float32), C.c_void_p(out.data_ptr()), m,
-                    C.c_void_p(stream))
+                args = (h, C.c_void_p(pcm.data_ptr()), dtype, B, N, pcm.stride(0), ptr(lengths, torch.int32),
+                        ptr(mean, torch.float32), ptr(istd, torch.float32), C.c_void_p(out.data_ptr()), m)
+                if dither == 0.0:
+                    rc = _native.lib().wekws_fbank_forward(*args, C.c_void_p(stream))
+                else:
+                    rc = _native.lib().wekws_fbank_forward_dither(*args, float(dither), draw_seed(generator),
+                                                                  C.c_void_p(stream))
             _native.check(rc, "wekws_fbank_forward")
         return out[0] if squeeze else out
+
+
+def draw_seed(generator: Optional[torch.Generator] = None) -> int:
+    """One 64-bit dither seed from ``generator`` (torch's default CPU generator when None): two 32-bit draws, low word
+    first."""
+    lo, hi = torch.randint(0, 1 << 32, (2,), dtype=torch.int64, generator=generator).tolist()
+    return lo | (hi << 32)
 
 
 class Mfcc(Fbank):
@@ -328,26 +343,24 @@ def fbank(waveform: torch.Tensor, num_mel_bins: int = 23, frame_length: float = 
           frame_shift: float = 10.0, dither: float = 0.0, energy_floor: float = 0.0,
           sample_frequency: float = 16000.0, window_type: str = "povey") -> torch.Tensor:
     """Signature-compatible subset of torchaudio.compliance.kaldi.fbank for the reference's
-    call sites: waveform (1, N) -> (m, num_mel_bins).  dither must be 0 (test-time setting)."""
-    if dither != 0.0:
-        raise NotImplementedError("wekws_b200.fbank: dither is a training-time augmentation; use dither=0.0")
+    call sites: waveform (1, N) -> (m, num_mel_bins).  A non-zero dither draws its seed from torch's default
+    generator (Fbank.__call__)."""
     key = (num_mel_bins, frame_length, frame_shift, sample_frequency, window_type)
     fb = _DEFAULT.get(key)
     if fb is None:
         fb = _DEFAULT[key] = Fbank(num_mel_bins, frame_length, frame_shift, sample_frequency, window_type)
     if waveform.dim() == 2:
         assert waveform.size(0) == 1, "kaldi.fbank expects a mono (1, N) waveform"
-        return fb(waveform)[0]
-    return fb(waveform)
+        return fb(waveform, dither=dither)[0]
+    return fb(waveform, dither=dither)
 
 
 def mfcc(waveform: torch.Tensor, num_ceps: int = 13, num_mel_bins: int = 23, frame_length: float = 25.0,
          frame_shift: float = 10.0, dither: float = 0.0, energy_floor: float = 0.0,
          sample_frequency: float = 16000.0, cepstral_lifter: float = 22.0, window_type: str = "povey") -> torch.Tensor:
     """Signature-compatible subset of torchaudio.compliance.kaldi.mfcc for the reference's call site
-    (processor.py:157-166): waveform (1, N) -> (m, num_ceps).  dither must be 0 (test-time setting)."""
-    if dither != 0.0:
-        raise NotImplementedError("wekws_b200.mfcc: dither is a training-time augmentation; use dither=0.0")
+    (processor.py:157-166): waveform (1, N) -> (m, num_ceps).  A non-zero dither draws its seed from torch's default
+    generator (Fbank.__call__)."""
     key = ("mfcc", num_ceps, num_mel_bins, frame_length, frame_shift, sample_frequency, cepstral_lifter, window_type)
     fe = _DEFAULT.get(key)
     if fe is None:
@@ -355,5 +368,5 @@ def mfcc(waveform: torch.Tensor, num_ceps: int = 13, num_mel_bins: int = 23, fra
                                   frame_shift=frame_shift, sample_frequency=sample_frequency, window_type=window_type)
     if waveform.dim() == 2:
         assert waveform.size(0) == 1, "kaldi.mfcc expects a mono (1, N) waveform"
-        return fe(waveform)[0]
-    return fe(waveform)
+        return fe(waveform, dither=dither)[0]
+    return fe(waveform, dither=dither)

@@ -1,0 +1,205 @@
+"""Training batches on the device: the data side of stage 2 of the recipes.
+
+In the reference, data-loader workers build each training batch one utterance at a time on the CPU
+(wekws/dataset/dataset.py Dataset(), and wekws/dataset/init_dataset.py on top of wenet's equivalent):
+
+    resample -> compute_fbank / compute_mfcc (dither) -> spec_aug -> context_expansion -> frame_skip -> padding
+
+``TrainFeatures`` runs that chain on a batch of decoded PCM: the resampler (csrc/resample.cu), the dithered Fbank /
+MFCC kernel (csrc/fbank.cu, noise from csrc/dither.cuh), SpecAugment (csrc/spec_aug.cu) and context expansion / frame
+skip (csrc/stream_frontend.cu), then ``padding``'s ordering.  It returns the batch dict ``Executor.train`` reads, with
+the features already on the device.  Deliberate differences from the reference:
+  * the dither noise is not torch.randn's (no device generator can reproduce it) but a documented function of a seed
+    drawn from torch's generator (include/wekws_b200.h), so torch.manual_seed still makes a run reproducible;
+  * ``speed_perturb: true`` is refused: the reference's sox effects are gone from the torchaudio it pins, and no
+    shipped config enables it.  ``reverb_prob`` / ``noise_prob`` are ignored, as Dataset() ignores them without LMDB
+    sources.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import random
+from typing import List, Optional, Sequence
+
+import torch
+
+from . import _native
+from .frontend import Fbank, Mfcc, Resample
+from .postproc import context_expansion
+
+FBANK_RATE = 16000
+
+
+def draw_spec_aug_masks(frames: Sequence[int], dim: int, num_t_mask: int = 2, num_f_mask: int = 2, max_t: int = 50,
+                        max_f: int = 10, rng=random) -> List[List[int]]:
+    """The masks processor.spec_aug draws for each row in turn, with the same ``rng`` calls in the same order:
+    num_t_mask x (randint(0, frames_b - 1), randint(1, max_t)), then num_f_mask x (randint(0, dim - 1),
+    randint(1, max_f)).  Row b -> [t_start, t_end, ..., f_start, f_end, ...] with end = min(limit, start + length).
+    A row with no frames raises ValueError, as the reference's randint(0, -1) does."""
+    out = []
+    for b, n in enumerate(frames):
+        n = int(n)
+        if n <= 0:
+            raise ValueError(f"spec_aug: row {b} has no frames")
+        row = []
+        for _ in range(num_t_mask):
+            start = rng.randint(0, n - 1)
+            length = rng.randint(1, max_t)
+            row += [start, min(n, start + length)]
+        for _ in range(num_f_mask):
+            start = rng.randint(0, dim - 1)
+            length = rng.randint(1, max_f)
+            row += [start, min(dim, start + length)]
+        out.append(row)
+    return out
+
+
+def spec_aug(feats: torch.Tensor, frames: Sequence[int], num_t_mask: int = 2, num_f_mask: int = 2, max_t: int = 50,
+             max_f: int = 10, rng=random) -> torch.Tensor:
+    """processor.spec_aug on a batch, in place: feats (B, T, D) float32 CUDA, row b's first frames[b] (host ints)
+    frames are its utterance.  The masks come from ``rng`` (Python's ``random`` by default) in the reference's order,
+    so with the same random state they are the reference's; one small asynchronous copy sends them up and one launch
+    writes the zeros.  Returns feats."""
+    if not feats.is_cuda:
+        raise RuntimeError("wekws_b200.spec_aug runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
+    if feats.dim() != 3 or feats.dtype != torch.float32 or not feats.is_contiguous():
+        raise ValueError("feats must be a contiguous (B, T, D) float32 tensor")
+    B, T, D = feats.shape
+    frames = [int(n) for n in frames]
+    if len(frames) != B or any(n > T for n in frames):
+        raise ValueError(f"frames must be {B} values of at most {T}")
+    masks = draw_spec_aug_masks(frames, D, num_t_mask, num_f_mask, max_t, max_f, rng)
+    if B == 0 or num_t_mask + num_f_mask == 0:
+        return feats
+    table = torch.tensor(frames + [v for row in masks for v in row], dtype=torch.int32).pin_memory()
+    dev = feats.device
+    with torch.cuda.device(dev):
+        d_table = table.to(dev, non_blocking=True)
+        rc = _native.lib().wekws_spec_aug(
+            C.c_void_p(feats.data_ptr()), C.c_void_p(d_table.data_ptr()), B, T, D,
+            C.c_void_p(d_table.data_ptr() + 4 * B), int(num_t_mask), int(num_f_mask),
+            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    _native.check(rc, "wekws_spec_aug")
+    return feats
+
+
+class TrainFeatures:
+    """The reference's training data chain after decoding, for one batch of PCM at a time.
+
+    ``feat_type`` 'fbank' or 'mfcc'; ``feat_conf`` the keys compute_fbank / compute_mfcc take (num_mel_bins,
+    num_ceps, frame_length, frame_shift, dither; their defaults when absent).  ``spec_aug_conf`` None = no SpecAugment.
+    ``context`` (left, right) or None; ``frame_skip`` >= 1."""
+
+    def __init__(self, feat_type: str = "fbank", feat_conf: Optional[dict] = None, resample_rate: int = FBANK_RATE,
+                 spec_aug_conf: Optional[dict] = None, context=None, frame_skip: int = 1):
+        conf = dict(feat_conf or {})
+        kw = dict(frame_length=float(conf.get("frame_length", 25)), frame_shift=float(conf.get("frame_shift", 10)))
+        if feat_type == "fbank":
+            self.frontend = Fbank(int(conf.get("num_mel_bins", 23)), **kw)
+        elif feat_type == "mfcc":
+            self.frontend = Mfcc(int(conf.get("num_ceps", 80)), int(conf.get("num_mel_bins", 80)), **kw)
+        else:
+            raise ValueError(f"feature type {feat_type!r}: the recipes use 'fbank' or 'mfcc'")
+        if int(resample_rate) != FBANK_RATE:
+            raise NotImplementedError(f"resample_rate {resample_rate}: the Fbank kernel runs at {FBANK_RATE} Hz only")
+        self.feat_type = feat_type
+        self.dither = float(conf.get("dither", 0.0))
+        self.resample_rate = int(resample_rate)
+        self.spec_aug_conf = None if spec_aug_conf is None else dict(spec_aug_conf)
+        self.context = None if context is None else (int(context[0]), int(context[1]))
+        self.frame_skip = int(frame_skip)
+        if self.frame_skip < 1:
+            raise ValueError(f"frame_skip must be >= 1, got {frame_skip}")
+        self._resamplers = {}
+
+    @classmethod
+    def from_config(cls, dataset_conf: dict, split: str = "train") -> "TrainFeatures":
+        """Reads ``dataset_conf`` as the reference's chains do: the live schema (feats_type + fbank_conf / mfcc_conf,
+        init_dataset.py) or the legacy one (feature_extraction_conf with feature_type, dataset.py Dataset());
+        resample_conf (16 kHz when absent, processor.resample's default); spec_aug (on when the key is absent, as in
+        Dataset()) with spec_aug_conf; context_expansion with context_expansion_conf; frame_skip.  split != 'train'
+        applies init_dataset.py's evaluation overrides: no spec_aug and no speed_perturb.  Dither stays on there, as
+        it does in the reference, whose overrides leave the feature config alone."""
+        conf = dict(dataset_conf)
+        if split != "train":
+            conf["speed_perturb"] = False
+            conf["spec_aug"] = False
+        if conf.get("speed_perturb", False):
+            raise NotImplementedError("speed_perturb: the reference's sox speed effect is not available in the "
+                                      "torchaudio it pins, and no shipped config enables it")
+        if "feats_type" in conf:
+            feat_type = conf["feats_type"]
+            feat_conf = conf.get(f"{feat_type}_conf", {})
+        else:
+            feat_conf = dict(conf.get("feature_extraction_conf", {}))
+            feat_type = feat_conf.pop("feature_type", None)
+            if feat_type is None:
+                raise KeyError("dataset_conf has neither feats_type nor feature_extraction_conf.feature_type")
+        resample_rate = conf.get("resample_conf", {}).get("resample_rate", FBANK_RATE)
+        sa = conf.get("spec_aug_conf", {}) if conf.get("spec_aug", True) else None
+        context = None
+        if conf.get("context_expansion", False):
+            cc = conf.get("context_expansion_conf", {})
+            context = (cc.get("left", 1), cc.get("right", 1))
+        return cls(feat_type, feat_conf, resample_rate, sa, context, conf.get("frame_skip", 1))
+
+    def _resampler(self, orig: int) -> Resample:
+        rs = self._resamplers.get(orig)
+        if rs is None:
+            rs = self._resamplers[orig] = Resample(orig, self.resample_rate)
+        return rs
+
+    def __call__(self, pcm: torch.Tensor, lengths: Sequence[int], sample_rate: int, labels, keys,
+                 rng=random, generator: Optional[torch.Generator] = None) -> dict:
+        """pcm (B, N) int16 or float32 CUDA tensor at int16 scale (the reference's waveform * (1 << 15)), row b = its
+        first lengths[b] samples (host ints), all at ``sample_rate``; labels: B ints or B token lists; keys: B
+        strings.  Returns {keys, feats, target, feats_lengths, target_lengths} in padding()'s order (longest first):
+        feats (B, T, D) float32 on pcm's device, the rest host tensors as padding() makes them.  ``rng`` draws the
+        SpecAugment masks, ``generator`` the dither seed."""
+        if not pcm.is_cuda:
+            raise RuntimeError("wekws_b200.TrainFeatures runs on CUDA (sm_90a) only; got a CPU tensor")
+        if pcm.dim() != 2:
+            raise ValueError("pcm must be (B, N)")
+        B, N = pcm.shape
+        lens = [int(n) for n in (lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)]
+        if len(lens) != B or any(n < 0 or n > N for n in lens) or len(labels) != B or len(keys) != B:
+            raise ValueError(f"lengths, labels and keys must have {B} entries, lengths in 0..{N}")
+        dev = pcm.device
+        wave = pcm
+        if int(sample_rate) != self.resample_rate:
+            rs = self._resampler(int(sample_rate))
+            wave = rs(pcm, torch.tensor(lens, dtype=torch.int32).to(dev))
+            lens = [rs.output_length(n) for n in lens]
+        fe = self.frontend
+        frames = [fe.num_frames(n) for n in lens]
+        wave = wave[:, :max(lens, default=0)]
+        feats = fe(wave, lengths=torch.tensor(lens, dtype=torch.int32).to(dev), dither=self.dither,
+                   generator=generator)
+        if self.spec_aug_conf is not None:
+            spec_aug(feats, frames, rng=rng, **self.spec_aug_conf)
+        feat_lens = torch.tensor(frames, dtype=torch.int32)
+        if self.context is not None or self.frame_skip > 1:
+            left, right = self.context or (0, 0)
+            feats, feat_lens = context_expansion(feats, left, right, self.frame_skip, feat_lens)
+        order, batch = padding_order(feat_lens, labels, keys)
+        T = int(batch["feats_lengths"][0]) if B else 0
+        batch["feats"] = feats.index_select(0, order.to(dev))[:, :T].contiguous()
+        return batch
+
+
+def padding_order(feat_lens: torch.Tensor, labels, keys):
+    """The host half of processor.padding(): order = torch.argsort(feat_lens, descending=True) (the same sort as the
+    reference, ties included), and the batch dict without feats: keys and labels in that order, int labels as a (B,)
+    int32 tensor with lengths 1, token lists padded with -1.  Returns (order, dict)."""
+    order = torch.argsort(feat_lens, descending=True)
+    idx = order.tolist()
+    if idx and isinstance(labels[0], int):
+        target = torch.tensor([labels[i] for i in idx], dtype=torch.int32)
+        target_lens = torch.ones(len(idx), dtype=torch.int32)
+    else:
+        seqs = [torch.tensor(labels[i], dtype=torch.int32) for i in idx]
+        target_lens = torch.tensor([len(s) for s in seqs], dtype=torch.int32)
+        target = (torch.nn.utils.rnn.pad_sequence(seqs, batch_first=True, padding_value=-1) if seqs
+                  else torch.zeros(0, 0, dtype=torch.int32))
+    return order, {"keys": [keys[i] for i in idx], "feats": None, "target": target,
+                   "feats_lengths": feat_lens[order], "target_lengths": target_lens}
