@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 10  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug */
+#define WEKWS_B200_ABI_VERSION 11  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -156,6 +156,28 @@ WEKWS_API int wekws_dither_noise(uint64_t seed, int64_t B, int64_t frames, float
  * (start, end) column pairs, ends exclusive.  No other element is read or written.  One launch.                */
 WEKWS_API int wekws_spec_aug(float* d_feats, const int32_t* d_frames, int64_t B, int64_t T, int D,
                              const int32_t* d_masks, int num_t_mask, int num_f_mask, void* stream);
+
+/* Training-audio augmentation (wekws/dataset/processor.py add_reverb / add_noise).  d_pcm as wekws_fbank_forward
+ * (int16 or float32 at int16 scale, row b at b * pcm_stride elements), num_samples per row.  d_rows: (B, 3) int32 on
+ * the device, per row (length n_b, offset, count); count 0 = the row is not augmented.  Every sample outside the
+ * augmented span [0, n_b) of an augmented row, and every sample of the other rows, is the input converted to float32
+ * (exact).  One launch each.
+ * wekws_reverb: (offset, count) = the row's RIR, d_rir[offset .. offset + count), all count taps (count > 0, not all
+ * zero).  d_out[b][i] = sum_{k <= min(i, count - 1)} h[k] x[i - k] for i < n_b, h = rir / sqrt(sum rir^2): the sum of
+ * squares in double in a fixed order, the convolution with FP64 FMAs, rounded once to float32 (within 1 ulp of the
+ * float64 evaluation).  A RIR longer than the row costs no more than the row.  d_out (out_stride floats per row) must
+ * not overlap d_pcm.
+ * wekws_add_noise: (offset, count) = the noise segment s = d_noise[offset .. offset + count); the row adds
+ * s[i mod count] for i < n_b (count = n_b for a segment cut from a longer clip, the whole clip otherwise, repeated as
+ * np.resize does).  gain = 2^15 sqrt(10^((audio_db - noise_db - d_snr[b]) / 10)), audio_db = 10 log10(mean((x
+ * 2^-15)^2) + 1e-4), noise_db = 10 log10(mean(s^2) + 1e-4) over the n_b samples added, in double with a fixed
+ * summation order, rounded once to float32; d_out[b][i] = x[i] + gain * s[i mod count] as one float32 multiply and
+ * one float32 add.  d_out may be d_pcm when the input is float32 with out_stride == pcm_stride.                  */
+WEKWS_API int wekws_reverb(const void* d_pcm, int pcm_dtype, int64_t B, int64_t num_samples, int64_t pcm_stride,
+                           const int32_t* d_rows, const float* d_rir, float* d_out, int64_t out_stride, void* stream);
+WEKWS_API int wekws_add_noise(const void* d_pcm, int pcm_dtype, int64_t B, int64_t num_samples, int64_t pcm_stride,
+                              const int32_t* d_rows, const double* d_snr, const float* d_noise, float* d_out,
+                              int64_t out_stride, void* stream);
 
 /* ----------------------------------------------------------------------------- model */
 typedef struct wekws_model wekws_model;

@@ -18,9 +18,12 @@ Public surface mirrors the reference (wenet-e2e/wekws):
     context_expansion        <- wekws/dataset/processor.py context_expansion + frame_skip (FSMN / CTC recipes)
     TrainFeatures, spec_aug  <- the training data chain of wekws/dataset/dataset.py / init_dataset.py: dithered
                                 Fbank / MFCC, SpecAugment, context expansion, frame skip and padding() on the device
+    AugmentSource, reverb, add_noise <- processor.py add_reverb / add_noise with their LMDB sources: room
+                                reverberation and additive noise of the training audio on the device
     export_native()          -> weight file for the C++ runtime shim (the role of wekws/bin/export_onnx.py)
     export_onnx()            <- wekws/bin/export_onnx.py: the ONNX file (input, cache -> output, r_cache) for the ORT runtime
 """
+from .augment import AugmentSource, add_noise, reverb
 from .cmvn import load_cmvn, load_kaldi_cmvn
 from .cmvn_stats import CmvnStats, scp_segment
 from .configs import MODEL_NAMES, model_config
@@ -43,5 +46,5 @@ __all__ = ["init_model", "KWSModel", "GlobalCMVN", "Fbank", "fbank", "Mfcc", "mf
            "Pipeline", "ctc_prefix_beam_search", "ctc_keyword_hits", "ctc_state", "write_ctc_scores",
            "KeywordSpotter", "SpotResult", "stream_score_ctc", "write_stream_ctc_scores", "ctc_det_stats",
            "write_ctc_det_stats", "space_mixed_label", "criterion", "Resample", "resample", "CmvnStats", "scp_segment",
-           "TrainFeatures", "spec_aug"]
+           "TrainFeatures", "spec_aug", "AugmentSource", "reverb", "add_noise"]
 __version__ = "0.1.0"

@@ -19,7 +19,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 
 class FbankConfig(C.Structure):
@@ -56,6 +56,10 @@ SIGNATURES = {
     "wekws_dither_noise": (C.c_int, [C.c_uint64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
     "wekws_spec_aug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                  C.c_void_p]),
+    "wekws_reverb": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_int64, C.c_void_p]),
+    "wekws_add_noise": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "wekws_model_create": (C.c_int, [C.POINTER(ModelConfig), C.POINTER(C.c_void_p)]),
     "wekws_model_destroy": (None, [C.c_void_p]),
     "wekws_model_padding": (C.c_int, [C.c_void_p]),

@@ -3,17 +3,18 @@
 In the reference, data-loader workers build each training batch one utterance at a time on the CPU
 (wekws/dataset/dataset.py Dataset(), and wekws/dataset/init_dataset.py on top of wenet's equivalent):
 
-    resample -> compute_fbank / compute_mfcc (dither) -> spec_aug -> context_expansion -> frame_skip -> padding
+    resample -> [add_reverb -> add_noise] -> compute_fbank / compute_mfcc (dither) -> spec_aug -> context_expansion
+    -> frame_skip -> padding
 
-``TrainFeatures`` runs that chain on a batch of decoded PCM: the resampler (csrc/resample.cu), the dithered Fbank /
+``TrainFeatures`` runs that chain on a batch of decoded PCM: the resampler (csrc/resample.cu), reverberation and
+additive noise when it is given their sources (csrc/augment.cu, wekws_b200/augment.py), the dithered Fbank /
 MFCC kernel (csrc/fbank.cu, noise from csrc/dither.cuh), SpecAugment (csrc/spec_aug.cu) and context expansion / frame
 skip (csrc/stream_frontend.cu), then ``padding``'s ordering.  It returns the batch dict ``Executor.train`` reads, with
 the features already on the device.  Deliberate differences from the reference:
   * the dither noise is not torch.randn's (no device generator can reproduce it) but a documented function of a seed
     drawn from torch's generator (include/wekws_b200.h), so torch.manual_seed still makes a run reproducible;
   * ``speed_perturb: true`` is refused: the reference's sox effects are gone from the torchaudio it pins, and no
-    shipped config enables it.  ``reverb_prob`` / ``noise_prob`` are ignored, as Dataset() ignores them without LMDB
-    sources.
+    shipped config enables it.
 """
 from __future__ import annotations
 
@@ -24,6 +25,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _native
+from .augment import AugmentSource, draw_noise, draw_reverb, launch_noise, launch_reverb
 from .frontend import Fbank, Mfcc, Resample
 from .postproc import context_expansion
 
@@ -36,21 +38,25 @@ def draw_spec_aug_masks(frames: Sequence[int], dim: int, num_t_mask: int = 2, nu
     num_t_mask x (randint(0, frames_b - 1), randint(1, max_t)), then num_f_mask x (randint(0, dim - 1),
     randint(1, max_f)).  Row b -> [t_start, t_end, ..., f_start, f_end, ...] with end = min(limit, start + length).
     A row with no frames raises ValueError, as the reference's randint(0, -1) does."""
+    return [draw_spec_aug_row(n, dim, num_t_mask, num_f_mask, max_t, max_f, rng, b) for b, n in enumerate(frames)]
+
+
+def draw_spec_aug_row(n: int, dim: int, num_t_mask: int = 2, num_f_mask: int = 2, max_t: int = 50, max_f: int = 10,
+                      rng=random, row: int = 0) -> List[int]:
+    """The masks processor.spec_aug draws for one utterance of n frames (row ``row`` of its batch, for the error
+    message): one row of draw_spec_aug_masks."""
+    n = int(n)
+    if n <= 0:
+        raise ValueError(f"spec_aug: row {row} has no frames")
     out = []
-    for b, n in enumerate(frames):
-        n = int(n)
-        if n <= 0:
-            raise ValueError(f"spec_aug: row {b} has no frames")
-        row = []
-        for _ in range(num_t_mask):
-            start = rng.randint(0, n - 1)
-            length = rng.randint(1, max_t)
-            row += [start, min(n, start + length)]
-        for _ in range(num_f_mask):
-            start = rng.randint(0, dim - 1)
-            length = rng.randint(1, max_f)
-            row += [start, min(dim, start + length)]
-        out.append(row)
+    for _ in range(num_t_mask):
+        start = rng.randint(0, n - 1)
+        length = rng.randint(1, max_t)
+        out += [start, min(n, start + length)]
+    for _ in range(num_f_mask):
+        start = rng.randint(0, dim - 1)
+        length = rng.randint(1, max_f)
+        out += [start, min(dim, start + length)]
     return out
 
 
@@ -69,6 +75,12 @@ def spec_aug(feats: torch.Tensor, frames: Sequence[int], num_t_mask: int = 2, nu
     if len(frames) != B or any(n > T for n in frames):
         raise ValueError(f"frames must be {B} values of at most {T}")
     masks = draw_spec_aug_masks(frames, D, num_t_mask, num_f_mask, max_t, max_f, rng)
+    return _apply_spec_aug(feats, frames, masks, num_t_mask, num_f_mask)
+
+
+def _apply_spec_aug(feats: torch.Tensor, frames: List[int], masks: List[List[int]], num_t_mask: int,
+                    num_f_mask: int) -> torch.Tensor:
+    B, T, D = feats.shape
     if B == 0 or num_t_mask + num_f_mask == 0:
         return feats
     table = torch.tensor(frames + [v for row in masks for v in row], dtype=torch.int32).pin_memory()
@@ -88,10 +100,14 @@ class TrainFeatures:
 
     ``feat_type`` 'fbank' or 'mfcc'; ``feat_conf`` the keys compute_fbank / compute_mfcc take (num_mel_bins,
     num_ceps, frame_length, frame_shift, dither; their defaults when absent).  ``spec_aug_conf`` None = no SpecAugment.
-    ``context`` (left, right) or None; ``frame_skip`` >= 1."""
+    ``context`` (left, right) or None; ``frame_skip`` >= 1.  ``reverb_source`` / ``noise_source``: AugmentSource
+    banks (Dataset()'s reverb_lmdb / noise_lmdb), applied after resampling with ``reverb_prob`` / ``noise_prob``; a
+    stage runs only when its source is given and its probability is above 0, as Dataset() adds it."""
 
     def __init__(self, feat_type: str = "fbank", feat_conf: Optional[dict] = None, resample_rate: int = FBANK_RATE,
-                 spec_aug_conf: Optional[dict] = None, context=None, frame_skip: int = 1):
+                 spec_aug_conf: Optional[dict] = None, context=None, frame_skip: int = 1,
+                 reverb_source: Optional[AugmentSource] = None, reverb_prob: float = 0.0,
+                 noise_source: Optional[AugmentSource] = None, noise_prob: float = 0.0):
         conf = dict(feat_conf or {})
         kw = dict(frame_length=float(conf.get("frame_length", 25)), frame_shift=float(conf.get("frame_shift", 10)))
         if feat_type == "fbank":
@@ -110,20 +126,28 @@ class TrainFeatures:
         self.frame_skip = int(frame_skip)
         if self.frame_skip < 1:
             raise ValueError(f"frame_skip must be >= 1, got {frame_skip}")
+        self.reverb_source = reverb_source if reverb_source is not None and float(reverb_prob) > 0 else None
+        self.reverb_prob = float(reverb_prob)
+        self.noise_source = noise_source if noise_source is not None and float(noise_prob) > 0 else None
+        self.noise_prob = float(noise_prob)
         self._resamplers = {}
 
     @classmethod
-    def from_config(cls, dataset_conf: dict, split: str = "train") -> "TrainFeatures":
+    def from_config(cls, dataset_conf: dict, split: str = "train", reverb_source: Optional[AugmentSource] = None,
+                    noise_source: Optional[AugmentSource] = None) -> "TrainFeatures":
         """Reads ``dataset_conf`` as the reference's chains do: the live schema (feats_type + fbank_conf / mfcc_conf,
         init_dataset.py) or the legacy one (feature_extraction_conf with feature_type, dataset.py Dataset());
         resample_conf (16 kHz when absent, processor.resample's default); spec_aug (on when the key is absent, as in
         Dataset()) with spec_aug_conf; context_expansion with context_expansion_conf; frame_skip.  split != 'train'
         applies init_dataset.py's evaluation overrides: no spec_aug and no speed_perturb.  Dither stays on there, as
-        it does in the reference, whose overrides leave the feature config alone."""
+        it does in the reference, whose overrides leave the feature config alone.  ``reverb_source`` /
+        ``noise_source`` take effect with reverb_prob / noise_prob (0 when absent) in the 'train' split only: the
+        held-out sets of the recipes are built without the LMDB sources."""
         conf = dict(dataset_conf)
         if split != "train":
             conf["speed_perturb"] = False
             conf["spec_aug"] = False
+            reverb_source = noise_source = None
         if conf.get("speed_perturb", False):
             raise NotImplementedError("speed_perturb: the reference's sox speed effect is not available in the "
                                       "torchaudio it pins, and no shipped config enables it")
@@ -141,7 +165,24 @@ class TrainFeatures:
         if conf.get("context_expansion", False):
             cc = conf.get("context_expansion_conf", {})
             context = (cc.get("left", 1), cc.get("right", 1))
-        return cls(feat_type, feat_conf, resample_rate, sa, context, conf.get("frame_skip", 1))
+        return cls(feat_type, feat_conf, resample_rate, sa, context, conf.get("frame_skip", 1),
+                   reverb_source, conf.get("reverb_prob", 0.0), noise_source, conf.get("noise_prob", 0.0))
+
+    def draw(self, lengths: Sequence[int], rng=random) -> dict:
+        """The host draws of a batch whose rows have ``lengths`` samples at resample_rate, made utterance by utterance
+        as the reference's lazy processors make them: row b's add_reverb draws, then its add_noise draws, then its
+        SpecAugment masks, before row b + 1 draws anything.  Returns {'reverb': B clip indices or None, 'noise': B
+        (index, start or None, snr) or None, 'masks': B mask rows (empty lists without SpecAugment)}."""
+        fe, sa = self.frontend, self.spec_aug_conf
+        out = {"reverb": [], "noise": [], "masks": []}
+        for b, n in enumerate(int(v) for v in lengths):
+            out["reverb"].append(None if self.reverb_source is None
+                                 else draw_reverb(n, self.reverb_source, self.reverb_prob, rng, b))
+            out["noise"].append(None if self.noise_source is None
+                                else draw_noise(n, self.noise_source, self.noise_prob, rng))
+            out["masks"].append([] if sa is None
+                                else draw_spec_aug_row(fe.num_frames(n), fe.feature_dim, rng=rng, row=b, **sa))
+        return out
 
     def _resampler(self, orig: int) -> Resample:
         rs = self._resamplers.get(orig)
@@ -154,8 +195,8 @@ class TrainFeatures:
         """pcm (B, N) int16 or float32 CUDA tensor at int16 scale (the reference's waveform * (1 << 15)), row b = its
         first lengths[b] samples (host ints), all at ``sample_rate``; labels: B ints or B token lists; keys: B
         strings.  Returns {keys, feats, target, feats_lengths, target_lengths} in padding()'s order (longest first):
-        feats (B, T, D) float32 on pcm's device, the rest host tensors as padding() makes them.  ``rng`` draws the
-        SpecAugment masks, ``generator`` the dither seed."""
+        feats (B, T, D) float32 on pcm's device, the rest host tensors as padding() makes them.  ``rng`` makes the
+        augmentation draws and the SpecAugment masks (see ``draw``), ``generator`` the dither seed."""
         if not pcm.is_cuda:
             raise RuntimeError("wekws_b200.TrainFeatures runs on CUDA (sm_90a) only; got a CPU tensor")
         if pcm.dim() != 2:
@@ -173,10 +214,25 @@ class TrainFeatures:
         fe = self.frontend
         frames = [fe.num_frames(n) for n in lens]
         wave = wave[:, :max(lens, default=0)]
+        draws = None
+        if self.reverb_source is not None or self.noise_source is not None:
+            draws = self.draw(lens, rng)
+            owned = int(sample_rate) != self.resample_rate          # wave is the resampler's buffer, not the caller's
+            if wave.stride(1) != 1:
+                wave, owned = wave.contiguous(), True
+            if any(p is not None for p in draws["reverb"]):
+                wave, owned = launch_reverb(wave, lens, draws["reverb"], self.reverb_source), True
+            if any(p is not None for p in draws["noise"]):
+                wave = launch_noise(wave, lens, draws["noise"], self.noise_source,
+                                    out=wave if owned and wave.dtype == torch.float32 else None)
         feats = fe(wave, lengths=torch.tensor(lens, dtype=torch.int32).to(dev), dither=self.dither,
                    generator=generator)
         if self.spec_aug_conf is not None:
-            spec_aug(feats, frames, rng=rng, **self.spec_aug_conf)
+            if draws is None:
+                spec_aug(feats, frames, rng=rng, **self.spec_aug_conf)
+            else:
+                sa = self.spec_aug_conf
+                _apply_spec_aug(feats, frames, draws["masks"], sa.get("num_t_mask", 2), sa.get("num_f_mask", 2))
         feat_lens = torch.tensor(frames, dtype=torch.int32)
         if self.context is not None or self.frame_skip > 1:
             left, right = self.context or (0, 0)
