@@ -1,6 +1,7 @@
 """Round-2 parity cases (VERDICT r01 "What's weak" 1-4, ADVICE r01): BASELINE.json shapes that had no test, absolute
 1e-4 gates on SIGMOID posteriors over >= 1000 clips, the hidden-32 tile bug, stale weight packs, patch_reference().
 Everything goes through the C ABI; the checker is oracle/kws_oracle.py (pinned to the reference's goldens)."""
+import copy
 import io
 import os
 import sys
@@ -403,7 +404,8 @@ def test_gru_tensor_core_path(B, T, idim):
 
 def test_pipeline_native_call_matches_two_step_chain_and_oracle():
     """Pipeline(frontend, model)(pcm) == model(frontend(pcm)) bit for bit (same kernels, L2-pinned features), for Fbank
-    and MFCC front-ends, with a carried cache, and against the oracle at the posterior gate."""
+    and MFCC front-ends, with a carried cache, and against the oracle at the posterior gate; with the model's precision
+    set to "tensor" as well."""
     from wekws_b200 import Pipeline
     cfg, m, sd = _model("mdtc", cmvn=True)
     pcm = synth.pcm_int16(33, 16000, seed=4)
@@ -420,3 +422,18 @@ def test_pipeline_native_call_matches_two_step_chain_and_oracle():
     assert float((y1.cpu() - y_ref).abs().max()) <= TOL_POST
     with pytest.raises(ValueError):
         Pipeline(Fbank(40), m)
+    # precision = "tensor" takes the tensor-core kernels through the Pipeline as it does through forward: the GRU at a
+    # batch where "auto" takes the FP32 kernel
+    _, g, _ = _model("gru", cmvn=True)
+    fe, pcm = Fbank(80), synth.pcm_int16(4, 16000, seed=6).to(DEV)
+    ref = copy.deepcopy(g)
+    ref.precision = "tensor"
+    y_tc, c_tc = ref(fe(pcm))
+    B, T = y_tc.shape[:2]
+    assert ref.uses_tensor_cores(T, B)
+    ref.precision = "auto"
+    assert not ref.uses_tensor_cores(T, B)
+    g.precision = "tensor"
+    y, c = Pipeline(fe, g)(pcm)
+    assert g.uses_tensor_cores(T, B)
+    assert torch.equal(y, y_tc) and torch.equal(c, c_tc)

@@ -18,10 +18,32 @@ from wekws_b200 import frontend
 
 
 def test_library_exports_every_declared_symbol(native):
+    """The binding agrees with include/wekws_b200.h: every declared symbol with its argument count, the limits, and the
+    layout and size of the records the kernels write."""
     hdr = open(os.path.join(ROOT, "include", "wekws_b200.h")).read()
-    declared = re.findall(r"^WEKWS_API [\w\s\*]+?\b(wekws_\w+)\(", hdr, flags=re.M)
+    code = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
+    params = dict(re.findall(r"^WEKWS_API [\w\s\*]+?\b(wekws_\w+)\(([^)]*)\)", code, flags=re.M))
+    declared = list(params)
     assert len(declared) >= 18
     assert sorted(declared) == sorted(native.SIGNATURES), "binding and header disagree"
+    for name, p in params.items():
+        n = 0 if p.strip() in ("", "void") else p.count(",") + 1
+        assert len(native.SIGNATURES[name][1]) == n, f"{name}: the header declares {n} arguments"
+    defines = {k: int(v) for k, v in re.findall(r"^#define (WEKWS_\w+) (\d+)\b", code, flags=re.M)}
+    assert defines["WEKWS_B200_ABI_VERSION"] == native.ABI_VERSION
+    assert defines["WEKWS_CTC_MAX_PREFIX"] == native.CTC_MAX_PREFIX
+    assert defines["WEKWS_CTC_MAX_PATH_BEAM"] == native.CTC_MAX_PATH_BEAM
+    assert defines["WEKWS_CTC_MAX_SCORE_BEAM"] == native.CTC_MAX_SCORE_BEAM
+    assert defines["WEKWS_CRITERION_MAX_LABEL"] == native.CRITERION_MAX_LABEL
+    numpy_type = {"double": "<f8", "int32_t": "<i4"}
+    for struct, dtype, nbytes in (("wekws_ctc_spot_result", native.SPOT_RESULT_DTYPE, native.SPOT_RESULT_BYTES),
+                                  ("wekws_ctc_stream_detection", native.STREAM_DETECTION_DTYPE,
+                                   native.STREAM_DETECTION_BYTES)):
+        body = re.search(r"typedef struct \{([^}]*)\} " + struct + ";", code).group(1)
+        fields = [(f.strip(), numpy_type[t]) for t, names in re.findall(r"(\w+)\s+([\w\s,]+);", body)
+                  for f in names.split(",")]
+        assert fields == list(dtype), struct
+        assert np.dtype(dtype).itemsize == nbytes, struct
     lib = C.CDLL(native.LIB_PATH)
     for name in declared:
         assert hasattr(lib, name), f"{name} not exported"

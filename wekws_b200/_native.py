@@ -1,4 +1,6 @@
-"""ctypes binding of the C-ABI shared library (include/wekws_b200.h).
+"""ctypes binding of the C-ABI shared library (include/wekws_b200.h), and the one place that knows how a native call
+is made: ``call`` for the stream-taking entry points, ``invoke`` / ``create`` for the others, ``pcm_rows`` /
+``host_lengths`` for the PCM input every audio entry point accepts, ``DeviceHandles`` for per-device native objects.
 
 The library is built in-tree (``python -c 'import __graft_entry__ as g; g.build()'`` or
 ``make -C wekws_b200/csrc``).  There is NO fallback: if the library is missing or a call
@@ -8,6 +10,8 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # WEKWS_B200_LIB: development override (A/B of two builds of the same ABI); the product default is the in-tree library
@@ -20,6 +24,17 @@ PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
 ABI_VERSION = 11
+
+# limits (include/wekws_b200.h #defines)
+CTC_MAX_PREFIX, CTC_MAX_PATH_BEAM, CTC_MAX_SCORE_BEAM = 64, 20, 3
+CRITERION_MAX_LABEL = 511        # one thread per extended-label state (2 L + 1 <= 1023)
+
+# records the kernels write (numpy dtypes of wekws_ctc_spot_result / wekws_ctc_stream_detection)
+SPOT_RESULT_DTYPE = [("score", "<f8"), ("state", "<i4"), ("keyword", "<i4"), ("start", "<i4"), ("end", "<i4"),
+                     ("overflow", "<i4"), ("reserved", "<i4")]
+SPOT_RESULT_BYTES = 32
+STREAM_DETECTION_DTYPE = [("score", "<f8"), ("keyword", "<i4"), ("start", "<i4"), ("end", "<i4"), ("frame", "<i4")]
+STREAM_DETECTION_BYTES = 24
 
 
 class FbankConfig(C.Structure):
@@ -157,3 +172,92 @@ def check(rc: int, what: str) -> None:
 
 def launch_count() -> int:
     return int(lib().wekws_launch_count())
+
+
+def call(name: str, *args, device: torch.device) -> None:
+    """Runs the stream-taking entry point ``name(*args, stream)`` on ``device``'s current stream with ``device``
+    current (no switch when it already is).  A tensor argument is passed as its data pointer; None (NULL), integers
+    and ctypes objects as they are.  Raises RuntimeError with the library's message on a non-zero status."""
+    fn = getattr(_lib if _lib is not None else lib(), name)
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    stream = torch.cuda.current_stream(device).cuda_stream
+    if torch.cuda.current_device() == device.index:
+        rc = fn(*args, stream)
+    else:
+        with torch.cuda.device(device):
+            rc = fn(*args, stream)
+    if rc != 0:
+        check(rc, name)
+
+
+def invoke(name: str, *args, what: str = None) -> None:
+    """Runs a status-returning entry point that takes no stream (set-up calls), arguments as ``call`` takes them;
+    ``what`` names it in the error (default: ``name``)."""
+    check(getattr(lib(), name)(*[a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]), what or name)
+
+
+def create(name: str, *args) -> C.c_void_p:
+    """A new native object from ``name(*args, &handle)`` (the ``*_create`` entry points)."""
+    h = C.c_void_p()
+    invoke(name, *args, C.byref(h))
+    return h
+
+
+_PCM_CODES = {torch.int16: PCM_S16, torch.float32: PCM_F32}
+
+
+def pcm_rows(pcm: torch.Tensor, what: str, one_d: bool = True, dtype_error=TypeError):
+    """Checks PCM input: int16 or float32 samples at int16 scale on a CUDA device, (B, N) rows or, with ``one_d``, one
+    (N,) row.  Returns (the (B, N) rows with unit inner stride, their PCM_* code, whether an (N,) input was lifted to
+    one row).  ``what`` names the entry point in the error for a CPU tensor; another dtype raises ``dtype_error``."""
+    if not pcm.is_cuda:
+        raise RuntimeError(f"wekws_b200.{what} runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
+    lifted = one_d and pcm.dim() == 1
+    if lifted:
+        pcm = pcm.unsqueeze(0)
+    if pcm.dim() != 2:
+        raise ValueError("pcm must be (N,) or (B, N)" if one_d else "pcm must be (B, N)")
+    code = _PCM_CODES.get(pcm.dtype)
+    if code is None:
+        raise dtype_error(f"pcm must be int16 or float32, got {pcm.dtype}")
+    if pcm.stride(1) != 1:
+        pcm = pcm.contiguous()
+    return pcm, code, lifted
+
+
+def host_lengths(lengths, B: int, N: int) -> list:
+    """Valid samples per row given on the host (a sequence or tensor of B ints in 0..N) as a list of ints."""
+    lens = [int(n) for n in (lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)]
+    if len(lens) != B or any(n < 0 or n > N for n in lens):
+        raise ValueError(f"lengths must be {B} values in 0..{N}")
+    return lens
+
+
+class DeviceHandles:
+    """Base of the objects that keep one native object per CUDA device: ``_handle(dev)`` makes it on first use with
+    ``_create()`` and then ``_configure(handle)``, both on that device; the ``_DESTROY`` entry point frees them all
+    when the owner goes."""
+    _DESTROY = ""
+
+    def _create(self) -> C.c_void_p:
+        raise NotImplementedError
+
+    def _configure(self, handle) -> None:
+        """Hook for subclasses: extra native configuration of a freshly created handle."""
+
+    def _handle(self, dev: torch.device) -> C.c_void_p:
+        handles = self.__dict__.setdefault("_handles", {})
+        h = handles.get(dev)
+        if h is None:
+            with torch.cuda.device(dev):
+                h = self._create()
+                self._configure(h)
+            handles[dev] = h
+        return h
+
+    def __del__(self):
+        for h in self.__dict__.get("_handles", {}).values():
+            try:
+                getattr(lib(), self._DESTROY)(h)
+            except Exception:
+                pass

@@ -16,7 +16,6 @@ Deliberate differences from the reference:
 """
 from __future__ import annotations
 
-import ctypes as C
 import io
 import random
 from typing import List, Optional, Sequence, Tuple
@@ -143,27 +142,9 @@ def draw_noise(n: int, source: AugmentSource, prob: float, rng=random) -> Option
     return i, start, rng.uniform(lo, hi)
 
 
-def _pcm_dtype(pcm: torch.Tensor) -> int:
-    if pcm.dtype == torch.int16:
-        return _native.PCM_S16
-    if pcm.dtype == torch.float32:
-        return _native.PCM_F32
-    raise TypeError(f"pcm must be int16 or float32, got {pcm.dtype}")
-
-
 def _check(pcm: torch.Tensor, lengths, what: str) -> Tuple[torch.Tensor, List[int]]:
-    if not pcm.is_cuda:
-        raise RuntimeError(f"wekws_b200.{what} runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
-    if pcm.dim() != 2:
-        raise ValueError("pcm must be (B, N)")
-    _pcm_dtype(pcm)
-    if pcm.stride(1) != 1:
-        pcm = pcm.contiguous()
-    B, N = pcm.shape
-    lens = [int(n) for n in (lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)]
-    if len(lens) != B or any(n < 0 or n > N for n in lens):
-        raise ValueError(f"lengths must be {B} values in 0..{N}")
-    return pcm, lens
+    pcm, _, _ = _native.pcm_rows(pcm, what, one_d=False)
+    return pcm, _native.host_lengths(lengths, *pcm.shape)
 
 
 def _upload(dev, rows: Sequence[int], clips: Sequence[np.ndarray], snr: Optional[Sequence[float]] = None):
@@ -190,14 +171,11 @@ def _upload(dev, rows: Sequence[int], clips: Sequence[np.ndarray], snr: Optional
     return d, o_rows, o_clip
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def launch_reverb(pcm: torch.Tensor, lens: Sequence[int], picks: Sequence[Optional[int]],
                   source: AugmentSource) -> torch.Tensor:
     """The device half of ``reverb``: row b convolved with source clip picks[b] (None = a copy).  pcm (B, N)
     contiguous rows; returns a new float32 (B, N) tensor."""
+    pcm, code, _ = _native.pcm_rows(pcm, "reverb", one_d=False)
     B, N = pcm.shape
     dev = pcm.device
     out = torch.empty(B, N, dtype=torch.float32, device=dev)
@@ -216,11 +194,8 @@ def launch_reverb(pcm: torch.Tensor, lens: Sequence[int], picks: Sequence[Option
     if B == 0 or N == 0:
         return out
     d, o_rows, o_clip = _upload(dev, rows, clips)
-    with torch.cuda.device(dev):
-        rc = _native.lib().wekws_reverb(C.c_void_p(pcm.data_ptr()), _pcm_dtype(pcm), B, N, pcm.stride(0),
-                                        C.c_void_p(d.data_ptr() + o_rows), C.c_void_p(d.data_ptr() + o_clip),
-                                        C.c_void_p(out.data_ptr()), out.stride(0), _stream(dev))
-    _native.check(rc, "wekws_reverb")
+    _native.call("wekws_reverb", pcm, code, B, N, pcm.stride(0), d.data_ptr() + o_rows, d.data_ptr() + o_clip, out,
+                 out.stride(0), device=dev)
     return out
 
 
@@ -228,6 +203,7 @@ def launch_noise(pcm: torch.Tensor, lens: Sequence[int], picks, source: AugmentS
                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The device half of ``add_noise``: picks[b] = (index, start or None, snr) or None.  ``out`` None = a new float32
     (B, N) tensor; ``out`` may be ``pcm`` itself when pcm is float32."""
+    pcm, code, _ = _native.pcm_rows(pcm, "add_noise", one_d=False)
     B, N = pcm.shape
     dev = pcm.device
     if out is None:
@@ -256,12 +232,8 @@ def launch_noise(pcm: torch.Tensor, lens: Sequence[int], picks, source: AugmentS
     if not clips:
         clips = [np.zeros(1, np.float32)]
     d, o_rows, o_clip = _upload(dev, rows, clips, snr)
-    with torch.cuda.device(dev):
-        rc = _native.lib().wekws_add_noise(C.c_void_p(pcm.data_ptr()), _pcm_dtype(pcm), B, N, pcm.stride(0),
-                                           C.c_void_p(d.data_ptr() + o_rows), C.c_void_p(d.data_ptr()),
-                                           C.c_void_p(d.data_ptr() + o_clip), C.c_void_p(out.data_ptr()),
-                                           out.stride(0), _stream(dev))
-    _native.check(rc, "wekws_add_noise")
+    _native.call("wekws_add_noise", pcm, code, B, N, pcm.stride(0), d.data_ptr() + o_rows, d, d.data_ptr() + o_clip,
+                 out, out.stride(0), device=dev)
     return out
 
 

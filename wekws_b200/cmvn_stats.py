@@ -13,7 +13,6 @@ differences from the tool:
 """
 from __future__ import annotations
 
-import ctypes as C
 import json
 from typing import Optional, Sequence, Tuple, Union
 
@@ -72,15 +71,9 @@ class CmvnStats:
     def update(self, pcm: torch.Tensor, lengths: Union[Sequence[int], torch.Tensor, None], sample_rate: int) -> None:
         """Adds the utterances of ``pcm`` (B, N) (int16 or float32 at int16 scale, CUDA), row b = its first
         lengths[b] samples, all at ``sample_rate``."""
-        if not pcm.is_cuda:
-            raise RuntimeError("wekws_b200.CmvnStats runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
-        if pcm.dim() != 2:
-            raise ValueError("pcm must be (B, N)")
+        pcm, _, _ = _native.pcm_rows(pcm, "CmvnStats", one_d=False)
         B, N = pcm.shape
-        lens = [N] * B if lengths is None else [int(n) for n in (
-            lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)]
-        if len(lens) != B or any(n < 0 or n > N for n in lens):
-            raise ValueError(f"lengths must be {B} values in 0..{N}")
+        lens = [N] * B if lengths is None else _native.host_lengths(lengths, B, N)
         dev = pcm.device
         if self._acc is None:
             self._acc = torch.zeros(2, self.feat_dim, dtype=torch.float64, device=dev)
@@ -110,13 +103,8 @@ class CmvnStats:
         feats = self.frontend(wave, lengths=d_lens)
         ws = torch.empty(_native.lib().wekws_cmvn_stats_workspace_bytes(B, self.feat_dim), dtype=torch.uint8,
                          device=dev)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            rc = _native.lib().wekws_cmvn_stats_accumulate(
-                C.c_void_p(feats.data_ptr()), B, feats.shape[1], self.feat_dim, C.c_void_p(d_frames.data_ptr()),
-                C.c_void_p(self._acc.data_ptr()), C.c_void_p(self._frames.data_ptr()), C.c_void_p(ws.data_ptr()),
-                C.c_void_p(stream))
-        _native.check(rc, "wekws_cmvn_stats_accumulate")
+        _native.call("wekws_cmvn_stats_accumulate", feats, B, feats.shape[1], self.feat_dim, d_frames, self._acc,
+                     self._frames, ws, device=dev)
 
     @property
     def frame_num(self) -> int:

@@ -13,17 +13,16 @@ reference's own ``Executor.cv`` / ``Executor.test`` evaluate a set with it.  The
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 import sys
 
 import torch
 
 from . import _native
+from ._native import CRITERION_MAX_LABEL as MAX_LABEL
+from ._native import CTC_MAX_PREFIX as MAX_PREFIX      # longest hypothesis the accuracy decode keeps
 
 IGNORE_INDEX = -100          # F.cross_entropy's default, part of the reference's contract
-MAX_LABEL = 511              # WEKWS_CRITERION_MAX_LABEL: one thread per extended-label state (2 L + 1 <= 1023)
-MAX_PREFIX = 64              # WEKWS_CTC_MAX_PREFIX: longest hypothesis the accuracy decode keeps
 _INTS = (torch.int8, torch.int16, torch.int32, torch.int64, torch.uint8)
 
 
@@ -58,14 +57,6 @@ def _ints(name, t, x, dim=1, size=None):
     return t
 
 
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream(x):
-    return C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-
-
 def max_pooling_loss(logits, target, lengths, min_duration=0, terms=False):
     """loss.py:26-88.  logits (B, T, D) posteriors, target (B,) (< 0 = filler), lengths (B,) with max == T.
     terms=True also returns {'term': (B, D) losses, 'correct': (B,) 0/1}."""
@@ -81,16 +72,14 @@ def max_pooling_loss(logits, target, lengths, min_duration=0, terms=False):
                          f"{int(lens_h.max())}): the reference's padding mask does not broadcast otherwise")
     tgt = target.clamp(-1, D).to(torch.int32)          # < 0: filler, D: no keyword column -- the reference's cases
     lens = lengths.to(torch.int32)
-    lib = _native.lib()
-    ws = torch.empty(int(lib.wekws_criterion_max_pooling_workspace_bytes(B, D)), dtype=torch.uint8, device=x.device)
+    ws = torch.empty(int(_native.lib().wekws_criterion_max_pooling_workspace_bytes(B, D)), dtype=torch.uint8,
+                     device=x.device)
     loss = torch.empty((), dtype=torch.float32, device=x.device)
     acc = torch.empty(1, dtype=torch.float64, device=x.device)
     out = dict(term=torch.empty(B, D, dtype=torch.float32, device=x.device),
                correct=torch.empty(B, dtype=torch.int32, device=x.device)) if terms else {}
-    with torch.cuda.device(x.device):
-        rc = lib.wekws_criterion_max_pooling(_p(x), _p(tgt), _p(lens), B, T, D, int(min_duration), _p(ws), _p(loss),
-                                             _p(acc), _p(out.get("term")), _p(out.get("correct")), _stream(x))
-    _native.check(rc, "wekws_criterion_max_pooling")
+    _native.call("wekws_criterion_max_pooling", x, tgt, lens, B, T, D, int(min_duration), ws, loss, acc,
+                 out.get("term"), out.get("correct"), device=x.device)
     return loss, float(acc.item()), out
 
 
@@ -104,16 +93,13 @@ def cross_entropy(logits, target, terms=False):
     if bool(bad.any()):
         raise IndexError(f"Target {int(target[bad][0])} is out of bounds.")
     tgt = target.to(torch.int32)
-    lib = _native.lib()
-    ws = torch.empty(int(lib.wekws_criterion_ce_workspace_bytes(B)), dtype=torch.uint8, device=x.device)
+    ws = torch.empty(int(_native.lib().wekws_criterion_ce_workspace_bytes(B)), dtype=torch.uint8, device=x.device)
     loss = torch.empty((), dtype=torch.float32, device=x.device)
     acc = torch.empty(1, dtype=torch.float64, device=x.device)
     out = dict(term=torch.empty(B, dtype=torch.float32, device=x.device),
                correct=torch.empty(B, dtype=torch.int32, device=x.device)) if terms else {}
-    with torch.cuda.device(x.device):
-        rc = lib.wekws_criterion_ce(_p(x), _p(tgt), B, Cn, _p(ws), _p(loss), _p(acc), _p(out.get("term")),
-                                    _p(out.get("correct")), _stream(x))
-    _native.check(rc, "wekws_criterion_ce")
+    _native.call("wekws_criterion_ce", x, tgt, B, Cn, ws, loss, acc, out.get("term"), out.get("correct"),
+                 device=x.device)
     return loss, float(acc.item()), out
 
 
@@ -153,10 +139,9 @@ def ctc_loss(logits, target, lengths, target_lengths, validation=False, terms=Fa
     lab = target.to(torch.int32).contiguous()
     lens = lengths.to(torch.int32)
     tls = target_lengths.to(torch.int32)
-    lib = _native.lib()
     dev = x.device
-    ws = torch.empty(int(lib.wekws_criterion_ctc_workspace_bytes(B, T, int(bool(validation)))), dtype=torch.uint8,
-                     device=dev)
+    ws = torch.empty(int(_native.lib().wekws_criterion_ctc_workspace_bytes(B, T, int(bool(validation)))),
+                     dtype=torch.uint8, device=dev)
     loss = torch.empty((), dtype=torch.float32, device=dev)
     acc = torch.empty(1, dtype=torch.float64, device=dev)
     overflow = torch.empty(B, dtype=torch.int32, device=dev) if validation else None
@@ -167,11 +152,8 @@ def ctc_loss(logits, target, lengths, target_lengths, validation=False, terms=Fa
             out["correct"] = torch.empty(B, dtype=torch.int32, device=dev)
             out["best"] = torch.empty(B, 1 + MAX_PREFIX, dtype=torch.int32, device=dev)
     stride = n_lab if target.dim() == 2 else 0
-    with torch.cuda.device(dev):
-        rc = lib.wekws_criterion_ctc(_p(x), _p(lens), B, T, V, _p(lab), stride, _p(tls), int(tl_h.max()),
-                                     int(bool(validation)), _p(ws), _p(loss), _p(acc), _p(out.get("term")),
-                                     _p(out.get("correct")), _p(overflow), _p(out.get("best")), _stream(x))
-    _native.check(rc, "wekws_criterion_ctc")
+    _native.call("wekws_criterion_ctc", x, lens, B, T, V, lab, stride, tls, int(tl_h.max()), int(bool(validation)), ws,
+                 loss, acc, out.get("term"), out.get("correct"), overflow, out.get("best"), device=dev)
     if not validation:
         return loss, 0.0, out
     res = torch.cat([acc, overflow.to(torch.float64)]).cpu()

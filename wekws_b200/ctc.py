@@ -8,15 +8,26 @@ order, scores as doubles, node frames / probabilities; see csrc/ctc_decode.cu fo
 """
 from __future__ import annotations
 
-import ctypes as C
-import math
+import itertools
 from typing import Dict, Iterable, List, Optional, Sequence
 
 import torch
 
 from . import _native
+from ._native import CTC_MAX_PATH_BEAM as MAX_PATH_BEAM
+from ._native import CTC_MAX_PREFIX as MAX_PREFIX
+from ._native import CTC_MAX_SCORE_BEAM as MAX_SCORE_BEAM
+from ._native import SPOT_RESULT_BYTES, SPOT_RESULT_DTYPE, STREAM_DETECTION_BYTES, STREAM_DETECTION_DTYPE  # noqa: F401
 
-MAX_PREFIX, MAX_PATH_BEAM, MAX_SCORE_BEAM = 64, 20, 3
+STREAM_SCORE_CAPACITY = 32         # detection records per utterance of the first launch of stream_score_ctc
+
+
+def _pack_keywords(seqs: Sequence[Sequence[int]], device):
+    """Keyword token lists as the kernels take them: int32 device tensors (tokens back to back, offsets), keyword k
+    being tokens[offsets[k]:offsets[k + 1]]."""
+    offsets = [0, *itertools.accumulate(len(s) for s in seqs)]
+    return (torch.tensor([t for s in seqs for t in s], dtype=torch.int32, device=device),
+            torch.tensor(offsets, dtype=torch.int32, device=device))
 
 
 class CtcHyps:
@@ -78,17 +89,10 @@ def ctc_prefix_beam_search(probs: torch.Tensor, lengths: Optional[torch.Tensor] 
     if state is not None and (state.dtype != torch.uint8 or state.device != dev or not state.is_contiguous()
                               or tuple(state.shape) != (B, int(_native.lib().wekws_ctc_state_bytes()))):
         raise ValueError("state must come from ctc_state(B, device)")
-
-    def p(t):
-        return C.c_void_p(t.data_ptr()) if t is not None else None
-
-    with torch.cuda.device(dev):
-        rc = _native.lib().wekws_ctc_prefix_beam_search(
-            p(probs), p(lens), B, T, V, p(kw), 0 if kw is None else kw.numel(), int(score_beam_size), int(path_beam_size),
-            int(frame_offset), int(frame_stride), p(state), 1 if reset_state else 0, p(out.nhyp), p(out.hyp_len),
-            p(out.hyp_tokens), p(out.hyp_score), p(out.node_frame), p(out.node_prob), p(out.overflow),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    _native.check(rc, "wekws_ctc_prefix_beam_search")
+    _native.call("wekws_ctc_prefix_beam_search", probs, lens, B, T, V, kw, 0 if kw is None else kw.numel(),
+                 int(score_beam_size), int(path_beam_size), int(frame_offset), int(frame_stride), state,
+                 1 if reset_state else 0, out.nhyp, out.hyp_len, out.hyp_tokens, out.hyp_score, out.node_frame,
+                 out.node_prob, out.overflow, device=dev)
     return out
 
 
@@ -97,27 +101,14 @@ def ctc_keyword_hits(hyps: CtcHyps, keywords_token: Dict[str, dict]):
     (dict order) -> list of (word or None, hit_score, start_frame, end_frame).  keywords_token: {word: {'token_id':
     [...]}} as the reference builds it (score_ctc.py:159-171)."""
     words = list(keywords_token.keys())
-    seqs = [list(keywords_token[w]["token_id"]) for w in words]
     dev = hyps.nhyp.device
-    flat = torch.tensor([t for s in seqs for t in s], dtype=torch.int32, device=dev)
-    offs = [0]
-    for s in seqs:
-        offs.append(offs[-1] + len(s))
-    offs = torch.tensor(offs, dtype=torch.int32, device=dev)
+    flat, offs = _pack_keywords([list(keywords_token[w]["token_id"]) for w in words], dev)
     hit = torch.empty(hyps.B, dtype=torch.int32, device=dev)
     score = torch.empty(hyps.B, dtype=torch.float64, device=dev)
     start = torch.empty(hyps.B, dtype=torch.int32, device=dev)
     end = torch.empty(hyps.B, dtype=torch.int32, device=dev)
-
-    def p(t):
-        return C.c_void_p(t.data_ptr())
-
-    with torch.cuda.device(dev):
-        rc = _native.lib().wekws_ctc_keyword_hit(
-            p(hyps.nhyp), p(hyps.hyp_len), p(hyps.hyp_tokens), p(hyps.node_frame), p(hyps.node_prob), hyps.B,
-            hyps.path_beam, p(flat), p(offs), len(words), p(hit), p(score), p(start), p(end),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    _native.check(rc, "wekws_ctc_keyword_hit")
+    _native.call("wekws_ctc_keyword_hit", hyps.nhyp, hyps.hyp_len, hyps.hyp_tokens, hyps.node_frame, hyps.node_prob,
+                 hyps.B, hyps.path_beam, flat, offs, len(words), hit, score, start, end, device=dev)
     hit, score, start, end = hit.cpu().tolist(), score.cpu().tolist(), start.cpu().tolist(), end.cpu().tolist()
     return [(words[h] if h >= 0 else None, score[b], start[b], end[b]) for b, h in enumerate(hit)]
 
@@ -129,12 +120,6 @@ def write_ctc_scores(fout, keys: Sequence[str], hits) -> None:
             fout.write('{} detected {} {:.3f}\n'.format(key, word, hit_score))
         else:
             fout.write('{} rejected\n'.format(key))
-
-
-# one wekws_ctc_spot_result per stream (include/wekws_b200.h)
-SPOT_RESULT_DTYPE = [("score", "<f8"), ("state", "<i4"), ("keyword", "<i4"), ("start", "<i4"), ("end", "<i4"),
-                     ("overflow", "<i4"), ("reserved", "<i4")]
-SPOT_RESULT_BYTES = 32
 
 
 def check_spot_args(keywords: Dict[str, Sequence[int]], score_beam_size: int, path_beam_size: int,
@@ -154,12 +139,6 @@ def check_spot_args(keywords: Dict[str, Sequence[int]], score_beam_size: int, pa
         if not 1 <= len(s) <= MAX_PREFIX or min(s) < 0:
             raise ValueError(f"keyword {w!r}: 1..{MAX_PREFIX} non-negative token ids are needed, got {s}")
     return words, seqs
-
-
-# one wekws_ctc_stream_detection per activation (include/wekws_b200.h)
-STREAM_DETECTION_DTYPE = [("score", "<f8"), ("keyword", "<i4"), ("start", "<i4"), ("end", "<i4"), ("frame", "<i4")]
-STREAM_DETECTION_BYTES = 24
-STREAM_SCORE_CAPACITY = 32         # detection records per utterance of the first launch
 
 
 class StreamScores:
@@ -210,25 +189,15 @@ def stream_score_ctc(probs: torch.Tensor, lengths, keywords: Dict[str, Sequence[
     probs = probs.contiguous()
     lens = lens_host.to(device=dev, dtype=torch.int32)
     tset = torch.tensor(sorted(tokenset), dtype=torch.int32, device=dev)
-    kw = torch.tensor([t for s in seqs for t in s], dtype=torch.int32, device=dev)
-    offs = [0]
-    for s in seqs:
-        offs.append(offs[-1] + len(s))
-    off = torch.tensor(offs, dtype=torch.int32, device=dev)
+    kw, off = _pack_keywords(seqs, dev)
     count = torch.zeros(B, dtype=torch.int32, device=dev)
     overflow = torch.zeros(B, dtype=torch.int32, device=dev)
 
-    def p(t):
-        return C.c_void_p(t.data_ptr())
-
     def launch(cap):
         det = torch.empty(B, cap, STREAM_DETECTION_BYTES, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            rc = _native.lib().wekws_ctc_stream_score(
-                p(probs), p(lens), B, T, V, p(tset), tset.numel(), p(kw), p(off), len(words), int(score_beam_size),
-                int(path_beam_size), int(frame_skip), float(threshold), int(min_frames), int(max_frames), cap, p(count),
-                p(det), p(overflow), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _native.check(rc, "wekws_ctc_stream_score")
+        _native.call("wekws_ctc_stream_score", probs, lens, B, T, V, tset, tset.numel(), kw, off, len(words),
+                     int(score_beam_size), int(path_beam_size), int(frame_skip), float(threshold), int(min_frames),
+                     int(max_frames), cap, count, det, overflow, device=dev)
         return det
 
     cap = STREAM_SCORE_CAPACITY
@@ -270,12 +239,8 @@ class CtcSpotDecoder:
             tokenset.update(s)
         self.tokenset = tokenset
         self.max_token = max(tokenset)
-        offs = [0]
-        for s in seqs:
-            offs.append(offs[-1] + len(s))
         self._set = torch.tensor(sorted(tokenset), dtype=torch.int32, device=self.dev)
-        self._kw = torch.tensor([t for s in seqs for t in s], dtype=torch.int32, device=self.dev)
-        self._off = torch.tensor(offs, dtype=torch.int32, device=self.dev)
+        self._kw, self._off = _pack_keywords(seqs, self.dev)
         self.state = ctc_state(self.B, self.dev)
         self.det = torch.zeros(self.B, int(_native.lib().wekws_ctc_spot_state_bytes()), dtype=torch.uint8,
                                device=self.dev)
@@ -309,17 +274,10 @@ class CtcSpotDecoder:
         for b, x in enumerate(live):
             if x:
                 self._live[b] = True
-
-        def p(t):
-            return C.c_void_p(t.data_ptr())
-
-        with torch.cuda.device(self.dev):
-            rc = _native.lib().wekws_ctc_spot(
-                p(probs), V, p(rows), p(frames), self.B, p(self._set), self._set.numel(), p(self._kw), p(self._off),
-                len(self.words), self.score_beam, self.path_beam, self.frame_stride, self.threshold, self.min_frames,
-                self.max_frames, self.interval_frames, p(self.state), p(self.det), p(self.result),
-                C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream))
-        _native.check(rc, "wekws_ctc_spot")
+        _native.call("wekws_ctc_spot", probs, V, rows, frames, self.B, self._set, self._set.numel(), self._kw, self._off,
+                     len(self.words), self.score_beam, self.path_beam, self.frame_stride, self.threshold,
+                     self.min_frames, self.max_frames, self.interval_frames, self.state, self.det, self.result,
+                     device=self.dev)
         return self.result
 
     def hypotheses(self) -> List[list]:

@@ -74,7 +74,7 @@ def lifter_coeffs(num_ceps: int, cepstral_lifter: float) -> torch.Tensor:
     return 1.0 + 0.5 * cepstral_lifter * torch.sin(math.pi * i / cepstral_lifter)
 
 
-class Fbank:
+class Fbank(_native.DeviceHandles):
     """Batched GPU Fbank(+CMVN).  ``__call__(pcm)``: pcm (B, N) or (N,) int16 / float32 CUDA
     tensor in int16 scale (the reference multiplies normalised audio by 1<<15 first,
     processor.py:194) -> (B, m, num_mel_bins) float32 with m = 1 + (N - 400) // 160."""
@@ -91,34 +91,16 @@ class Fbank:
                                        float(preemphasis_coefficient), int(bool(remove_dc_offset)), EPSILON)
         self.window = window_function(window_type, self.win).contiguous()
         self.mel = mel_filterbank(num_mel_bins, self.n_fft, sample_frequency, low_freq, high_freq)
-        self._handles = {}
         self.device = device
         self.feature_dim = num_mel_bins          # row width of the output (num_ceps for the Mfcc subclass)
 
-    def _configure(self, handle) -> None:
-        """Hook for subclasses: extra native configuration of a freshly created handle."""
+    _DESTROY = "wekws_fbank_destroy"
+
+    def _create(self):
+        return _native.create("wekws_fbank_create", C.byref(self.cfg), self.window, self.mel)
 
     def num_frames(self, num_samples: int) -> int:
         return 0 if num_samples < self.win else 1 + (num_samples - self.win) // self.shift
-
-    def _handle(self, dev: torch.device):
-        h = self._handles.get(dev)
-        if h is None:
-            h = C.c_void_p()
-            with torch.cuda.device(dev):
-                _native.check(_native.lib().wekws_fbank_create(
-                    C.byref(self.cfg), C.c_void_p(self.window.data_ptr()), C.c_void_p(self.mel.data_ptr()),
-                    C.byref(h)), "wekws_fbank_create")
-                self._configure(h)
-            self._handles[dev] = h
-        return h
-
-    def __del__(self):
-        for h in getattr(self, "_handles", {}).values():
-            try:
-                _native.lib().wekws_fbank_destroy(h)
-            except Exception:
-                pass
 
     def __call__(self, pcm: torch.Tensor, lengths: Optional[torch.Tensor] = None,
                  mean: Optional[torch.Tensor] = None, istd: Optional[torch.Tensor] = None,
@@ -128,21 +110,7 @@ class Fbank:
         every framed sample.  One 64-bit seed is drawn per call from ``generator`` (torch's default CPU generator when
         None, so torch.manual_seed governs it as it governs the reference's torch.randn); the noise is a documented
         function of (seed, row, frame, sample) (include/wekws_b200.h), not torch.randn's values."""
-        if not pcm.is_cuda:
-            raise RuntimeError("wekws_b200.Fbank runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
-        squeeze = pcm.dim() == 1
-        if squeeze:
-            pcm = pcm.unsqueeze(0)
-        if pcm.dim() != 2:
-            raise ValueError("pcm must be (N,) or (B, N)")
-        if pcm.dtype == torch.int16:
-            dtype = _native.PCM_S16
-        elif pcm.dtype == torch.float32:
-            dtype = _native.PCM_F32
-        else:
-            raise TypeError(f"pcm must be int16 or float32, got {pcm.dtype}")
-        if pcm.stride(1) != 1:
-            pcm = pcm.contiguous()
+        pcm, code, lifted = _native.pcm_rows(pcm, "Fbank")
         dev = pcm.device
         B, N = pcm.shape
         m = self.num_frames(N)
@@ -150,28 +118,15 @@ class Fbank:
             out = torch.empty(B, m, self.feature_dim, device=dev, dtype=torch.float32)
         elif tuple(out.shape) != (B, m, self.feature_dim) or not out.is_contiguous():
             raise ValueError("out must be a contiguous (B, m, feature_dim) tensor")
-
-        def ptr(t, dt):
-            if t is None:
-                return None
-            t = t.to(device=dev, dtype=dt).contiguous()
-            keep.append(t)
-            return C.c_void_p(t.data_ptr())
-
-        keep = []
         if B > 0 and m > 0:
-            h = self._handle(dev)
-            with torch.cuda.device(dev):
-                stream = torch.cuda.current_stream(dev).cuda_stream
-                args = (h, C.c_void_p(pcm.data_ptr()), dtype, B, N, pcm.stride(0), ptr(lengths, torch.int32),
-                        ptr(mean, torch.float32), ptr(istd, torch.float32), C.c_void_p(out.data_ptr()), m)
-                if dither == 0.0:
-                    rc = _native.lib().wekws_fbank_forward(*args, C.c_void_p(stream))
-                else:
-                    rc = _native.lib().wekws_fbank_forward_dither(*args, float(dither), draw_seed(generator),
-                                                                  C.c_void_p(stream))
-            _native.check(rc, "wekws_fbank_forward")
-        return out[0] if squeeze else out
+            lengths, mean, istd = (None if t is None else t.to(device=dev, dtype=dt).contiguous() for t, dt in
+                                   ((lengths, torch.int32), (mean, torch.float32), (istd, torch.float32)))
+            args = (self._handle(dev), pcm, code, B, N, pcm.stride(0), lengths, mean, istd, out, m)
+            if dither == 0.0:
+                _native.call("wekws_fbank_forward", *args, device=dev)
+            else:
+                _native.call("wekws_fbank_forward_dither", *args, float(dither), draw_seed(generator), device=dev)
+        return out[0] if lifted else out
 
 
 def draw_seed(generator: Optional[torch.Generator] = None) -> int:
@@ -198,9 +153,7 @@ class Mfcc(Fbank):
         self.lifter = lifter_coeffs(num_ceps, cepstral_lifter).float().contiguous() if cepstral_lifter != 0.0 else None
 
     def _configure(self, handle) -> None:
-        _native.check(_native.lib().wekws_fbank_set_mfcc(
-            handle, self.num_ceps, C.c_void_p(self.dct.data_ptr()),
-            C.c_void_p(self.lifter.data_ptr()) if self.lifter is not None else None), "wekws_fbank_set_mfcc")
+        _native.invoke("wekws_fbank_set_mfcc", handle, self.num_ceps, self.dct, self.lifter)
 
 
 def sinc_resample_kernel(orig_freq: int, new_freq: int, lowpass_filter_width: int = 6, rolloff: float = 0.99,
@@ -237,7 +190,7 @@ def sinc_resample_kernel(orig_freq: int, new_freq: int, lowpass_filter_width: in
 _RESAMPLE_DENSE_MAX = 1 << 24        # dense table entries; far past any pair whose compact table fits on chip
 
 
-class Resample:
+class Resample(_native.DeviceHandles):
     """Batched GPU twin of ``torchaudio.transforms.Resample(orig_freq, new_freq)`` (sinc_interp_hann,
     lowpass_filter_width 6, rolloff 0.99), as wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py
     call it.  ``__call__(pcm, lengths=None)``: pcm (B, N) or (N,) int16 / float32 CUDA tensor at int16 scale ->
@@ -256,7 +209,6 @@ class Resample:
             self.kernel, self.width = sinc_resample_kernel(self.orig_freq, self.new_freq, lowpass_filter_width,
                                                            rolloff, resampling_method)
             self.kernel = self.kernel.reshape(self.kernel.shape[0], -1).contiguous()
-        self._handles = {}
 
     def output_length(self, num_samples: int) -> int:
         """torchaudio's target length ceil(torch.as_tensor(new * n / orig)): the quotient passes through float32, so
@@ -269,42 +221,15 @@ class Resample:
         target = math.ceil(float(np.float32(n * int(num_samples) / o)))
         return min(target, (int(num_samples) // o + 1) * n)
 
-    def _handle(self, dev: torch.device):
-        h = self._handles.get(dev)
-        if h is None:
-            h = C.c_void_p()
-            with torch.cuda.device(dev):
-                _native.check(_native.lib().wekws_resample_create(
-                    self.orig_freq, self.new_freq, C.c_void_p(self.kernel.data_ptr()), self.width, C.byref(h)),
-                    "wekws_resample_create")
-            self._handles[dev] = h
-        return h
+    _DESTROY = "wekws_resample_destroy"
 
-    def __del__(self):
-        for h in getattr(self, "_handles", {}).values():
-            try:
-                _native.lib().wekws_resample_destroy(h)
-            except Exception:
-                pass
+    def _create(self):
+        return _native.create("wekws_resample_create", self.orig_freq, self.new_freq, self.kernel, self.width)
 
     def __call__(self, pcm: torch.Tensor, lengths=None) -> torch.Tensor:
         if self.orig_freq == self.new_freq:
             return pcm                       # as the transform does
-        if not pcm.is_cuda:
-            raise RuntimeError("wekws_b200.Resample runs on CUDA (sm_90a) only; got a CPU tensor (no CPU fallback)")
-        squeeze = pcm.dim() == 1
-        if squeeze:
-            pcm = pcm.unsqueeze(0)
-        if pcm.dim() != 2:
-            raise ValueError("pcm must be (N,) or (B, N)")
-        if pcm.dtype == torch.int16:
-            dtype = _native.PCM_S16
-        elif pcm.dtype == torch.float32:
-            dtype = _native.PCM_F32
-        else:
-            raise TypeError(f"pcm must be int16 or float32, got {pcm.dtype}")
-        if pcm.stride(1) != 1:
-            pcm = pcm.contiguous()
+        pcm, code, lifted = _native.pcm_rows(pcm, "Resample")
         dev = pcm.device
         B, N = pcm.shape
         max_out = self.output_length(N)
@@ -315,15 +240,9 @@ class Resample:
             if lens.shape != (B,):
                 raise ValueError(f"lengths must have shape ({B},), got {tuple(lens.shape)}")
         if B > 0 and max_out > 0:
-            h = self._handle(dev)
-            with torch.cuda.device(dev):
-                stream = torch.cuda.current_stream(dev).cuda_stream
-                rc = _native.lib().wekws_resample_forward(
-                    h, C.c_void_p(pcm.data_ptr()), dtype, B, N, pcm.stride(0),
-                    C.c_void_p(lens.data_ptr()) if lens is not None else None, C.c_void_p(out.data_ptr()),
-                    out.stride(0), max_out, C.c_void_p(stream))
-            _native.check(rc, "wekws_resample_forward")
-        return out[0] if squeeze else out
+            _native.call("wekws_resample_forward", self._handle(dev), pcm, code, B, N, pcm.stride(0), lens, out,
+                         out.stride(0), max_out, device=dev)
+        return out[0] if lifted else out
 
 
 def resample(waveform: torch.Tensor, orig_freq: int, new_freq: int) -> torch.Tensor:

@@ -250,24 +250,17 @@ class KWSModel(nn.Module):
 
     def _build_handle(self, finalize: bool = True):
         """Creates the native model and feeds it the state_dict by its reference key names."""
-        lib = _native.lib()
         self._release()
-        cfg = self._native_config()
-        h = C.c_void_p()
-        _native.check(lib.wekws_model_create(C.byref(cfg), C.byref(h)), "wekws_model_create")
-        self._handle = h
+        h = self._handle = _native.create("wekws_model_create", C.byref(self._native_config()))
         if self.head is not None:
-            _native.check(lib.wekws_model_set_head(h, _HEADS[self.head]), "wekws_model_set_head")
+            _native.invoke("wekws_model_set_head", h, _HEADS[self.head])
         for name, t in self.state_dict().items():
             if name.endswith("num_batches_tracked"):
                 continue
             host = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
-            _native.check(lib.wekws_model_set_tensor(h, name.encode(), C.c_void_p(host.data_ptr()), host.numel()),
-                          f"wekws_model_set_tensor({name})")
-        if finalize:
-            _native.check(lib.wekws_model_finalize(h), "wekws_model_finalize")
-        else:
-            _native.check(lib.wekws_model_pack(h), "wekws_model_pack")
+            _native.invoke("wekws_model_set_tensor", h, name.encode(), host, host.numel(),
+                           what=f"wekws_model_set_tensor({name})")
+        _native.invoke("wekws_model_finalize" if finalize else "wekws_model_pack", h)
         return h
 
     def _fingerprint(self) -> int:
@@ -305,10 +298,53 @@ class KWSModel(nn.Module):
         if self._precision_applied != self.precision:
             if self.precision not in self._PRECISIONS:
                 raise ValueError("precision must be 'auto', 'fp32' or 'tensor'")
-            _native.check(_native.lib().wekws_model_set_precision(h, self._PRECISIONS[self.precision]),
-                          "wekws_model_set_precision")
+            _native.invoke("wekws_model_set_precision", h, self._PRECISIONS[self.precision])
             self._precision_applied = self.precision
 
+    def _prepare(self, device: torch.device):
+        """The native model for a call on `device`: packed from the current weights, with `precision` applied."""
+        h = self._ensure(device)
+        self._apply_precision(h)
+        return h
+
+    # ------------------------------------------------------------------------- streaming cache
+    def cache_shape(self, B: int) -> Tuple[int, ...]:
+        """Shape of the streaming cache of B streams: GRU (num_layers, B, hdim); FSMN (B, proj_dim, cache_len,
+        num_layers), one column block per layer (fsmn.py:488); the convolutional backbones (B, hdim, padding)."""
+        bb = self.backbone
+        if isinstance(bb, nn.GRU):
+            return (bb.num_layers, B, self.hdim)
+        if getattr(bb, "kind", None) == "fsmn":
+            return (B, bb.proj_dim, bb.cache_len, bb.fsmn_layers)
+        return (B, self.hdim, bb.padding)
+
+    @property
+    def cache_batch_dim(self) -> int:
+        """The dimension of the streaming cache that indexes the streams."""
+        return 1 if isinstance(self.backbone, nn.GRU) else 0
+
+    def _io_tensors(self, in_cache: Optional[torch.Tensor], B: int, T: int, dev: torch.device):
+        """(input cache as the native call takes it -- None when empty --, output, output cache) of a call over B
+        streams of T frames.  Without frames to run the output cache is already the result: the input cache, or zeros."""
+        head = self.head
+        if head is not None and T == 0:
+            raise ValueError(f"the '{head}' classifier head needs at least one frame per call")
+        shape = self.cache_shape(B)
+        cache = None
+        if in_cache is not None and in_cache.numel() > 0:
+            if tuple(in_cache.shape) != shape:
+                raise ValueError(f"in_cache must be {shape}, got {tuple(in_cache.shape)}")
+            if in_cache.device != dev or in_cache.dtype != torch.float32 or not in_cache.is_contiguous():
+                in_cache = in_cache.to(device=dev, dtype=torch.float32).contiguous()
+            cache = in_cache
+        out = torch.empty((B, self.odim) if head is not None else (B, T, self.odim), device=dev, dtype=torch.float32)
+        if B > 0 and T > 0:
+            out_cache = torch.empty(shape, device=dev, dtype=torch.float32)
+        elif cache is not None:
+            out_cache = cache.clone()
+        else:
+            out_cache = torch.zeros(shape, device=dev, dtype=torch.float32)
+        return cache, out, out_cache
 
     # ------------------------------------------------------------------------- forward
     def _run(self, x: torch.Tensor, in_cache: torch.Tensor, flags: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -324,45 +360,12 @@ class KWSModel(nn.Module):
             raise ValueError(f"features must be (B, T, {self.idim}), got {tuple(x.shape)}")
         dev = x.device
         B, T = x.size(0), x.size(1)
-        head = self.head
-        if head is not None and T == 0:
-            raise ValueError(f"the '{head}' classifier head needs at least one frame per call")
         if not x.is_contiguous():
             x = x.contiguous()
-        gru = isinstance(self.backbone, nn.GRU)
-        if gru:
-            cache_shape = (self.backbone.num_layers, B, self.hdim)
-        elif getattr(self.backbone, "kind", None) == "fsmn":      # 4-D: one column block per layer (fsmn.py:488)
-            cache_shape = (B, self.backbone.proj_dim, self.backbone.cache_len, self.backbone.fsmn_layers)
-        else:
-            cache_shape = (B, self.hdim, self.backbone.padding)
-        cache_ptr = None
-        if in_cache is not None and in_cache.numel() > 0:
-            if tuple(in_cache.shape) != cache_shape:
-                raise ValueError(f"in_cache must be {cache_shape}, got {tuple(in_cache.shape)}")
-            if in_cache.device != dev or in_cache.dtype != torch.float32 or not in_cache.is_contiguous():
-                in_cache = in_cache.to(device=dev, dtype=torch.float32).contiguous()
-            cache_ptr = in_cache.data_ptr()
-        h = self._ensure(dev)
-        self._apply_precision(h)
-        out = torch.empty((B, self.odim) if head is not None else (B, T, self.odim), device=dev, dtype=torch.float32)
-        if T == 0 and cache_ptr is not None:
-            out_cache = in_cache.clone()
-        elif T == 0:
-            out_cache = torch.zeros(cache_shape, device=dev, dtype=torch.float32)
-        else:
-            out_cache = torch.empty(cache_shape, device=dev, dtype=torch.float32)
+        cache, out, out_cache = self._io_tensors(in_cache, B, T, dev)
+        h = self._prepare(dev)
         if B > 0 and T > 0:
-            fwd = _native.lib().wekws_model_forward
-            if torch.cuda.current_device() == dev.index:          # common case: no device switch needed
-                rc = fwd(h, x.data_ptr(), cache_ptr, out.data_ptr(), out_cache.data_ptr(), B, T, flags,
-                         torch.cuda.current_stream(dev).cuda_stream)
-            else:
-                with torch.cuda.device(dev):
-                    rc = fwd(h, x.data_ptr(), cache_ptr, out.data_ptr(), out_cache.data_ptr(), B, T, flags,
-                             torch.cuda.current_stream(dev).cuda_stream)
-            if rc != 0:
-                _native.check(rc, "wekws_model_forward")
+            _native.call("wekws_model_forward", h, x, cache, out, out_cache, B, T, flags, device=dev)
         return out, out_cache
 
     def forward(self, x: torch.Tensor, in_cache: torch.Tensor = _EMPTY) -> Tuple[torch.Tensor, torch.Tensor]:

@@ -7,7 +7,6 @@ of CTC score files (``compute_det_ctc.py``) are per utterance and tiny; they run
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 import re
 from typing import Optional
@@ -42,12 +41,8 @@ def det_stats(post: torch.Tensor, lengths: Optional[torch.Tensor] = None, step: 
     lens = None if lengths is None else lengths.to(device=post.device, dtype=torch.int32).contiguous()
     max_score = torch.empty(B, K, device=post.device, dtype=torch.float64)
     triggers = torch.empty(B, K, thr.numel(), device=post.device, dtype=torch.int32)
-    with torch.cuda.device(post.device):
-        rc = _native.lib().wekws_det_stats(
-            C.c_void_p(post.data_ptr()), C.c_void_p(lens.data_ptr()) if lens is not None else None, B, T, K,
-            C.c_void_p(d_thr.data_ptr()), thr.numel(), int(window_shift), C.c_void_p(max_score.data_ptr()),
-            C.c_void_p(triggers.data_ptr()), C.c_void_p(torch.cuda.current_stream(post.device).cuda_stream))
-    _native.check(rc, "wekws_det_stats")
+    _native.call("wekws_det_stats", post, lens, B, T, K, d_thr, thr.numel(), int(window_shift), max_score, triggers,
+                 device=post.device)
     return thr, max_score, triggers
 
 
@@ -169,16 +164,11 @@ def context_expansion(feats: torch.Tensor, left: int = 1, right: int = 1, skip_r
         raise ValueError("feats must be a (B, T, D) float32 tensor")
     feats = feats.contiguous()
     B, T, D = feats.shape
-    lib = _native.lib()
-    m = int(lib.wekws_context_expand_frames(T, int(right), int(skip_rate)))
+    m = int(_native.lib().wekws_context_expand_frames(T, int(right), int(skip_rate)))
     out = torch.empty(B, m, D * (left + right + 1), device=feats.device, dtype=torch.float32)
     lens = None if lengths is None else lengths.to(device=feats.device, dtype=torch.int32).contiguous()
-    with torch.cuda.device(feats.device):
-        rc = lib.wekws_context_expand(
-            C.c_void_p(feats.data_ptr()), C.c_void_p(lens.data_ptr()) if lens is not None else None, B, T, D, int(left),
-            int(right), int(skip_rate), C.c_void_p(out.data_ptr()), m,
-            C.c_void_p(torch.cuda.current_stream(feats.device).cuda_stream))
-    _native.check(rc, "wekws_context_expand")
+    _native.call("wekws_context_expand", feats, lens, B, T, D, int(left), int(right), int(skip_rate), out, m,
+                 device=feats.device)
     n = torch.full((B,), T, dtype=torch.int64) if lengths is None else lengths.detach().cpu().to(torch.int64)
     new_len = torch.where(n > right, (n - right + skip_rate - 1) // skip_rate, torch.zeros_like(n)).to(torch.int32)
     return out, new_len

@@ -18,12 +18,10 @@ its samples and returns ``{}`` until the buffer is long enough.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Iterable, List, Optional, Sequence
 
 import numpy as np
 import torch
-import torch.nn as nn
 
 from . import _native
 from .ctc import SPOT_RESULT_DTYPE, CtcSpotDecoder, check_spot_args
@@ -119,16 +117,6 @@ class SpotResult:
         return self._x[int(self._dst[b]):int(self._dst[b]) + n] if n else torch.zeros(0, 0)
 
 
-def _cache_layout(model):
-    """(shape for B streams as a function of B, batch dimension) of the model's streaming cache."""
-    bb = model.backbone
-    if isinstance(bb, nn.GRU):
-        return (lambda B: (bb.num_layers, B, model.hdim)), 1
-    if getattr(bb, "kind", None) == "fsmn":
-        return (lambda B: (B, bb.proj_dim, bb.cache_len, bb.fsmn_layers)), 0
-    return (lambda B: (B, model.hdim, bb.padding)), 0
-
-
 class KeywordSpotter:
     """``KeyWordSpotter`` (stream_kws_ctc.py:218-529) for `num_streams` independent streams, one call per chunk.
 
@@ -172,8 +160,7 @@ class KeywordSpotter:
         self.decoder = CtcSpotDecoder(self.B, keywords, score_beam_size, path_beam_size, self.skip, threshold,
                                       min_frames, max_frames, interval_frames, self.dev)
         self.words = self.decoder.words
-        self._cache_shape, self._bdim = _cache_layout(model)
-        self.cache = torch.zeros(self._cache_shape(self.B), dtype=torch.float32, device=self.dev)
+        self.cache = torch.zeros(model.cache_shape(self.B), dtype=torch.float32, device=self.dev)
         self.pcm_rem = torch.zeros(self.B, (self.mirror.rem_capacity + 7) // 8 * 8, dtype=torch.int16, device=self.dev)
         self.feat_rem = torch.zeros(self.B, max(left + right, 1), D, dtype=torch.float32, device=self.dev)
         self._table = torch.zeros(9, self.B, dtype=torch.int32).pin_memory()
@@ -205,27 +192,25 @@ class KeywordSpotter:
         if idx is None:
             self.cache.zero_()
         elif idx:
-            self.cache.index_fill_(self._bdim, torch.tensor(idx, dtype=torch.int64, device=self.dev), 0.0)
+            self.cache.index_fill_(self.model.cache_batch_dim, torch.tensor(idx, dtype=torch.int64, device=self.dev),
+                                   0.0)
 
     def _forward_group(self, x, out, idx, T):
         """The model over the streams `idx` (host list, ascending) with T frames each, softmax fused, cache in place."""
         m = self.model
         if m.training:
             raise RuntimeError("wekws_b200.KWSModel is inference-only: call model.eval() first")
-        h = m._ensure(self.dev)
-        m._apply_precision(h)
+        h = m._prepare(self.dev)
         n = len(idx)
         whole = n == self.B
         if whole:
             cache = self.cache
         else:
             sel = torch.tensor(idx, dtype=torch.int64, device=self.dev)
-            cache = self.cache.index_select(self._bdim, sel)
-        rc = _native.lib().wekws_model_forward(h, x.data_ptr(), cache.data_ptr(), out.data_ptr(), cache.data_ptr(), n, T,
-                                               _native.FWD_SOFTMAX, torch.cuda.current_stream(self.dev).cuda_stream)
-        _native.check(rc, "wekws_model_forward")
+            cache = self.cache.index_select(m.cache_batch_dim, sel)
+        _native.call("wekws_model_forward", h, x, cache, out, cache, n, T, _native.FWD_SOFTMAX, device=self.dev)
         if not whole:
-            self.cache.index_copy_(self._bdim, sel, cache)
+            self.cache.index_copy_(m.cache_batch_dim, sel, cache)
 
     def __call__(self, pcm: torch.Tensor, lengths=None) -> SpotResult:
         """pcm (B, N) int16 CUDA: one chunk per stream; lengths: host ints 0..N (None = N for every stream)."""
@@ -265,34 +250,25 @@ class KeywordSpotter:
         d = self._table.to(self.dev, non_blocking=True)
         self._table_sent = torch.cuda.Event()
         self._table_sent.record(torch.cuda.current_stream(self.dev))
-        lib, stream = _native.lib(), torch.cuda.current_stream(self.dev).cuda_stream
         S = (self.pcm_rem.size(1) + N + 7) // 8 * 8
         stage = torch.empty(self.B, S, dtype=torch.int16, device=self.dev)
-
-        def p(t):
-            return C.c_void_p(t.data_ptr())
-
-        with torch.cuda.device(self.dev):
-            _native.check(lib.wekws_stream_pcm(p(pcm), pcm.stride(0), self.B, p(d[0]), p(d[1]), p(d[2]),
-                                               p(self.pcm_rem), self.pcm_rem.size(1), p(stage), S, C.c_void_p(stream)),
-                          "wekws_stream_pcm")
-            Fmax = int(nfeat.max()) if self.B else 0
-            feats = torch.empty(self.B, Fmax, self.D, dtype=torch.float32, device=self.dev)
-            x = torch.empty(base, self.model.idim, dtype=torch.float32, device=self.dev)
-            raw = np.zeros(self.B, dtype=SPOT_RESULT_DTYPE)
-            if Fmax > 0:
-                _native.check(lib.wekws_fbank_forward(self.frontend._handle(self.dev), p(stage), _native.PCM_S16,
-                                                      self.B, S, S, p(d[3]), None, None, p(feats), Fmax,
-                                                      C.c_void_p(stream)), "wekws_fbank_forward")
-                _native.check(lib.wekws_stream_context(p(feats), Fmax, self.B, self.D, p(d[4]), p(d[5]), p(d[6]),
-                                                       p(d[7]), p(d[8]), self.left, self.right, self.skip,
-                                                       p(self.feat_rem), p(x), C.c_void_p(stream)),
-                              "wekws_stream_context")
-            if base > 0:
-                probs = torch.empty(base, self.model.odim, dtype=torch.float32, device=self.dev)
-                for T, idx, row in groups:
-                    n = len(idx) * T
-                    self._forward_group(x[row:row + n], probs[row:row + n], idx, T)
-                res = self.decoder(probs, d[8], d[7], live=(nout > 0).tolist())
-                raw = res.cpu().numpy().view(SPOT_RESULT_DTYPE).reshape(self.B)
+        _native.call("wekws_stream_pcm", pcm, pcm.stride(0), self.B, d[0], d[1], d[2], self.pcm_rem,
+                     self.pcm_rem.size(1), stage, S, device=self.dev)
+        Fmax = int(nfeat.max()) if self.B else 0
+        feats = torch.empty(self.B, Fmax, self.D, dtype=torch.float32, device=self.dev)
+        x = torch.empty(base, self.model.idim, dtype=torch.float32, device=self.dev)
+        raw = np.zeros(self.B, dtype=SPOT_RESULT_DTYPE)
+        if Fmax > 0:
+            # the int16 stage rows (remainder + chunk) of each stream through the front-end
+            _native.call("wekws_fbank_forward", self.frontend._handle(self.dev), stage, _native.PCM_S16, self.B, S, S,
+                         d[3], None, None, feats, Fmax, device=self.dev)
+            _native.call("wekws_stream_context", feats, Fmax, self.B, self.D, d[4], d[5], d[6], d[7], d[8], self.left,
+                         self.right, self.skip, self.feat_rem, x, device=self.dev)
+        if base > 0:
+            probs = torch.empty(base, self.model.odim, dtype=torch.float32, device=self.dev)
+            for T, idx, row in groups:
+                n = len(idx) * T
+                self._forward_group(x[row:row + n], probs[row:row + n], idx, T)
+            res = self.decoder(probs, d[8], d[7], live=(nout > 0).tolist())
+            raw = res.cpu().numpy().view(SPOT_RESULT_DTYPE).reshape(self.B)
         return SpotResult(self.words, self.resolution, nout, raw, feats, nfeat, x, dst)

@@ -18,7 +18,6 @@ the features already on the device.  Deliberate differences from the reference:
 """
 from __future__ import annotations
 
-import ctypes as C
 import random
 from typing import List, Optional, Sequence
 
@@ -87,11 +86,8 @@ def _apply_spec_aug(feats: torch.Tensor, frames: List[int], masks: List[List[int
     dev = feats.device
     with torch.cuda.device(dev):
         d_table = table.to(dev, non_blocking=True)
-        rc = _native.lib().wekws_spec_aug(
-            C.c_void_p(feats.data_ptr()), C.c_void_p(d_table.data_ptr()), B, T, D,
-            C.c_void_p(d_table.data_ptr() + 4 * B), int(num_t_mask), int(num_f_mask),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    _native.check(rc, "wekws_spec_aug")
+    _native.call("wekws_spec_aug", feats, d_table, B, T, D, d_table.data_ptr() + 4 * B, int(num_t_mask),
+                 int(num_f_mask), device=dev)
     return feats
 
 
@@ -197,14 +193,11 @@ class TrainFeatures:
         strings.  Returns {keys, feats, target, feats_lengths, target_lengths} in padding()'s order (longest first):
         feats (B, T, D) float32 on pcm's device, the rest host tensors as padding() makes them.  ``rng`` makes the
         augmentation draws and the SpecAugment masks (see ``draw``), ``generator`` the dither seed."""
-        if not pcm.is_cuda:
-            raise RuntimeError("wekws_b200.TrainFeatures runs on CUDA (sm_90a) only; got a CPU tensor")
-        if pcm.dim() != 2:
-            raise ValueError("pcm must be (B, N)")
+        pcm, _, _ = _native.pcm_rows(pcm, "TrainFeatures", one_d=False)
         B, N = pcm.shape
-        lens = [int(n) for n in (lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)]
-        if len(lens) != B or any(n < 0 or n > N for n in lens) or len(labels) != B or len(keys) != B:
-            raise ValueError(f"lengths, labels and keys must have {B} entries, lengths in 0..{N}")
+        lens = _native.host_lengths(lengths, B, N)
+        if len(labels) != B or len(keys) != B:
+            raise ValueError(f"labels and keys must have {B} entries")
         dev = pcm.device
         wave = pcm
         if int(sample_rate) != self.resample_rate:
@@ -218,8 +211,6 @@ class TrainFeatures:
         if self.reverb_source is not None or self.noise_source is not None:
             draws = self.draw(lens, rng)
             owned = int(sample_rate) != self.resample_rate          # wave is the resampler's buffer, not the caller's
-            if wave.stride(1) != 1:
-                wave, owned = wave.contiguous(), True
             if any(p is not None for p in draws["reverb"]):
                 wave, owned = launch_reverb(wave, lens, draws["reverb"], self.reverb_source), True
             if any(p is not None for p in draws["noise"]):
