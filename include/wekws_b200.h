@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 11  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise */
+#define WEKWS_B200_ABI_VERSION 12  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -418,6 +418,48 @@ WEKWS_API int wekws_criterion_ctc(const float* d_logits, const int32_t* d_lens, 
                         const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len,
                         int validation, void* d_workspace, float* d_loss, double* d_acc, float* d_utt_loss,
                         int32_t* d_correct, int32_t* d_overflow, int32_t* d_best, void* stream);
+
+/* The training step of wekws/utils/executor.py Executor.train (criterion(...), then loss.backward()): the gradient
+ * of each criterion's loss with respect to its logits, the one torch's autograd gives for loss.py.
+ *
+ * wekws_criterion_*_train run the forward above (same arguments, outputs, workspace and launches) and also keep what
+ * the gradient needs: max_pooling d_pooled (B,D), the pooled value of every (utterance, column); ce d_count (one
+ * float), the number of counted rows; ctc d_utt_loss (B, required here), d_row_max and d_row_sum (B*T each: the
+ * softmax normaliser of every frame t < lens[b]) and d_alpha (B, T, 2 * max_label_len + 1: alpha of every frame and
+ * extended-label state of each utterance; the rest is not written).
+ *
+ * wekws_criterion_*_backward write d_grad, every element of a tensor shaped like d_logits, = *d_upstream (one float
+ * in device memory: d loss_total / d loss) times d loss / d logits.  No atomics: equal inputs give equal bits.
+ *   max_pooling: per (utterance, column) term -1 / (pooled * B) at the pooled frame of the keyword column and
+ *     +1 / (pooled * B) for the others, split evenly over the frames whose masked, clamped value equals the pooled
+ *     value; a tie that is masked (padding, the first min_duration frames of the keyword column) or outside the
+ *     clamp's closed interval [1e-8, 1] counts in the split and gets zero.  1 launch.
+ *   ce: (softmax - onehot) / count on counted rows, zero on ignored rows.  1 launch.
+ *   ctc: (softmax - occupancy) / B on frames t < lens[b] of a feasible utterance, NaN on those of an infeasible one
+ *     (d_utt_loss[b] = +inf), zero on frames t >= lens[b].  The first call (alpha_is_occupancy == 0) overwrites
+ *     d_alpha with the state occupancies (beta recurrence, 2 launches); a later call on the same forward passes
+ *     alpha_is_occupancy != 0 and reuses them (1 launch).  The logits are read once by the gradient kernel and the
+ *     gradient is written once; nothing else of B*T*V elements exists.                                            */
+WEKWS_API int wekws_criterion_max_pooling_train(const float* d_logits, const int32_t* d_target, const int32_t* d_lens,
+                                int64_t B, int64_t T, int D, int min_duration, void* d_workspace, float* d_loss,
+                                double* d_acc, float* d_term_loss, int32_t* d_correct, float* d_pooled, void* stream);
+WEKWS_API int wekws_criterion_max_pooling_backward(const float* d_logits, const int32_t* d_target,
+                                const int32_t* d_lens, int64_t B, int64_t T, int D, int min_duration,
+                                const float* d_pooled, const float* d_upstream, float* d_grad, void* stream);
+WEKWS_API int wekws_criterion_ce_train(const float* d_logits, const int32_t* d_target, int64_t B, int C,
+                       void* d_workspace, float* d_loss, double* d_acc, float* d_utt_loss, int32_t* d_correct,
+                       float* d_count, void* stream);
+WEKWS_API int wekws_criterion_ce_backward(const float* d_logits, const int32_t* d_target, int64_t B, int C,
+                       const float* d_count, const float* d_upstream, float* d_grad, void* stream);
+WEKWS_API int wekws_criterion_ctc_train(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                        const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len,
+                        int validation, void* d_workspace, float* d_loss, double* d_acc, float* d_utt_loss,
+                        int32_t* d_correct, int32_t* d_overflow, int32_t* d_best, float* d_row_max, float* d_row_sum,
+                        float* d_alpha, void* stream);
+WEKWS_API int wekws_criterion_ctc_backward(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                        const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len,
+                        const float* d_row_max, const float* d_row_sum, const float* d_utt_loss, float* d_alpha,
+                        int alpha_is_occupancy, const float* d_upstream, float* d_grad, void* stream);
 
 /* Resampling: torchaudio.transforms.Resample(orig_freq, new_freq) with sinc_interp_hann (the resampling of
  * wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py:50-53), for B waveforms of their own lengths.

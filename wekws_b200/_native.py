@@ -23,7 +23,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 # limits (include/wekws_b200.h #defines)
 CTC_MAX_PREFIX, CTC_MAX_PATH_BEAM, CTC_MAX_SCORE_BEAM = 64, 20, 3
@@ -124,6 +124,22 @@ SIGNATURES = {
     "wekws_criterion_ctc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
                                       C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_criterion_max_pooling_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int,
+                                                    C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p]),
+    "wekws_criterion_max_pooling_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int,
+                                                       C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_criterion_ce_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_criterion_ce_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]),
+    "wekws_criterion_ctc_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                            C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
+    "wekws_criterion_ctc_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                               C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wekws_pipeline_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64,
                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_uint32, C.c_void_p]),

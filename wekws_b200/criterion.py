@@ -10,6 +10,11 @@ reference's own ``Executor.cv`` / ``Executor.test`` evaluate a set with it.  The
 * ``ctc`` (loss.py:102-164): ``F.ctc_loss(log_softmax, ..., blank=0, reduction='sum') / B`` (+inf for an infeasible
   utterance, as ``zero_infinity=False`` gives) and, with ``validation=True``, ``acc_utterance``: prefix beam search
   (score beam 3, path beam 5) on the softmax and the word accuracy of the best hypothesis against the label.
+
+Training (``Executor.train``): when ``logits.requires_grad`` and grad mode is on, the returned loss is attached to
+the graph, and ``loss.backward()`` delivers ``d loss / d logits`` -- the gradient torch's autograd gives for
+``loss.py``, computed by the backward kernels of csrc/criterion.cu -- as a float32 tensor of the logits' shape.
+Otherwise the forward-only entry points run, exactly as before.  Double backward is not supported.
 """
 from __future__ import annotations
 
@@ -17,6 +22,7 @@ import math
 import sys
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _native
 from ._native import CRITERION_MAX_LABEL as MAX_LABEL
@@ -57,6 +63,90 @@ def _ints(name, t, x, dim=1, size=None):
     return t
 
 
+def _wants_grad(logits):
+    return torch.is_grad_enabled() and logits.requires_grad
+
+
+def _upstream(g, x):
+    """The gradient arriving at the loss: the kernels read one float32 from device memory."""
+    if g.dim() != 0 or g.dtype != torch.float32 or g.device != x.device:
+        raise ValueError(f"criterion: the loss is a 0-dim float32 tensor on {x.device}; its upstream gradient must "
+                         f"be one too, got {tuple(g.shape)} {g.dtype} on {g.device}")
+    return g.contiguous()
+
+
+class _MaxPoolingLoss(torch.autograd.Function):
+    """The loss of wekws_criterion_max_pooling_train; ``args`` are the forward entry point's, from B to d_correct."""
+
+    @staticmethod
+    def forward(ctx, x, tgt, lens, *args):
+        B, T, D, min_duration = args[:4]
+        pooled = torch.empty(B, D, dtype=torch.float32, device=x.device)
+        loss = torch.empty_like(args[5])
+        _native.call("wekws_criterion_max_pooling_train", x, tgt, lens, *args[:5], loss, *args[6:], pooled,
+                     device=x.device)
+        ctx.save_for_backward(x, tgt, lens, pooled)
+        ctx.min_duration = min_duration
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, tgt, lens, pooled = ctx.saved_tensors
+        grad = torch.empty_like(x)
+        _native.call("wekws_criterion_max_pooling_backward", x, tgt, lens, *x.shape, ctx.min_duration, pooled,
+                     _upstream(g, x), grad, device=x.device)
+        return (grad,) + (None,) * (len(ctx.needs_input_grad) - 1)
+
+
+class _CrossEntropyLoss(torch.autograd.Function):
+    """The loss of wekws_criterion_ce_train; ``args`` are the forward entry point's, from B to d_correct."""
+
+    @staticmethod
+    def forward(ctx, x, tgt, *args):
+        count = torch.empty((), dtype=torch.float32, device=x.device)
+        loss = torch.empty_like(args[3])
+        _native.call("wekws_criterion_ce_train", x, tgt, *args[:3], loss, *args[4:], count, device=x.device)
+        ctx.save_for_backward(x, tgt, count)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, tgt, count = ctx.saved_tensors
+        grad = torch.empty_like(x)
+        _native.call("wekws_criterion_ce_backward", x, tgt, *x.shape, count, _upstream(g, x), grad, device=x.device)
+        return (grad,) + (None,) * (len(ctx.needs_input_grad) - 1)
+
+
+class _CtcLoss(torch.autograd.Function):
+    """The loss of wekws_criterion_ctc_train; ``args`` are the forward entry point's, from B to d_best.  Keeps alpha
+    (B, T, 2 Lmax + 1), which the first backward turns into the state occupancies in place."""
+
+    @staticmethod
+    def forward(ctx, x, lens, *args):
+        B, T, V, lab, stride, tls, max_label = args[:7]
+        utt, loss = args[11], torch.empty_like(args[9])
+        row_max = torch.empty(B, T, dtype=torch.float32, device=x.device)
+        row_sum = torch.empty(B, T, dtype=torch.float32, device=x.device)
+        alpha = torch.empty(B, T, 2 * max_label + 1, dtype=torch.float32, device=x.device)
+        _native.call("wekws_criterion_ctc_train", x, lens, *args[:9], loss, *args[10:], row_max, row_sum, alpha,
+                     device=x.device)
+        ctx.save_for_backward(x, lens, lab, tls, row_max, row_sum, utt)
+        ctx.alpha, ctx.stride, ctx.max_label, ctx.occupancy = alpha, stride, max_label, False
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, lens, lab, tls, row_max, row_sum, utt = ctx.saved_tensors
+        grad = torch.empty_like(x)
+        _native.call("wekws_criterion_ctc_backward", x, lens, *x.shape, lab, ctx.stride, tls, ctx.max_label, row_max,
+                     row_sum, utt, ctx.alpha, int(ctx.occupancy), _upstream(g, x), grad, device=x.device)
+        ctx.occupancy = True
+        return (grad,) + (None,) * (len(ctx.needs_input_grad) - 1)
+
+
 def max_pooling_loss(logits, target, lengths, min_duration=0, terms=False):
     """loss.py:26-88.  logits (B, T, D) posteriors, target (B,) (< 0 = filler), lengths (B,) with max == T.
     terms=True also returns {'term': (B, D) losses, 'correct': (B,) 0/1}."""
@@ -78,8 +168,11 @@ def max_pooling_loss(logits, target, lengths, min_duration=0, terms=False):
     acc = torch.empty(1, dtype=torch.float64, device=x.device)
     out = dict(term=torch.empty(B, D, dtype=torch.float32, device=x.device),
                correct=torch.empty(B, dtype=torch.int32, device=x.device)) if terms else {}
-    _native.call("wekws_criterion_max_pooling", x, tgt, lens, B, T, D, int(min_duration), ws, loss, acc,
-                 out.get("term"), out.get("correct"), device=x.device)
+    args = (x, tgt, lens, B, T, D, int(min_duration), ws, loss, acc, out.get("term"), out.get("correct"))
+    if _wants_grad(x):
+        loss = _MaxPoolingLoss.apply(*args)
+    else:
+        _native.call("wekws_criterion_max_pooling", *args, device=x.device)
     return loss, float(acc.item()), out
 
 
@@ -98,8 +191,11 @@ def cross_entropy(logits, target, terms=False):
     acc = torch.empty(1, dtype=torch.float64, device=x.device)
     out = dict(term=torch.empty(B, dtype=torch.float32, device=x.device),
                correct=torch.empty(B, dtype=torch.int32, device=x.device)) if terms else {}
-    _native.call("wekws_criterion_ce", x, tgt, B, Cn, ws, loss, acc, out.get("term"), out.get("correct"),
-                 device=x.device)
+    args = (x, tgt, B, Cn, ws, loss, acc, out.get("term"), out.get("correct"))
+    if _wants_grad(x):
+        loss = _CrossEntropyLoss.apply(*args)
+    else:
+        _native.call("wekws_criterion_ce", *args, device=x.device)
     return loss, float(acc.item()), out
 
 
@@ -152,8 +248,13 @@ def ctc_loss(logits, target, lengths, target_lengths, validation=False, terms=Fa
             out["correct"] = torch.empty(B, dtype=torch.int32, device=dev)
             out["best"] = torch.empty(B, 1 + MAX_PREFIX, dtype=torch.int32, device=dev)
     stride = n_lab if target.dim() == 2 else 0
-    _native.call("wekws_criterion_ctc", x, lens, B, T, V, lab, stride, tls, int(tl_h.max()), int(bool(validation)), ws,
-                 loss, acc, out.get("term"), out.get("correct"), overflow, out.get("best"), device=dev)
+    args = (x, lens, B, T, V, lab, stride, tls, int(tl_h.max()), int(bool(validation)), ws, loss, acc,
+            out.get("term"), out.get("correct"), overflow, out.get("best"))
+    if _wants_grad(x):                                    # the backward needs the per-utterance losses
+        utt = out["term"] if terms else torch.empty(B, dtype=torch.float32, device=dev)
+        loss = _CtcLoss.apply(*args[:13], utt, *args[14:])
+    else:
+        _native.call("wekws_criterion_ctc", *args, device=dev)
     if not validation:
         return loss, 0.0, out
     res = torch.cat([acc, overflow.to(torch.float64)]).cpu()

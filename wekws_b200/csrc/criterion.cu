@@ -11,6 +11,18 @@
 //     it is the edit distance and `all` is the label length: the accuracy needs the distance only.
 //   * criterion_reduce_kernel (one thread) folds the per-term values in a fixed order and writes loss and accuracy.
 // NaN propagates as in torch (max / min / clamp / argmax keep it), which fmaxf / fminf would not.
+//
+// Training (Executor.train: loss.backward()): the *_train entry points run the same forward and keep what the
+// gradient needs (max_pooling: the pooled values; ce: the counted rows; ctc: alpha, (B, T, 2 Lmax + 1)), and the
+// *_backward entry points write d loss / d logits, every element of it, as upstream * (unit gradient), the gradient
+// torch's autograd gives for loss.py:
+//   * max_pooling: the pooled frame gets -1 / (p B) (keyword column) or +1 / ((1 - p) B) (others), split evenly over
+//     the positions that tie after masked_fill and clamp; masked ties and ties outside the clamp's closed interval
+//     count in the split and receive nothing.
+//   * ce: (softmax - onehot) / count on the counted rows.
+//   * ctc: (softmax - occupancy) / B on the frames of a feasible utterance, NaN on those of an infeasible one, zero
+//     on padding.  ctc_beta_kernel turns alpha into occupancies in place (one owner state per token, so the gradient
+//     kernel needs no atomics), ctc_grad_kernel streams the logits once and the gradient once.
 #include <math.h>
 
 #include "common.cuh"
@@ -41,9 +53,12 @@ __device__ __forceinline__ bool argmax_wins(float v, int i, float bv, int bi) {
 
 // max_pooling_loss (loss.py:44-87).  term[b][j]: -log(max) of the keyword column j == target, -log(min(1 - p)) of the
 // others; correct[b]: the accuracy rule on the masked max over T then the first-index max over D.
+// kTrain: pooled[b][j] keeps the pooled value for max_pool_grad_kernel.
+template <bool kTrain>
 __global__ void max_pool_kernel(const float* __restrict__ x, const int32_t* __restrict__ target,
                                 const int32_t* __restrict__ lens, int T, int D, int min_duration,
-                                float* __restrict__ term, int32_t* __restrict__ correct) {
+                                float* __restrict__ term, int32_t* __restrict__ correct,
+                                float* __restrict__ pooled) {
   extern __shared__ float colmax[];              // (D) masked max over T of each column
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   const long long b = blockIdx.x;
@@ -66,6 +81,7 @@ __global__ void max_pool_kernel(const float* __restrict__ x, const int32_t* __re
     }
     if (lane == 0) {
       term[b * D + j] = -logf(pool);
+      if constexpr (kTrain) pooled[b * D + j] = pool;
       colmax[j] = cmax;
     }
   }
@@ -135,11 +151,13 @@ __device__ __forceinline__ const int32_t* label_of(const int32_t* labels, long l
 // F.ctc_loss of one utterance (blank 0, zero_infinity=False): torch's CPU recurrence (LossCTC.cpp), in float32.
 // Thread s is extended-label state s of l' = (blank, l1, blank, l2, ..., blank); alpha is double-buffered in shared
 // memory with one barrier per frame, and frame t + 1's log-probability is gathered before that barrier.
+// kTrain: alpha[t][s] of the utterance's frames and states is also stored, (B, T, alpha_stride), for ctc_beta_kernel.
+template <bool kTrain>
 __global__ void ctc_alpha_kernel(const float* __restrict__ x, const float* __restrict__ row_max,
                                  const float* __restrict__ row_sum, const int32_t* __restrict__ lens,
                                  const int32_t* __restrict__ labels, long long label_stride,
                                  const int32_t* __restrict__ label_lens, long long T, int V,
-                                 float* __restrict__ utt_loss) {
+                                 float* __restrict__ utt_loss, float* __restrict__ alpha_out, int alpha_stride) {
   extern __shared__ float alpha[];               // [2][blockDim.x]
   const int s = threadIdx.x, ns = blockDim.x;
   const long long b = blockIdx.x;
@@ -160,6 +178,11 @@ __global__ void ctc_alpha_kernel(const float* __restrict__ x, const float* __res
   float* cur = alpha;
   float* nxt = alpha + ns;
   cur[s] = (s == 0 || (s == 1 && L > 0)) ? log_prob(0) : -INFINITY;
+  float* ab = nullptr;
+  if constexpr (kTrain) {
+    ab = alpha_out + b * T * alpha_stride + s;
+    if (active) ab[0] = cur[s];
+  }
   float lp = (active && n > 1) ? log_prob(1) : 0.f;
   __syncthreads();
   for (int t = 1; t < n; ++t) {
@@ -172,6 +195,7 @@ __global__ void ctc_alpha_kernel(const float* __restrict__ x, const float* __res
       if (la3 > lamax) lamax = la3;
       if (lamax == -INFINITY) lamax = 0.f;       // cannot do -inf - -inf
       nxt[s] = logf(expf(la1 - lamax) + expf(la2 - lamax) + expf(la3 - lamax)) + lamax + lp;
+      if constexpr (kTrain) ab[(long long)t * alpha_stride] = nxt[s];
       if (t + 1 < n) lp = log_prob(t + 1);
     }
     float* tmp = cur;
@@ -191,6 +215,228 @@ __global__ void ctc_alpha_kernel(const float* __restrict__ x, const float* __res
     }
     utt_loss[b] = nll;
   }
+}
+
+// ---------------------------------------------------------------------------------------------- gradients
+// out[i] = f(p[i]) for the n floats of one row across a warp.  Rows of V floats start on any 4-byte boundary (V =
+// 2599), so the 16-byte accesses start at the first aligned element of `out`; `p` must be aligned alike, or the row
+// goes one float at a time.
+// kRead = false fills the row with f(0) and never touches `p`.
+template <bool kRead = true, class F>
+__device__ __forceinline__ void warp_row_map(const float* __restrict__ p, float* __restrict__ out, int n, int lane,
+                                             F f) {
+  int head = (int)(((16 - (reinterpret_cast<uintptr_t>(out) & 15)) & 15) >> 2);
+  head = head < n ? head : n;
+  auto at = [&](int i) { return kRead ? p[i] : 0.f; };
+  if (kRead && (reinterpret_cast<uintptr_t>(p + head) & 15)) {
+    for (int i = lane; i < n; i += 32) out[i] = f(at(i));
+    return;
+  }
+  if (lane < head) out[lane] = f(at(lane));
+  const int nv = (n - head) >> 2;
+  const float4* p4 = reinterpret_cast<const float4*>(p + head);
+  float4* o4 = reinterpret_cast<float4*>(out + head);
+#pragma unroll 4
+  for (int i = lane; i < nv; i += 32) {
+    const float4 v = kRead ? __ldg(p4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+    o4[i] = make_float4(f(v.x), f(v.y), f(v.z), f(v.w));
+  }
+  const int done = head + 4 * nv;
+  if (done + lane < n) out[done + lane] = f(at(done + lane));
+}
+
+// d max_pooling_loss / d logits, one CTA per utterance and one warp per column like max_pool_kernel.  Pass 1 counts
+// the positions whose masked, clamped value equals the pooled value (torch's max() / min() backward splits the
+// gradient evenly over them; a NaN pooled value ties with the NaNs).  Pass 2 writes every element of the column: the
+// share where the position ties, is not masked and lies in the clamp's closed interval [1e-8, 1], zero elsewhere.
+__global__ void max_pool_grad_kernel(const float* __restrict__ x, const int32_t* __restrict__ target,
+                                     const int32_t* __restrict__ lens, int T, int D, int min_duration,
+                                     const float* __restrict__ pooled, const float* __restrict__ upstream,
+                                     float* __restrict__ grad) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const long long b = blockIdx.x;
+  const int len = lens[b], tgt = target[b];
+  const float* xb = x + b * (long long)T * D;
+  float* gb = grad + b * (long long)T * D;
+  const float g = *upstream, inv_b = __fdiv_rn(1.f, (float)gridDim.x);
+  for (int j = warp; j < D; j += nw) {
+    const bool kw = j == tgt;
+    const float pool = pooled[b * D + j];
+    const bool pool_nan = pool != pool;
+    // the value the reference pools at frame t, and whether the gradient passes masked_fill and clamp there
+    auto pooled_at = [&](int t, float v, bool& passes) {
+      const bool masked = t >= len || (kw && t < min_duration);
+      const float w = kw ? v : 1.f - v;
+      passes = !masked && w >= 1e-8f && w <= 1.f;
+      return clamp_nan(masked ? (kw ? 0.f : 1.f) : w, 1e-8f, 1.f);
+    };
+    int ties = 0;
+    for (int t = lane; t < T; t += 32) {
+      bool passes;
+      const float c = pooled_at(t, xb[(long long)t * D + j], passes);
+      ties += pool_nan ? c != c : c == pool;
+    }
+    for (int o = 16; o > 0; o >>= 1) ties += __shfl_xor_sync(0xffffffffu, ties, o);
+    // d(-log(pool)) / B over the ties; 1 - p flips the sign for the other columns
+    float share = __fdiv_rn(__fdiv_rn(-inv_b, pool), (float)ties);
+    share = __fmul_rn(g, kw ? share : -share);
+    for (int t = lane; t < T; t += 32) {
+      bool passes;
+      const float c = pooled_at(t, xb[(long long)t * D + j], passes);
+      const bool tie = pool_nan ? c != c : c == pool;
+      gb[(long long)t * D + j] = (tie && passes) ? share : 0.f;
+    }
+  }
+}
+
+// d cross_entropy / d logits, one warp per row: upstream * (softmax - onehot) / count, zeros on an ignored row
+__global__ void ce_grad_kernel(const float* __restrict__ x, const int32_t* __restrict__ target, long long B, int C,
+                               const float* __restrict__ count, const float* __restrict__ upstream,
+                               float* __restrict__ grad) {
+  const long long b = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;
+  const int lane = threadIdx.x & 31;
+  const float* p = x + b * C;
+  float* out = grad + b * C;
+  const int t = target[b];
+  if (t == kIgnoreIndex) {
+    for (int i = lane; i < C; i += 32) out[i] = 0.f;
+    return;
+  }
+  float m, s;
+  warp_row_max_sum(p, C, lane, m, s);
+  const float g = *upstream, rs = __fdiv_rn(1.f, s), rc = __fdiv_rn(1.f, *count);
+  for (int i = lane; i < C; i += 32)
+    out[i] = __fmul_rn(g, __fmul_rn(__fmul_rn(expf(p[i] - m), rs) - (i == t ? 1.f : 0.f), rc));
+}
+
+// Turns alpha[b][t][s] into the state occupancy gamma = exp(alpha + beta - log p + nll) in place: one CTA per
+// utterance, thread s is state s, t walks down in torch's log-space beta recurrence (LossCTC.cpp), beta
+// double-buffered in shared memory with one barrier per frame like ctc_alpha_kernel.  Label states that carry the
+// same token are merged here, so that ctc_grad_kernel has one writer per token column: the first state of a token
+// gets the sum of its occupancies (in label order) and the others -1.  Blank states, and label states whose token is
+// the blank, stay as they are (ctc_grad_kernel sums them across a warp).  An infeasible utterance is left alone:
+// its rows are NaN whatever alpha holds.
+__global__ void ctc_beta_kernel(const float* __restrict__ x, const float* __restrict__ row_max,
+                                const float* __restrict__ row_sum, const int32_t* __restrict__ lens,
+                                const int32_t* __restrict__ labels, long long label_stride,
+                                const int32_t* __restrict__ label_lens, long long T, int V,
+                                const float* __restrict__ utt_loss, float* __restrict__ occ, int occ_stride) {
+  extern __shared__ float beta[];                // [2][blockDim.x], gamma [2][blockDim.x], next state [blockDim.x]
+  const int s = threadIdx.x, ns = blockDim.x;
+  float* gam = beta + 2 * ns;
+  int* nexts = reinterpret_cast<int*>(gam + 2 * ns);
+  const long long b = blockIdx.x;
+  const int n = lens[b], L = label_lens[b], S = 2 * L + 1;
+  const float nll = utt_loss[b];
+  if (n == 0 || nll == INFINITY) return;
+  const int32_t* lab = label_of(labels, label_stride, label_lens, b);
+  const bool active = s < S;
+  const int tok = (active && (s & 1)) ? lab[s >> 1] : 0;
+  const bool skip = active && (s & 1) && s + 2 < S && lab[(s >> 1) + 1] != tok;        // l'_{s+2} != l'_s
+  // label states of one token: `first` owns the column, `next` is the following state of the same token
+  bool first = true;
+  int next = -1;
+  if (tok != 0) {
+    for (int k = 0; k < (s >> 1); ++k) first = first && __ldg(lab + k) != tok;
+    for (int k = L - 1; k > (s >> 1); --k)
+      if (__ldg(lab + k) == tok) next = 2 * k + 1;
+  }
+  nexts[s] = next;                               // read after the first frame's barrier
+  const float* xb = x + b * T * V;
+  const float* mb = row_max + b * T;
+  const float* sb = row_sum + b * T;
+  float* ob = occ + b * T * occ_stride + s;
+  auto log_prob = [&](int t) { return (__ldg(xb + (long long)t * V + tok) - __ldg(mb + t)) - logf(__ldg(sb + t)); };
+
+  float* cur = beta;                             // beta of frame t + 1
+  float* nxt = beta + ns;
+  float lp = active ? log_prob(n - 1) : 0.f;
+  float la = active ? ob[(long long)(n - 1) * occ_stride] : 0.f;
+  for (int t = n - 1; t >= 0; --t) {
+    float* gt = gam + (t & 1) * ns;
+    if (active) {
+      float bt;
+      if (t == n - 1) {
+        bt = (s == 2 * L || s == 2 * L - 1) ? lp : -INFINITY;
+      } else {
+        const float lb1 = cur[s];
+        const float lb2 = s + 1 < S ? cur[s + 1] : -INFINITY;
+        const float lb3 = skip ? cur[s + 2] : -INFINITY;
+        float lbmax = lb1;
+        if (lb2 > lbmax) lbmax = lb2;
+        if (lb3 > lbmax) lbmax = lb3;
+        if (lbmax == -INFINITY) lbmax = 0.f;
+        bt = logf(expf(lb1 - lbmax) + expf(lb2 - lbmax) + expf(lb3 - lbmax)) + lbmax + lp;
+      }
+      nxt[s] = bt;
+      gt[s] = expf(la + bt + nll - lp);
+      if (t > 0) {
+        lp = log_prob(t - 1);
+        la = ob[(long long)(t - 1) * occ_stride];
+      }
+    }
+    float* tmp = cur;
+    cur = nxt;
+    nxt = tmp;
+    __syncthreads();
+    // frame t's occupancies are complete; the next frame writes the other half of gam
+    if (active) {
+      float v = gt[s];
+      if (tok != 0) {
+        if (first) {
+          for (int k = next; k >= 0; k = nexts[k]) v += gt[k];
+        } else {
+          v = -1.f;
+        }
+      }
+      ob[(long long)t * occ_stride] = v;
+    }
+  }
+}
+
+// d ctc_loss / d logits, one warp per (b, t) row; the hot path, bound by HBM: the logits are read once and the
+// gradient is written once.  A frame of a feasible utterance gets upstream * (softmax - occupancy) / B: the warp
+// streams the softmax part, then every token column of the label is rewritten by the one state that owns it
+// (ctc_beta_kernel merged the states of a token) from the logit read again, and the blank column from the sum of the
+// blank occupancies, folded in a fixed order.  Padding rows are zeros; the frames of an infeasible utterance are NaN,
+// as torch's backward gives with zero_infinity=False.
+__global__ void ctc_grad_kernel(const float* __restrict__ x, const int32_t* __restrict__ lens,
+                                const int32_t* __restrict__ labels, long long label_stride,
+                                const int32_t* __restrict__ label_lens, long long B, long long T, int V,
+                                const float* __restrict__ row_max, const float* __restrict__ row_sum,
+                                const float* __restrict__ utt_loss, const float* __restrict__ occ, int occ_stride,
+                                const float* __restrict__ upstream, float* __restrict__ grad) {
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= B * T) return;
+  const int lane = threadIdx.x & 31;
+  const long long b = row / T;
+  const float* p = x + row * V;
+  float* out = grad + row * V;
+  if (row - b * T >= lens[b]) {
+    warp_row_map<false>(nullptr, out, V, lane, [](float) { return 0.f; });
+    return;
+  }
+  if (utt_loss[b] == INFINITY) {
+    warp_row_map<false>(nullptr, out, V, lane, [](float) { return __int_as_float(0x7fc00000); });
+    return;
+  }
+  const float g = *upstream, m = row_max[row], rs = __fdiv_rn(1.f, row_sum[row]), inv_b = __fdiv_rn(1.f, (float)B);
+  auto unit = [&](float v, float gamma) { return __fmul_rn(g, __fmul_rn(__fmul_rn(expf(v - m), rs) - gamma, inv_b)); };
+  warp_row_map(p, out, V, lane, [&](float v) { return unit(v, 0.f); });
+  __syncwarp();
+  const int32_t* lab = label_of(labels, label_stride, label_lens, b);
+  const int S = 2 * label_lens[b] + 1;
+  const float* ob = occ + row * occ_stride;
+  float blank = 0.f;
+  for (int s = lane; s < S; s += 32) {
+    const float gamma = ob[s];
+    const int tok = (s & 1) ? lab[s >> 1] : 0;
+    if (tok == 0) blank += gamma;
+    else if (!(gamma < 0.f)) out[tok] = unit(p[tok], gamma);
+  }
+  for (int o = 16; o > 0; o >>= 1) blank += __shfl_xor_sync(0xffffffffu, blank, o);
+  if (lane == 0) out[0] = unit(p[0], blank);
 }
 
 // Levenshtein distance of the best hypothesis to label b, one warp per utterance: the hypothesis (<= 64 tokens)
@@ -244,10 +490,12 @@ __global__ void ctc_edit_kernel(const int32_t* __restrict__ nhyp, const int32_t*
 //   ce: double sum of the counted terms, as float / count; acc = correct * 100.0 / B (acc_frame);
 //   ctc: double sum of the utterance losses, as float / B; acc = (sum of L - distance) * 100.0 / (sum of L) over the
 //        non-empty labels (acc_utterance), 0 without validation.
+// ce_count (optional, ce): the number of counted rows, which ce_grad_kernel divides by.
 __global__ void criterion_reduce_kernel(int kind, long long B, int D, const float* __restrict__ term,
                                         const int32_t* __restrict__ correct, const int32_t* __restrict__ target,
                                         const int32_t* __restrict__ label_lens, int validation,
-                                        float* __restrict__ loss, double* __restrict__ acc) {
+                                        float* __restrict__ loss, double* __restrict__ acc,
+                                        float* __restrict__ ce_count) {
   if (threadIdx.x != 0) return;
   if (kind == kMaxPooling) {
     float sum = 0.f;
@@ -267,6 +515,7 @@ __global__ void criterion_reduce_kernel(int kind, long long B, int D, const floa
       n += correct[b];
     }
     *loss = __fdiv_rn((float)sum, (float)counted);
+    if (ce_count) *ce_count = (float)counted;
     *acc = __ddiv_rn(__dmul_rn((double)n, 100.0), (double)B);
   } else {
     double sum = 0.0;
@@ -286,8 +535,10 @@ __global__ void criterion_reduce_kernel(int kind, long long B, int D, const floa
 }
 
 int reduce_launch(int kind, long long B, int D, const float* term, const int32_t* correct, const int32_t* target,
-                  const int32_t* label_lens, int validation, float* loss, double* acc, cudaStream_t st) {
-  criterion_reduce_kernel<<<1, 32, 0, st>>>(kind, B, D, term, correct, target, label_lens, validation, loss, acc);
+                  const int32_t* label_lens, int validation, float* loss, double* acc, float* ce_count,
+                  cudaStream_t st) {
+  criterion_reduce_kernel<<<1, 32, 0, st>>>(kind, B, D, term, correct, target, label_lens, validation, loss, acc,
+                                            ce_count);
   return check_launch("criterion_reduce_kernel");
 }
 
@@ -339,10 +590,10 @@ extern "C" int64_t wekws_criterion_max_pooling_workspace_bytes(int64_t B, int D)
   return (int64_t)c.off;
 }
 
-extern "C" int wekws_criterion_max_pooling(const float* d_logits, const int32_t* d_target, const int32_t* d_lens,
-                                           int64_t B, int64_t T, int D, int min_duration, void* d_workspace,
-                                           float* d_loss, double* d_acc, float* d_term_loss, int32_t* d_correct,
-                                           void* stream) {
+// d_pooled != NULL: the training forward
+static int max_pooling_forward(const float* d_logits, const int32_t* d_target, const int32_t* d_lens, int64_t B,
+                               int64_t T, int D, int min_duration, void* d_workspace, float* d_loss, double* d_acc,
+                               float* d_term_loss, int32_t* d_correct, float* d_pooled, cudaStream_t st) {
   WEKWS_REQUIRE(B >= 1 && B < (1ll << 31) && T >= 1 && D >= 1 && D <= 8192,
                 "wekws_criterion_max_pooling: bad sizes (B >= 1, T >= 1, 1 <= D <= 8192)");
   WEKWS_REQUIRE(d_logits && d_target && d_lens && d_workspace && d_loss && d_acc,
@@ -352,13 +603,47 @@ extern "C" int wekws_criterion_max_pooling(const float* d_logits, const int32_t*
   int32_t* correct = c.take<int32_t>(B);
   if (d_term_loss) term = d_term_loss;
   if (d_correct) correct = d_correct;
-  cudaStream_t st = (cudaStream_t)stream;
   const int nw = D < 8 ? D : 8;
-  max_pool_kernel<<<(unsigned)B, nw * 32, (size_t)D * sizeof(float), st>>>(d_logits, d_target, d_lens, (int)T, D,
-                                                                        min_duration, term, correct);
+  if (d_pooled)
+    max_pool_kernel<true><<<(unsigned)B, nw * 32, (size_t)D * sizeof(float), st>>>(d_logits, d_target, d_lens, (int)T, D,
+                                                                                min_duration, term, correct, d_pooled);
+  else
+    max_pool_kernel<false><<<(unsigned)B, nw * 32, (size_t)D * sizeof(float), st>>>(d_logits, d_target, d_lens, (int)T,
+                                                                                 D, min_duration, term, correct, nullptr);
   int rc = check_launch("max_pool_kernel");
   if (rc) return rc;
-  return reduce_launch(kMaxPooling, B, D, term, correct, nullptr, nullptr, 0, d_loss, d_acc, st);
+  return reduce_launch(kMaxPooling, B, D, term, correct, nullptr, nullptr, 0, d_loss, d_acc, nullptr, st);
+}
+
+extern "C" int wekws_criterion_max_pooling(const float* d_logits, const int32_t* d_target, const int32_t* d_lens,
+                                           int64_t B, int64_t T, int D, int min_duration, void* d_workspace,
+                                           float* d_loss, double* d_acc, float* d_term_loss, int32_t* d_correct,
+                                           void* stream) {
+  return max_pooling_forward(d_logits, d_target, d_lens, B, T, D, min_duration, d_workspace, d_loss, d_acc, d_term_loss,
+                             d_correct, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int wekws_criterion_max_pooling_train(const float* d_logits, const int32_t* d_target, const int32_t* d_lens,
+                                                 int64_t B, int64_t T, int D, int min_duration, void* d_workspace,
+                                                 float* d_loss, double* d_acc, float* d_term_loss, int32_t* d_correct,
+                                                 float* d_pooled, void* stream) {
+  WEKWS_REQUIRE(d_pooled, "wekws_criterion_max_pooling_train: null argument");
+  return max_pooling_forward(d_logits, d_target, d_lens, B, T, D, min_duration, d_workspace, d_loss, d_acc, d_term_loss,
+                             d_correct, d_pooled, (cudaStream_t)stream);
+}
+
+extern "C" int wekws_criterion_max_pooling_backward(const float* d_logits, const int32_t* d_target,
+                                                    const int32_t* d_lens, int64_t B, int64_t T, int D,
+                                                    int min_duration, const float* d_pooled, const float* d_upstream,
+                                                    float* d_grad, void* stream) {
+  WEKWS_REQUIRE(B >= 1 && B < (1ll << 31) && T >= 1 && T < (1ll << 31) && D >= 1 && D <= 8192,
+                "wekws_criterion_max_pooling_backward: bad sizes (B >= 1, T >= 1, 1 <= D <= 8192)");
+  WEKWS_REQUIRE(d_logits && d_target && d_lens && d_pooled && d_upstream && d_grad,
+                "wekws_criterion_max_pooling_backward: null argument");
+  const int nw = D < 8 ? D : 8;
+  max_pool_grad_kernel<<<(unsigned)B, nw * 32, 0, (cudaStream_t)stream>>>(d_logits, d_target, d_lens, (int)T, D,
+                                                                         min_duration, d_pooled, d_upstream, d_grad);
+  return check_launch("max_pool_grad_kernel");
 }
 
 extern "C" int64_t wekws_criterion_ce_workspace_bytes(int64_t B) {
@@ -368,8 +653,8 @@ extern "C" int64_t wekws_criterion_ce_workspace_bytes(int64_t B) {
   return (int64_t)c.off;
 }
 
-extern "C" int wekws_criterion_ce(const float* d_logits, const int32_t* d_target, int64_t B, int C, void* d_workspace,
-                                  float* d_loss, double* d_acc, float* d_utt_loss, int32_t* d_correct, void* stream) {
+static int ce_forward(const float* d_logits, const int32_t* d_target, int64_t B, int C, void* d_workspace, float* d_loss,
+                      double* d_acc, float* d_utt_loss, int32_t* d_correct, float* d_count, cudaStream_t st) {
   WEKWS_REQUIRE(B >= 1 && B < (1ll << 31) && C >= 1, "wekws_criterion_ce: bad sizes (B >= 1, C >= 1)");
   WEKWS_REQUIRE(d_logits && d_target && d_workspace && d_loss && d_acc, "wekws_criterion_ce: null argument");
   Carver c{(uint8_t*)d_workspace};
@@ -377,12 +662,36 @@ extern "C" int wekws_criterion_ce(const float* d_logits, const int32_t* d_target
   int32_t* correct = c.take<int32_t>(B);
   if (d_utt_loss) term = d_utt_loss;
   if (d_correct) correct = d_correct;
-  cudaStream_t st = (cudaStream_t)stream;
   const int wpb = 8;
   ce_kernel<<<(unsigned)((B + wpb - 1) / wpb), wpb * 32, 0, st>>>(d_logits, d_target, B, C, term, correct);
   int rc = check_launch("ce_kernel");
   if (rc) return rc;
-  return reduce_launch(kCe, B, 1, term, correct, d_target, nullptr, 0, d_loss, d_acc, st);
+  return reduce_launch(kCe, B, 1, term, correct, d_target, nullptr, 0, d_loss, d_acc, d_count, st);
+}
+
+extern "C" int wekws_criterion_ce(const float* d_logits, const int32_t* d_target, int64_t B, int C, void* d_workspace,
+                                  float* d_loss, double* d_acc, float* d_utt_loss, int32_t* d_correct, void* stream) {
+  return ce_forward(d_logits, d_target, B, C, d_workspace, d_loss, d_acc, d_utt_loss, d_correct, nullptr,
+                    (cudaStream_t)stream);
+}
+
+extern "C" int wekws_criterion_ce_train(const float* d_logits, const int32_t* d_target, int64_t B, int C,
+                                        void* d_workspace, float* d_loss, double* d_acc, float* d_utt_loss,
+                                        int32_t* d_correct, float* d_count, void* stream) {
+  WEKWS_REQUIRE(d_count, "wekws_criterion_ce_train: null argument");
+  return ce_forward(d_logits, d_target, B, C, d_workspace, d_loss, d_acc, d_utt_loss, d_correct, d_count,
+                    (cudaStream_t)stream);
+}
+
+extern "C" int wekws_criterion_ce_backward(const float* d_logits, const int32_t* d_target, int64_t B, int C,
+                                           const float* d_count, const float* d_upstream, float* d_grad,
+                                           void* stream) {
+  WEKWS_REQUIRE(B >= 1 && B < (1ll << 31) && C >= 1, "wekws_criterion_ce_backward: bad sizes (B >= 1, C >= 1)");
+  WEKWS_REQUIRE(d_logits && d_target && d_count && d_upstream && d_grad, "wekws_criterion_ce_backward: null argument");
+  const int wpb = 8;
+  ce_grad_kernel<<<(unsigned)((B + wpb - 1) / wpb), wpb * 32, 0, (cudaStream_t)stream>>>(d_logits, d_target, B, C,
+                                                                                       d_count, d_upstream, d_grad);
+  return check_launch("ce_grad_kernel");
 }
 
 extern "C" int64_t wekws_criterion_ctc_workspace_bytes(int64_t B, int64_t T, int validation) {
@@ -391,34 +700,49 @@ extern "C" int64_t wekws_criterion_ctc_workspace_bytes(int64_t B, int64_t T, int
   return (int64_t)ctc_work(c, B, T, validation, w);
 }
 
-extern "C" int wekws_criterion_ctc(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
-                                   const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens,
-                                   int max_label_len, int validation, void* d_workspace, float* d_loss, double* d_acc,
-                                   float* d_utt_loss, int32_t* d_correct, int32_t* d_overflow, int32_t* d_best,
-                                   void* stream) {
+static int ctc_check(const char* who, const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                     const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len) {
   WEKWS_REQUIRE(B >= 1 && B < (1ll << 31) && T >= 1 && T < (1ll << 31) && V >= 1 && V <= 32767,
-                "wekws_criterion_ctc: bad sizes (B >= 1, T >= 1, 1 <= V <= 32767)");
+                "%s: bad sizes (B >= 1, T >= 1, 1 <= V <= 32767)", who);
   WEKWS_REQUIRE(max_label_len >= 0 && max_label_len <= WEKWS_CRITERION_MAX_LABEL && label_stride >= 0,
-                "wekws_criterion_ctc: labels of up to %d tokens", WEKWS_CRITERION_MAX_LABEL);
-  WEKWS_REQUIRE(d_logits && d_lens && d_label_lens && (d_labels || max_label_len == 0) && d_workspace && d_loss &&
-                    d_acc && (d_overflow || !validation),
-                "wekws_criterion_ctc: null argument");
+                "%s: labels of up to %d tokens", who, WEKWS_CRITERION_MAX_LABEL);
+  WEKWS_REQUIRE(d_logits && d_lens && d_label_lens && (d_labels || max_label_len == 0), "%s: null argument", who);
+  return WEKWS_OK;
+}
+
+// d_alpha != NULL: the training forward, which keeps the row normalisers in d_row_max / d_row_sum and alpha
+static int ctc_forward(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                       const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len,
+                       int validation, void* d_workspace, float* d_loss, double* d_acc, float* d_utt_loss,
+                       int32_t* d_correct, int32_t* d_overflow, int32_t* d_best, float* d_row_max, float* d_row_sum,
+                       float* d_alpha, cudaStream_t st) {
+  int rc = ctc_check("wekws_criterion_ctc", d_logits, d_lens, B, T, V, d_labels, label_stride, d_label_lens,
+                     max_label_len);
+  if (rc) return rc;
+  WEKWS_REQUIRE(d_workspace && d_loss && d_acc && (d_overflow || !validation), "wekws_criterion_ctc: null argument");
   Carver c{(uint8_t*)d_workspace};
   CtcWork w;
   ctc_work(c, B, T, validation, w);
   if (d_utt_loss) w.utt_loss = d_utt_loss;
   if (d_correct && validation) w.correct = d_correct;
-  cudaStream_t st = (cudaStream_t)stream;
+  if (d_alpha) {
+    w.row_max = d_row_max;
+    w.row_sum = d_row_sum;
+  }
 
   const int wpb = 8;
   const long long rows = B * T;
   ctc_row_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, st>>>(d_logits, d_lens, B, T, V, w.row_max,
                                                                         w.row_sum);
-  int rc = check_launch("ctc_row_kernel");
-  if (rc) return rc;
+  if ((rc = check_launch("ctc_row_kernel"))) return rc;
   const int ns = (2 * max_label_len + 1 + 31) / 32 * 32;
-  ctc_alpha_kernel<<<(unsigned)B, ns, 2 * ns * sizeof(float), st>>>(d_logits, w.row_max, w.row_sum, d_lens, d_labels,
-                                                                  label_stride, d_label_lens, T, V, w.utt_loss);
+  if (d_alpha)
+    ctc_alpha_kernel<true><<<(unsigned)B, ns, 2 * ns * sizeof(float), st>>>(
+        d_logits, w.row_max, w.row_sum, d_lens, d_labels, label_stride, d_label_lens, T, V, w.utt_loss, d_alpha,
+        2 * max_label_len + 1);
+  else
+    ctc_alpha_kernel<false><<<(unsigned)B, ns, 2 * ns * sizeof(float), st>>>(
+        d_logits, w.row_max, w.row_sum, d_lens, d_labels, label_stride, d_label_lens, T, V, w.utt_loss, nullptr, 0);
   if ((rc = check_launch("ctc_alpha_kernel"))) return rc;
   if (validation) {
     CtcArgs a;
@@ -437,5 +761,56 @@ extern "C" int wekws_criterion_ctc(const float* d_logits, const int32_t* d_lens,
     if ((rc = check_launch("ctc_edit_kernel"))) return rc;
   }
   return reduce_launch(kCtc, B, 1, w.utt_loss, validation ? w.correct : nullptr, nullptr, d_label_lens, validation,
-                       d_loss, d_acc, st);
+                       d_loss, d_acc, nullptr, st);
+}
+
+extern "C" int wekws_criterion_ctc(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                                   const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens,
+                                   int max_label_len, int validation, void* d_workspace, float* d_loss, double* d_acc,
+                                   float* d_utt_loss, int32_t* d_correct, int32_t* d_overflow, int32_t* d_best,
+                                   void* stream) {
+  return ctc_forward(d_logits, d_lens, B, T, V, d_labels, label_stride, d_label_lens, max_label_len, validation,
+                     d_workspace, d_loss, d_acc, d_utt_loss, d_correct, d_overflow, d_best, nullptr, nullptr, nullptr,
+                     (cudaStream_t)stream);
+}
+
+extern "C" int wekws_criterion_ctc_train(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                                         const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens,
+                                         int max_label_len, int validation, void* d_workspace, float* d_loss,
+                                         double* d_acc, float* d_utt_loss, int32_t* d_correct, int32_t* d_overflow,
+                                         int32_t* d_best, float* d_row_max, float* d_row_sum, float* d_alpha,
+                                         void* stream) {
+  WEKWS_REQUIRE(d_utt_loss && d_row_max && d_row_sum && d_alpha, "wekws_criterion_ctc_train: null argument");
+  return ctc_forward(d_logits, d_lens, B, T, V, d_labels, label_stride, d_label_lens, max_label_len, validation,
+                     d_workspace, d_loss, d_acc, d_utt_loss, d_correct, d_overflow, d_best, d_row_max, d_row_sum,
+                     d_alpha, (cudaStream_t)stream);
+}
+
+extern "C" int wekws_criterion_ctc_backward(const float* d_logits, const int32_t* d_lens, int64_t B, int64_t T, int V,
+                                            const int32_t* d_labels, int64_t label_stride,
+                                            const int32_t* d_label_lens, int max_label_len, const float* d_row_max,
+                                            const float* d_row_sum, const float* d_utt_loss, float* d_alpha,
+                                            int alpha_is_occupancy, const float* d_upstream, float* d_grad,
+                                            void* stream) {
+  int rc = ctc_check("wekws_criterion_ctc_backward", d_logits, d_lens, B, T, V, d_labels, label_stride, d_label_lens,
+                     max_label_len);
+  if (rc) return rc;
+  WEKWS_REQUIRE(d_row_max && d_row_sum && d_utt_loss && d_alpha && d_upstream && d_grad,
+                "wekws_criterion_ctc_backward: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int stride = 2 * max_label_len + 1;
+  if (!alpha_is_occupancy) {
+    const int ns = (stride + 31) / 32 * 32;
+    ctc_beta_kernel<<<(unsigned)B, ns, 5 * ns * sizeof(float), st>>>(d_logits, d_row_max, d_row_sum, d_lens, d_labels,
+                                                                   label_stride, d_label_lens, T, V, d_utt_loss,
+                                                                   d_alpha, stride);
+    if ((rc = check_launch("ctc_beta_kernel"))) return rc;
+  }
+  const int wpb = 8;
+  const long long rows = B * T;
+  ctc_grad_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, st>>>(d_logits, d_lens, d_labels, label_stride,
+                                                                         d_label_lens, B, T, V, d_row_max, d_row_sum,
+                                                                         d_utt_loss, d_alpha, stride, d_upstream,
+                                                                         d_grad);
+  return check_launch("ctc_grad_kernel");
 }
