@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 12  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward */
+#define WEKWS_B200_ABI_VERSION 13  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training) */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -460,6 +460,37 @@ WEKWS_API int wekws_criterion_ctc_backward(const float* d_logits, const int32_t*
                         const int32_t* d_labels, int64_t label_stride, const int32_t* d_label_lens, int max_label_len,
                         const float* d_row_max, const float* d_row_sum, const float* d_utt_loss, float* d_alpha,
                         int alpha_is_occupancy, const float* d_upstream, float* d_grad, void* stream);
+
+/* Training the FSMN model (wekws/utils/executor.py Executor.train with an fsmn_ctc.yaml model): the training-mode
+ * forward keeps its activations, the backward gives the gradient of every parameter of wekws/model/fsmn.py FSMN.
+ * The handle is an FSMN model made by wekws_model_create / _set_tensor / _finalize, with the identity activation
+ * (every FSMN config).  Parameters and gradients travel as host arrays of wekws_fsmn_num_params(m) = 8 + 5 L device
+ * pointers, in state_dict order (the model's parameters without the CMVN buffers):
+ *   backbone.in_linear1.linear.{weight,bias}, backbone.in_linear2.linear.{weight,bias},
+ *   per layer l: backbone.fsmn.{l}.0.linear.weight, .1.conv_left.weight, .1.conv_right.weight, .2.linear.{weight,bias},
+ *   backbone.out_linear1.linear.{weight,bias}, backbone.out_linear2.linear.{weight,bias}
+ * each contiguous float32 in the parameter's own shape (conv_left.weight is (proj, 1, left_order, 1)).
+ *
+ * wekws_fsmn_load_params: the handle's packed weights from those tensors, on the device (1 launch): the optimiser's
+ *   updates reach the kernels without a host round trip.  The CMVN buffers keep what _finalize packed.
+ * wekws_fsmn_train_forward: wekws_model_forward of B utterances of T frames from empty caches (same launches, same
+ *   d_out / d_out_cache bits), also writing d_saved: wekws_fsmn_train_saved_floats(m, B, T) =
+ *   B * T * (input_affine_dim + linear_dim + L * (2 proj_dim + linear_dim) + output_affine_dim) floats.
+ * wekws_fsmn_backward: from d_feats and d_saved of that forward and d_grad_out = d loss / d out (B, T, odim), writes
+ *   every element of every gradient buffer, with all B * T frames as rows (padding included, as torch does).  Weight
+ *   and bias gradients are summed in 32 fixed row slices, then the slices in order: no atomics, equal inputs give
+ *   equal bits.  d_workspace: wekws_fsmn_backward_workspace_bytes(m, B, T) = 4 * (32 * (number of parameter
+ *   elements) + 2 * B * T * max(input_affine_dim, linear_dim, proj_dim, output_affine_dim)) bytes.
+ *   wekws_fsmn_backward_launches(m) = 8 + 5 L launches.                                                        */
+WEKWS_API int wekws_fsmn_num_params(const wekws_model* m);
+WEKWS_API int wekws_fsmn_load_params(wekws_model* m, const float* const* h_params, int n, void* stream);
+WEKWS_API int64_t wekws_fsmn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_fsmn_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
+                                       float* d_saved, int64_t B, int64_t T, void* stream);
+WEKWS_API int64_t wekws_fsmn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_fsmn_backward_launches(const wekws_model* m);
+WEKWS_API int wekws_fsmn_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_grad_out,
+                                  int64_t B, int64_t T, float* const* h_grads, int n, void* d_workspace, void* stream);
 
 /* Resampling: torchaudio.transforms.Resample(orig_freq, new_freq) with sinc_interp_hann (the resampling of
  * wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py:50-53), for B waveforms of their own lengths.

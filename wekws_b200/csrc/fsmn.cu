@@ -135,7 +135,22 @@ __device__ void gemm_layer(Ring& ring, const float* __restrict__ src, int sp, in
   __syncthreads();                                    // dst complete / ring idle before the caller goes on
 }
 
-__global__ void __launch_bounds__(FN_T, 1) fsmn_kernel(const FsmnArgs a) {
+// training forward: rows [0, rows) of a shared activation buffer (row stride sp, width w) -> saved block `which` of
+// layer l, frame (b0 + s) * save_T + save_t0 + t.  Only reads shared memory: the caller's next writer is behind a barrier.
+__device__ __forceinline__ void save_rows(const FsmnArgs& a, const float* src, int sp, int w, int which, int l, int b0,
+                                          int rows, int T) {
+  const long long M = (long long)a.B * a.save_T;
+  float* dst = a.saved + fsmn_saved_offset(a, M, which, l);
+  for (int idx = threadIdx.x; idx < rows * w; idx += FN_T) {
+    const int r = idx / w, c = idx - r * w;
+    const int s = r / T, t = r - s * T;
+    dst[((long long)(b0 + s) * a.save_T + a.save_t0 + t) * w + c] = src[r * sp + c];
+  }
+}
+
+// SAVE: the training forward -- the same arithmetic, plus stores of every activation the backward needs
+template <bool SAVE>
+__device__ __forceinline__ void fsmn_body(const FsmnArgs& a) {
   extern __shared__ __align__(16) float smem[];
   const int T = a.T, S = a.S;
   const int sp0 = a.sp0, sp1 = a.sp1;
@@ -170,12 +185,15 @@ __global__ void __launch_bounds__(FN_T, 1) fsmn_kernel(const FsmnArgs a) {
     __syncthreads();
     // ---- in_linear1 (no activation), in_linear2 + ReLU                      (fsmn.py:470-472)
     gemm_layer<false>(ring, buf0, sp0, a.idim, a.w + a.o_w_in1, a.w + a.o_b_in1, a.aff_in, a.np_aff_in, buf1, sp1, nullptr, 0);
+    if constexpr (SAVE) save_rows(a, buf1, sp1, a.aff_in, 0, 0, b0, rows, T);
     gemm_layer<true>(ring, buf1, sp1, a.aff_in, a.w + a.o_w_in2, a.w + a.o_b_in2, a.lin, a.np_lin, buf0, sp0, nullptr, 0);
+    if constexpr (SAVE) save_rows(a, buf0, sp0, a.lin, 1, 0, b0, rows, T);
     // ---- FSMN layers
     for (int l = 0; l < L; ++l) {
       const float* wl = a.w + a.o_layers + (size_t)l * a.layer_stride;
       // LinearTransform (no bias): p = W h                                    (fsmn.py:387)
       gemm_layer<false>(ring, buf0, sp0, a.lin, wl + a.lo_wp, nullptr, P, a.np_proj, buf1, sp1, nullptr, 0);
+      if constexpr (SAVE) save_rows(a, buf1, sp1, P, 2, l, b0, rows, T);
       // memory block: taps over cat = [cache | p]; cache read straight from global (fsmn.py:226-248)
       const float* tl = wl + a.lo_taps;        // [lo + ro][P]: left taps then right taps
       for (int idx = tid; idx < rows * P; idx += FN_T) {
@@ -192,6 +210,7 @@ __global__ void __launch_bounds__(FN_T, 1) fsmn_kernel(const FsmnArgs a) {
         mem[r * spm + c] = v;
       }
       __syncthreads();                         // every old-cache read of this layer is done (in-place update is legal)
+      if constexpr (SAVE) save_rows(a, mem, spm, P, 3, l, b0, rows, T);
       // one thread per (stream, channel) row of the cache, positions ascending: position j takes cat[T + j], which for
       // T < pad is the OLD position T + j > j -- read before it is overwritten, so out_cache may alias in_cache
       for (int sc = tid; sc < Sv * P; sc += FN_T) {
@@ -207,12 +226,17 @@ __global__ void __launch_bounds__(FN_T, 1) fsmn_kernel(const FsmnArgs a) {
       }
       // AffineTransform + ReLU                                               (fsmn.py:389-390)
       gemm_layer<true>(ring, mem, spm, P, wl + a.lo_wa, wl + a.lo_ba, a.lin, a.np_lin, buf0, sp0, nullptr, 0);
+      if constexpr (SAVE) save_rows(a, buf0, sp0, a.lin, 4, l, b0, rows, T);
     }
     // ---- out_linear1, out_linear2 (+ activation) -> global                  (fsmn.py:478-479)
     gemm_layer<false>(ring, buf0, sp0, a.lin, a.w + a.o_w_out1, a.w + a.o_b_out1, a.aff_out, a.np_aff_out, buf1, sp1, nullptr, 0);
+    if constexpr (SAVE) save_rows(a, buf1, sp1, a.aff_out, 5, 0, b0, rows, T);
     gemm_layer<false>(ring, buf1, sp1, a.aff_out, a.w + a.o_w_out2, a.w + a.o_b_out2, a.odim, a.np_odim, nullptr, 0, grow, a.act);
   }
 }
+
+__global__ void __launch_bounds__(FN_T, 1) fsmn_kernel(const FsmnArgs a) { fsmn_body<false>(a); }
+__global__ void __launch_bounds__(FN_T, 1) fsmn_train_kernel(const FsmnArgs a) { fsmn_body<true>(a); }
 
 }  // namespace
 
@@ -222,7 +246,10 @@ size_t fsmn_smem_bytes(const FsmnArgs& a) {
 int fsmn_tile_rows() { return ROWS; }
 int fsmn_pass_cols() { return NPASS; }
 
-int fsmn_launch(FsmnArgs a, cudaStream_t st) {
+namespace {
+
+template <bool SAVE>
+int launch(FsmnArgs a, cudaStream_t st) {
   WEKWS_REQUIRE(a.T >= 1 && a.T <= ROWS && a.B >= 1, "fsmn_launch: chunk of %d frames does not fit a %d-row tile", a.T, ROWS);
   a.S = ROWS / a.T;
   if (a.S > a.B) a.S = a.B;
@@ -230,16 +257,27 @@ int fsmn_launch(FsmnArgs a, cudaStream_t st) {
   const size_t smem = fsmn_smem_bytes(a);
   WEKWS_REQUIRE(smem <= 226 * 1024, "fsmn: layer widths need %zu bytes of shared memory (max 226 KB + static)", smem);
   static size_t attr_bytes[64] = {0};                  // per device: the largest dynamic size opted into so far
+  auto kernel = SAVE ? fsmn_train_kernel : fsmn_kernel;
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && attr_bytes[dev] < smem) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(fsmn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    WEKWS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_bytes[dev] = smem;
   }
   const int sms = device_sm_count();
   const int grid = a.n_tiles < sms ? a.n_tiles : sms;
-  fsmn_kernel<<<grid, FN_T, smem, st>>>(a);
-  return check_launch("fsmn_kernel");
+  kernel<<<grid, FN_T, smem, st>>>(a);
+  return check_launch(SAVE ? "fsmn_train_kernel" : "fsmn_kernel");
+}
+
+}  // namespace
+
+int fsmn_launch(FsmnArgs a, cudaStream_t st) { return launch<false>(a, st); }
+
+int fsmn_train_launch(FsmnArgs a, cudaStream_t st) {
+  WEKWS_REQUIRE(a.saved != nullptr && a.save_T >= 1 && a.save_t0 >= 0 && a.save_t0 + a.T <= a.save_T,
+                "fsmn_train_launch: bad saved-activation arguments");
+  return launch<true>(a, st);
 }
 
 }  // namespace wekws

@@ -852,6 +852,123 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
   return WEKWS_OK;
 }
 
+// ------------------------------------------------------------------------------- FSMN training
+namespace {
+
+// the layer widths of an FSMN model's config (the fields the saved-activation and workspace sizes depend on)
+FsmnArgs fsmn_dims(const wekws_model_config& c) {
+  FsmnArgs a{};
+  a.idim = c.idim; a.aff_in = c.fsmn_input_affine_dim; a.lin = c.fsmn_linear_dim; a.proj = c.fsmn_proj_dim;
+  a.aff_out = c.fsmn_output_affine_dim; a.odim = c.odim; a.L = c.num_layers;
+  a.lorder = c.fsmn_left_order; a.rorder = c.fsmn_right_order;
+  return a;
+}
+
+int fsmn_train_check(const wekws_model* m, const char* what) {
+  WEKWS_REQUIRE(m, "%s: null handle", what);
+  WEKWS_REQUIRE(m->cfg.backbone == WEKWS_BACKBONE_FSMN, "%s: training is implemented for the FSMN backbone only", what);
+  if (!m->finalized) { set_error("%s called before wekws_model_finalize", what); return WEKWS_ERR_STATE; }
+  WEKWS_REQUIRE(m->cfg.activation == WEKWS_ACT_IDENTITY, "%s: the FSMN model trains with the identity activation", what);
+  int dev = 0;
+  WEKWS_CUDA_OK(cudaGetDevice(&dev));
+  WEKWS_REQUIRE(dev == m->device, "model was finalized on device %d but current device is %d", m->device, dev);
+  return WEKWS_OK;
+}
+
+}  // namespace
+
+extern "C" int wekws_fsmn_num_params(const wekws_model* m) {
+  if (!m || m->cfg.backbone != WEKWS_BACKBONE_FSMN) return 0;
+  return 8 + 5 * m->cfg.num_layers;
+}
+
+extern "C" int wekws_fsmn_load_params(wekws_model* m, const float* const* h_params, int n, void* stream) {
+  int rc = fsmn_train_check(m, "wekws_fsmn_load_params");
+  if (rc) return rc;
+  const FsmnArgs& a = m->fsmn;
+  WEKWS_REQUIRE(h_params && n == 8 + 5 * a.L, "wekws_fsmn_load_params: expected the %d parameters of a %d-layer FSMN, got %d",
+                8 + 5 * a.L, a.L, n);
+  FsmnPackArgs p{};
+  p.packed = m->d_vec;
+  p.n = n;
+  int k = 0;                                   // the parameters in state_dict order, each into its place in the pack
+  auto put = [&](int rows, int cols, long long dst, int ld) {
+    FsmnParamCopy& c = p.p[k];
+    c.src = h_params[k]; c.dst = dst; c.rows = rows; c.cols = cols; c.ld = ld;
+    ++k;
+  };
+  const int D = a.lin, P = a.proj;
+  put(a.aff_in, a.idim, a.o_w_in1, a.np_aff_in); put(a.aff_in, 1, a.o_b_in1, 1);
+  put(D, a.aff_in, a.o_w_in2, a.np_lin); put(D, 1, a.o_b_in2, 1);
+  for (int l = 0; l < a.L; ++l) {
+    const long long base = a.o_layers + (long long)l * a.layer_stride;
+    put(P, D, base + a.lo_wp, a.np_proj);
+    put(P, a.lorder, base + a.lo_taps, P);
+    put(P, a.rorder, base + a.lo_taps + (long long)a.lorder * P, P);
+    put(D, P, base + a.lo_wa, a.np_lin); put(D, 1, base + a.lo_ba, 1);
+  }
+  put(a.aff_out, D, a.o_w_out1, a.np_aff_out); put(a.aff_out, 1, a.o_b_out1, 1);
+  put(a.odim, a.aff_out, a.o_w_out2, a.np_odim); put(a.odim, 1, a.o_b_out2, 1);
+  for (int i = 0; i < p.n; ++i)
+    WEKWS_REQUIRE(p.p[i].src != nullptr, "wekws_fsmn_load_params: parameter %d is null", i);
+  return fsmn_pack_launch(p, (cudaStream_t)stream);
+}
+
+extern "C" int64_t wekws_fsmn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
+  WEKWS_REQUIRE(m && m->cfg.backbone == WEKWS_BACKBONE_FSMN && B >= 0 && T >= 0,
+                "wekws_fsmn_train_saved_floats: an FSMN model and B, T >= 0 are required");
+  return B * T * fsmn_saved_per_frame(fsmn_dims(m->cfg));
+}
+
+extern "C" int64_t wekws_fsmn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
+  WEKWS_REQUIRE(m && m->cfg.backbone == WEKWS_BACKBONE_FSMN && B >= 0 && T >= 0,
+                "wekws_fsmn_backward_workspace_bytes: an FSMN model and B, T >= 0 are required");
+  return (int64_t)sizeof(float) * fsmn_backward_workspace_floats(fsmn_dims(m->cfg), B * T);
+}
+
+extern "C" int wekws_fsmn_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
+                                        float* d_saved, int64_t B, int64_t T, void* stream) {
+  int rc = fsmn_train_check(m, "wekws_fsmn_train_forward");
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_fsmn_train_forward: bad B/T");
+  WEKWS_REQUIRE(d_feats && d_out && d_out_cache && d_saved, "wekws_fsmn_train_forward: null tensor");
+  cudaStream_t st = (cudaStream_t)stream;
+  // the time chunks of wekws_model_forward, each launch also storing its frames' activations
+  const int maxT = fsmn_tile_rows();
+  const int nchunk = (int)((T + maxT - 1) / maxT);
+  const int Tc = (int)((T + nchunk - 1) / nchunk);
+  for (int64_t t0 = 0; t0 < T; t0 += Tc) {
+    FsmnArgs a = m->fsmn;
+    a.feats = d_feats + t0 * m->cfg.idim;
+    a.out = d_out + t0 * m->cfg.odim;
+    a.in_cache = t0 == 0 ? nullptr : d_out_cache;
+    a.out_cache = d_out_cache;
+    a.B = (int)B;
+    a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
+    a.feat_bstride = T * m->cfg.idim;
+    a.out_bstride = T * m->cfg.odim;
+    a.saved = d_saved; a.save_T = (int)T; a.save_t0 = (int)t0;
+    if ((rc = fsmn_train_launch(a, st))) return rc;
+  }
+  return WEKWS_OK;
+}
+
+extern "C" int wekws_fsmn_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_grad_out,
+                                   int64_t B, int64_t T, float* const* h_grads, int n, void* d_workspace, void* stream) {
+  int rc = fsmn_train_check(m, "wekws_fsmn_backward");
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_fsmn_backward: bad B/T");
+  WEKWS_REQUIRE(d_feats && d_saved && d_grad_out && d_workspace && h_grads, "wekws_fsmn_backward: null argument");
+  WEKWS_REQUIRE(n == 8 + 5 * m->fsmn.L, "wekws_fsmn_backward: expected %d gradient buffers, got %d", 8 + 5 * m->fsmn.L, n);
+  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_grads[i] != nullptr, "wekws_fsmn_backward: gradient buffer %d is null", i);
+  return fsmn_backward_launch(m->fsmn, d_feats, d_saved, d_grad_out, (int)B, (int)T, h_grads, (float*)d_workspace,
+                              (cudaStream_t)stream);
+}
+
+extern "C" int wekws_fsmn_backward_launches(const wekws_model* m) {
+  return m && m->cfg.backbone == WEKWS_BACKBONE_FSMN ? fsmn_backward_launches(m->cfg.num_layers) : 0;
+}
+
 extern "C" int wekws_pipeline_forward(wekws_fbank* fb, wekws_model* m, const void* d_pcm, int pcm_dtype,
                                       int64_t B, int64_t num_samples, int64_t pcm_stride,
                                       float* d_feat_scratch, const float* d_in_cache, float* d_out,

@@ -10,8 +10,8 @@ Same constructor, attributes (``idim``, ``odim``, ``hdim``, ``backbone.padding``
 The modules in here are parameter HOLDERS only.  ``forward`` hands raw device pointers to
 the C-ABI library (include/wekws_b200.h) whose fused sm_90a kernels do all the work:
 CMVN -> Linear+ReLU -> backbone with streaming cache -> classifier -> activation
-(kws_model.py:65-76).  There is no PyTorch / CPU fallback: CPU tensors, training mode or a
-missing native library raise.
+(kws_model.py:65-76).  There is no PyTorch / CPU fallback: CPU tensors, training mode (except the FSMN model's,
+whose forward and backward run on the device: fsmn_train.py) or a missing native library raise.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ from typing import Optional, Tuple
 import torch
 import torch.nn as nn
 
-from . import _native
+from . import _native, fsmn_train
 from .cmvn import load_cmvn, load_kaldi_cmvn
 
 _EMPTY = torch.zeros(0, 0, 0, dtype=torch.float)
@@ -347,10 +347,25 @@ class KWSModel(nn.Module):
         return cache, out, out_cache
 
     # ------------------------------------------------------------------------- forward
+    def _training_handle(self, device: torch.device):
+        """The native model for a training forward on `device`: made by the host path when there is none yet (or it
+        is stale), otherwise kept as is -- the training forward packs the current parameters on the device itself,
+        and leaves the version-counter fingerprint alone, so the next eval call repacks from the host as usual."""
+        if self._dirty or self._handle is None or self._handle_dev != device:
+            self._ensure(device)
+        return self._handle
+
     def _run(self, x: torch.Tensor, in_cache: torch.Tensor, flags: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        train_fsmn = False
         if self.training:
-            raise RuntimeError("wekws_b200.KWSModel is inference-only: call model.eval() first "
-                               "(training-mode BatchNorm/Dropout are not implemented)")
+            # FSMN: the training-mode forward is the eval forward (no BatchNorm; its Dropout is never called), so under
+            # no_grad it takes the eval path; with grad it builds the graph (fsmn_train.py)
+            if getattr(self.backbone, "kind", None) != "fsmn":
+                raise RuntimeError("wekws_b200.KWSModel is inference-only: call model.eval() first "
+                                   "(training-mode BatchNorm/Dropout are not implemented)")
+            train_fsmn = fsmn_train.wants_grad(self)
+            if train_fsmn and flags != 0:
+                raise RuntimeError("wekws_b200: forward_softmax has no training path; call forward() for training")
         if not x.is_cuda:
             raise RuntimeError("wekws_b200.KWSModel runs on CUDA (sm_90a) only; got a CPU tensor. "
                                "There is no CPU fallback -- move the model and inputs to an H100.")
@@ -358,6 +373,8 @@ class KWSModel(nn.Module):
             raise TypeError(f"wekws_b200.KWSModel expects float32 features, got {x.dtype}")
         if x.dim() != 3 or x.size(2) != self.idim:
             raise ValueError(f"features must be (B, T, {self.idim}), got {tuple(x.shape)}")
+        if train_fsmn:
+            return fsmn_train.forward(self, x, in_cache)
         dev = x.device
         B, T = x.size(0), x.size(1)
         if not x.is_contiguous():
