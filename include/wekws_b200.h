@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 13  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training) */
+#define WEKWS_B200_ABI_VERSION 14  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training) */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -491,6 +491,52 @@ WEKWS_API int64_t wekws_fsmn_backward_workspace_bytes(const wekws_model* m, int6
 WEKWS_API int wekws_fsmn_backward_launches(const wekws_model* m);
 WEKWS_API int wekws_fsmn_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_grad_out,
                                   int64_t B, int64_t T, float* const* h_grads, int n, void* d_workspace, void* stream);
+
+/* Training the MDTC model (wekws/utils/executor.py Executor.train with an mdtc.yaml / mdtc_small.yaml model): the
+ * training-mode forward, every BatchNorm normalising with the biased variance of the batch (all B * T frames, padding
+ * included) and updating its running statistics, and the backward to every parameter of wekws/model/mdtc.py MDTC.
+ * The handle only supplies the config (wekws_model_create is enough): an MDTC model with hidden_dim 32 or 64, the
+ * per-frame linear classifier (no wekws_model_set_head), input_dim <= 128, output_dim <= 16, kernel_size <= 8 and at
+ * most 25 blocks.  Everything the kernels read travels with the call, so an optimiser step needs no host round trip:
+ *   h_params: wekws_mdtc_num_params(m) = 4 + 12 L device pointers (L = 1 + num_stack * stack_size blocks), in
+ *     named_parameters order, each contiguous float32 in the parameter's own shape:
+ *     preprocessing.out.0.{weight,bias}; per block (backbone.preprocessor, then backbone.blocks.{s}.res_blocks.{l}):
+ *     conv1.conv.{weight,bias}, conv1.bn.{weight,bias}, conv1.pointwise.{weight,bias}, bn1.{weight,bias},
+ *     conv2.{weight,bias}, bn2.{weight,bias}; classifier.linear.{weight,bias}.
+ *   d_cmvn_mean / d_cmvn_istd: global_cmvn.{mean,istd} (idim floats), or both NULL without CMVN; cfg.norm_var applies.
+ *   h_running: 6 L device pointers, running_mean and running_var of conv1.bn, bn1, bn2 of each block in block order;
+ *     h_bn: 6 L host doubles, (momentum, eps) of the same BatchNorms.  running_var takes the unbiased variance.  The
+ *     kernel writes them: a packed eval model of the same weights must be re-made (wekws_model_finalize) to see them.
+ *
+ * wekws_mdtc_train_forward: B utterances of T frames (B * T >= 2) from empty caches: d_out (B, T, odim), d_out_cache
+ *   (B, hdim, padding) as the reference's training-mode new_cache.  save != 0: also writes d_saved,
+ *   wekws_mdtc_train_saved_floats(m, B, T) = 12 L hdim + B T hdim (4 L + 2) floats (each BatchNorm's mean and invstd,
+ *   the preprocessing output, per block its three pre-BatchNorm tensors and its output, the stack sum).  save == 0:
+ *   d_saved may be NULL, same d_out / d_out_cache / running-statistics bits.  d_workspace:
+ *   wekws_mdtc_train_workspace_bytes(m, B, T, save) = 48 * 128 hdim + (save ? 0 : 24 B T hdim) bytes.
+ *   wekws_mdtc_train_forward_launches(m) = 2 + 3 L launches either way.
+ * wekws_mdtc_backward: from d_feats, the same h_params / CMVN buffers and d_saved of a save != 0 forward and
+ *   d_grad_out = d loss / d out (B, T, odim), writes every element of the 4 + 12 L gradient buffers h_grads (same
+ *   shapes as h_params), all B * T frames as rows.  Every batch statistic and weight-gradient sum is formed in double
+ *   over 128 fixed row slices and the slices added in order: no atomics, equal inputs give equal bits.
+ *   d_workspace: wekws_mdtc_backward_workspace_bytes(m, B, T) = 32 * 128 hdim + 20 B T hdim + 8 * 128 P bytes, P the
+ *   number of weight and bias elements of the preprocessing Linear, the convolutions and the classifier.
+ *   wekws_mdtc_backward_launches(m) = 3 + 4 L launches.
+ * The size and launch queries return a negative status (0 for the counts) for a model they do not accept.        */
+WEKWS_API int wekws_mdtc_num_params(const wekws_model* m);
+WEKWS_API int64_t wekws_mdtc_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int64_t wekws_mdtc_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save);
+WEKWS_API int wekws_mdtc_train_forward_launches(const wekws_model* m);
+WEKWS_API int wekws_mdtc_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                       const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
+                                       const double* h_bn, float* d_out, float* d_out_cache, float* d_saved, int save,
+                                       void* d_workspace, int64_t B, int64_t T, void* stream);
+WEKWS_API int64_t wekws_mdtc_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_mdtc_backward_launches(const wekws_model* m);
+WEKWS_API int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                  const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                  const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads,
+                                  void* d_workspace, void* stream);
 
 /* Resampling: torchaudio.transforms.Resample(orig_freq, new_freq) with sinc_interp_hann (the resampling of
  * wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py:50-53), for B waveforms of their own lengths.

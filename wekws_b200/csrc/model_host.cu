@@ -23,6 +23,7 @@
 #include "tcn_tc.h"
 #include "dstcn_tc.h"
 #include "fsmn.h"
+#include "mdtc_train.h"
 #include "linear_tc.h"
 #include "cls_head.h"
 #include "tc_common.cuh"
@@ -967,6 +968,126 @@ extern "C" int wekws_fsmn_backward(wekws_model* m, const float* d_feats, const f
 
 extern "C" int wekws_fsmn_backward_launches(const wekws_model* m) {
   return m && m->cfg.backbone == WEKWS_BACKBONE_FSMN ? fsmn_backward_launches(m->cfg.num_layers) : 0;
+}
+
+// ------------------------------------------------------------------------------- MDTC training
+namespace {
+
+// the dimensions of an MDTC model with the per-frame linear classifier, as the training kernels take them
+int mdtc_train_dims(const wekws_model* m, const char* what, MdtcTrainDims* d) {
+  WEKWS_REQUIRE(m, "%s: null handle", what);
+  const wekws_model_config& c = m->cfg;
+  WEKWS_REQUIRE(c.backbone == WEKWS_BACKBONE_MDTC, "%s: an MDTC model is required", what);
+  WEKWS_REQUIRE(m->head == WEKWS_HEAD_LINEAR, "%s: the MDTC model trains with the per-frame linear classifier", what);
+  WEKWS_REQUIRE(c.hdim == 32 || c.hdim == 64, "%s: hidden_dim %d unsupported in training (32 or 64)", what, c.hdim);
+  WEKWS_REQUIRE(c.kernel_size >= 2 && c.kernel_size <= MDTC_TRAIN_MAX_K, "%s: kernel_size %d unsupported (2..%d)", what,
+                c.kernel_size, MDTC_TRAIN_MAX_K);
+  WEKWS_REQUIRE(c.idim >= 1 && c.idim <= MDTC_TRAIN_MAX_IDIM, "%s: input_dim %d unsupported (1..%d)", what, c.idim,
+                MDTC_TRAIN_MAX_IDIM);
+  WEKWS_REQUIRE(c.odim >= 1 && c.odim <= MDTC_TRAIN_MAX_ODIM, "%s: output_dim %d unsupported in training (1..%d)", what,
+                c.odim, MDTC_TRAIN_MAX_ODIM);
+  const int L = 1 + c.num_stack * c.stack_size;
+  WEKWS_REQUIRE(c.num_stack >= 1 && c.stack_size >= 1 && L <= MDTC_TRAIN_MAX_BLOCKS,
+                "%s: %d stacks of %d blocks unsupported (at most %d blocks)", what, c.num_stack, c.stack_size,
+                MDTC_TRAIN_MAX_BLOCKS);
+  memset(d, 0, sizeof(*d));
+  d->C = c.hdim; d->idim = c.idim; d->odim = c.odim; d->K = c.kernel_size; d->L = L; d->stack_size = c.stack_size;
+  d->act = c.activation == WEKWS_ACT_SIGMOID ? 1 : 0;
+  d->norm_var = c.norm_var;
+  int off = 0;
+  for (int b = 0; b < L; ++b) {
+    d->dil[b] = b == 0 ? 1 : 1 << ((b - 1) % c.stack_size);
+    d->coff[b] = off;
+    off += d->dil[b] * (c.kernel_size - 1);
+  }
+  d->pad_total = off;
+  return WEKWS_OK;
+}
+
+}  // namespace
+
+extern "C" int wekws_mdtc_num_params(const wekws_model* m) {
+  MdtcTrainDims d;
+  return mdtc_train_dims(m, "wekws_mdtc_num_params", &d) ? 0 : mdtc_train_num_params(d.L);
+}
+
+extern "C" int64_t wekws_mdtc_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
+  MdtcTrainDims d;
+  int rc = mdtc_train_dims(m, "wekws_mdtc_train_saved_floats", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_train_saved_floats: B, T >= 0 are required");
+  return mdtc_train_saved_floats(d, B * T);
+}
+
+extern "C" int64_t wekws_mdtc_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save) {
+  MdtcTrainDims d;
+  int rc = mdtc_train_dims(m, "wekws_mdtc_train_workspace_bytes", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_train_workspace_bytes: B, T >= 0 are required");
+  return mdtc_train_workspace_bytes(d, B * T, save != 0);
+}
+
+extern "C" int64_t wekws_mdtc_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
+  MdtcTrainDims d;
+  int rc = mdtc_train_dims(m, "wekws_mdtc_backward_workspace_bytes", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_backward_workspace_bytes: B, T >= 0 are required");
+  return mdtc_backward_workspace_bytes(d, B * T);
+}
+
+extern "C" int wekws_mdtc_train_forward_launches(const wekws_model* m) {
+  MdtcTrainDims d;
+  return mdtc_train_dims(m, "wekws_mdtc_train_forward_launches", &d) ? 0 : mdtc_train_forward_launches(d.L);
+}
+
+extern "C" int wekws_mdtc_backward_launches(const wekws_model* m) {
+  MdtcTrainDims d;
+  return mdtc_train_dims(m, "wekws_mdtc_backward_launches", &d) ? 0 : mdtc_train_backward_launches(d.L);
+}
+
+extern "C" int wekws_mdtc_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                        const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
+                                        const double* h_bn, float* d_out, float* d_out_cache, float* d_saved, int save,
+                                        void* d_workspace, int64_t B, int64_t T, void* stream) {
+  MdtcTrainDims d;
+  int rc = mdtc_train_dims(m, "wekws_mdtc_train_forward", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31),
+                "wekws_mdtc_train_forward: B = %lld, T = %lld unsupported (B * T >= 2 frames are needed for batch "
+                "statistics)", (long long)B, (long long)T);
+  WEKWS_REQUIRE(n == mdtc_train_num_params(d.L), "wekws_mdtc_train_forward: expected %d parameters, got %d",
+                mdtc_train_num_params(d.L), n);
+  WEKWS_REQUIRE(d_feats && h_params && h_running && h_bn && d_out && d_out_cache && d_workspace && (!save || d_saved),
+                "wekws_mdtc_train_forward: null argument");
+  WEKWS_REQUIRE((d_cmvn_mean == nullptr) == (d_cmvn_istd == nullptr),
+                "wekws_mdtc_train_forward: pass both CMVN buffers or neither");
+  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_params[i] != nullptr, "wekws_mdtc_train_forward: parameter %d is null", i);
+  for (int i = 0; i < 6 * d.L; ++i)
+    WEKWS_REQUIRE(h_running[i] != nullptr, "wekws_mdtc_train_forward: running statistic %d is null", i);
+  for (int i = 0; i < 3 * d.L; ++i)
+    WEKWS_REQUIRE(h_bn[2 * i] >= 0.0 && h_bn[2 * i] <= 1.0 && h_bn[2 * i + 1] > 0.0,
+                  "wekws_mdtc_train_forward: BatchNorm %d has momentum %g, eps %g", i, h_bn[2 * i], h_bn[2 * i + 1]);
+  return mdtc_train_forward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache,
+                                   save ? d_saved : nullptr, d_workspace, (int)B, (int)T, (cudaStream_t)stream);
+}
+
+extern "C" int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                   const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                   const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads,
+                                   void* d_workspace, void* stream) {
+  MdtcTrainDims d;
+  int rc = mdtc_train_dims(m, "wekws_mdtc_backward", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31), "wekws_mdtc_backward: bad B/T");
+  WEKWS_REQUIRE(n == mdtc_train_num_params(d.L), "wekws_mdtc_backward: expected %d parameters, got %d",
+                mdtc_train_num_params(d.L), n);
+  WEKWS_REQUIRE(d_feats && h_params && d_saved && d_grad_out && h_grads && d_workspace,
+                "wekws_mdtc_backward: null argument");
+  for (int i = 0; i < n; ++i)
+    WEKWS_REQUIRE(h_params[i] != nullptr && h_grads[i] != nullptr, "wekws_mdtc_backward: parameter or gradient %d is "
+                  "null", i);
+  return mdtc_backward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B, (int)T,
+                              h_grads, d_workspace, (cudaStream_t)stream);
 }
 
 extern "C" int wekws_pipeline_forward(wekws_fbank* fb, wekws_model* m, const void* d_pcm, int pcm_dtype,

@@ -10,8 +10,9 @@ Same constructor, attributes (``idim``, ``odim``, ``hdim``, ``backbone.padding``
 The modules in here are parameter HOLDERS only.  ``forward`` hands raw device pointers to
 the C-ABI library (include/wekws_b200.h) whose fused sm_90a kernels do all the work:
 CMVN -> Linear+ReLU -> backbone with streaming cache -> classifier -> activation
-(kws_model.py:65-76).  There is no PyTorch / CPU fallback: CPU tensors, training mode (except the FSMN model's,
-whose forward and backward run on the device: fsmn_train.py) or a missing native library raise.
+(kws_model.py:65-76).  There is no PyTorch / CPU fallback: CPU tensors, training mode or a missing native library
+raise.  Training runs on the device for the FSMN model (fsmn_train.py) and, after ``enable_training()``, for the MDTC
+model with the per-frame linear classifier (mdtc_train.py).
 """
 from __future__ import annotations
 
@@ -22,7 +23,7 @@ from typing import Optional, Tuple
 import torch
 import torch.nn as nn
 
-from . import _native, fsmn_train
+from . import _native, fsmn_train, mdtc_train
 from .cmvn import load_cmvn, load_kaldi_cmvn
 
 _EMPTY = torch.zeros(0, 0, 0, dtype=torch.float)
@@ -174,6 +175,7 @@ class KWSModel(nn.Module):
         # FP32 FMA elsewhere; "fp32": FP32 FMA kernels only.
         self.precision = "auto"
         self._precision_applied = None
+        self._training_enabled = False   # enable_training(): BatchNorm models run training mode only after opting in
 
     # ---------------------------------------------------------------- weight life-cycle
     def invalidate(self) -> None:
@@ -346,6 +348,19 @@ class KWSModel(nn.Module):
             out_cache = torch.zeros(shape, device=dev, dtype=torch.float32)
         return cache, out, out_cache
 
+    # ------------------------------------------------------------------------- training
+    def enable_training(self) -> "KWSModel":
+        """Lets ``train()`` mode run the training forward of the MDTC model with the per-frame linear classifier
+        (mdtc_train.py): batch statistics, running-statistics updates, gradients for ``loss.backward()``.  Without it
+        a BatchNorm model in training mode refuses to run, so a model left in ``train()`` by accident cannot silently
+        give training-mode outputs or overwrite its running statistics.  A no-op for the FSMN model, whose training
+        needs no opt-in; NotImplementedError for the backbones and heads with Dropout (TCN, DS-TCN, the ``global`` /
+        ``last`` heads) and for the GRU.  Not part of the state_dict; kept by copies and pickles."""
+        if getattr(self.backbone, "kind", None) != "fsmn":
+            mdtc_train.check_trainable(self)
+            self._training_enabled = True
+        return self
+
     # ------------------------------------------------------------------------- forward
     def _training_handle(self, device: torch.device):
         """The native model for a training forward on `device`: made by the host path when there is none yet (or it
@@ -356,16 +371,22 @@ class KWSModel(nn.Module):
         return self._handle
 
     def _run(self, x: torch.Tensor, in_cache: torch.Tensor, flags: int) -> Tuple[torch.Tensor, torch.Tensor]:
-        train_fsmn = False
+        train_fsmn = train_mdtc = False
         if self.training:
+            kind = getattr(self.backbone, "kind", None)
             # FSMN: the training-mode forward is the eval forward (no BatchNorm; its Dropout is never called), so under
-            # no_grad it takes the eval path; with grad it builds the graph (fsmn_train.py)
-            if getattr(self.backbone, "kind", None) != "fsmn":
+            # no_grad it takes the eval path; with grad it builds the graph (fsmn_train.py).  MDTC after
+            # enable_training(): the batch-statistics forward, with or without grad (mdtc_train.py).
+            train_mdtc = kind == "mdtc" and self.__dict__.get("_training_enabled", False)
+            if kind != "fsmn" and not train_mdtc:
+                hint = " -- or call model.enable_training() to train this MDTC model" if kind == "mdtc" else ""
                 raise RuntimeError("wekws_b200.KWSModel is inference-only: call model.eval() first "
-                                   "(training-mode BatchNorm/Dropout are not implemented)")
-            train_fsmn = fsmn_train.wants_grad(self)
-            if train_fsmn and flags != 0:
+                                   "(training-mode BatchNorm/Dropout are not implemented)" + hint)
+            train_fsmn = kind == "fsmn" and fsmn_train.wants_grad(self)
+            if (train_fsmn or train_mdtc) and flags != 0:
                 raise RuntimeError("wekws_b200: forward_softmax has no training path; call forward() for training")
+            if train_mdtc:
+                mdtc_train.check_call(self, x, in_cache)
         if not x.is_cuda:
             raise RuntimeError("wekws_b200.KWSModel runs on CUDA (sm_90a) only; got a CPU tensor. "
                                "There is no CPU fallback -- move the model and inputs to an H100.")
@@ -375,6 +396,8 @@ class KWSModel(nn.Module):
             raise ValueError(f"features must be (B, T, {self.idim}), got {tuple(x.shape)}")
         if train_fsmn:
             return fsmn_train.forward(self, x, in_cache)
+        if train_mdtc:
+            return mdtc_train.forward(self, x, in_cache)
         dev = x.device
         B, T = x.size(0), x.size(1)
         if not x.is_contiguous():
