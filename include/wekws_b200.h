@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 14  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training) */
+#define WEKWS_B200_ABI_VERSION 15  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -537,6 +537,55 @@ WEKWS_API int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, co
                                   const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
                                   const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads,
                                   void* d_workspace, void* stream);
+
+/* Training the TCN / DS-TCN model (Executor.train with a tcn.yaml / ds_tcn.yaml / ds_tcn_ctc.yaml model): the
+ * training-mode forward of wekws/model/tcn.py with the per-frame linear classifier, every BatchNorm as in MDTC
+ * training above, every block's Dropout applying a device mask, and the backward to every parameter.  Supported: the
+ * dense (TCN) and depthwise-separable (DS-TCN) backbones, hidden_dim 64 or 256, kernel_size 2..8, 1..8 layers,
+ * input_dim <= 128, output_dim <= 4096; the per-frame linear classifier; Sigmoid or Identity activation.
+ *   h_params: wekws_tcn_num_params(m) = 4 + P L device pointers (P = 4 dense, 8 ds), named_parameters order:
+ *     preprocessing.out.0.{weight,bias}; per block backbone.network.{l}.cnn.: 0.{weight,bias} (the dilated conv),
+ *     1.{weight,bias} (BatchNorm), ds only: 3.{weight,bias} (pointwise conv), 4.{weight,bias} (BatchNorm);
+ *     classifier.linear.{weight,bias}.
+ *   h_running / h_bn: as for MDTC, for the BatchNorms cnn.1 [, cnn.4] of each block in block order (L or 2 L).
+ *   Dropout: h_p, L host doubles, block l's probability p_l; seed, a 64-bit seed.  Element (b, t, c) of block l's
+ *     ReLU output is kept iff (word >> 8) >= theta_l, theta_l = ceil(p_l 2^24) (in double), word = component c % 4
+ *     of Philox4x32-10(counter = (c / 4, t, b, 1 + l), key = (seed lo, seed hi)) (Random123 constants, as the dither;
+ *     the dither's counters have word 3 = 0, so the streams are disjoint); a kept element is multiplied by
+ *     s_l = 1.0f / (float)(1 - p_l), a dropped one is 0 (selected, not multiplied: p = 1 gives exact zeros).  The
+ *     backward recomputes the masks from the same seed and h_p.
+ * wekws_tcn_train_forward: B utterances of T frames (B * T >= 2) from empty caches: d_out (B, T, odim), d_out_cache
+ *   (B, hdim, padding).  save != 0: also writes d_saved, wekws_tcn_train_saved_floats(m, B, T) = 4 N hdim +
+ *   B T hdim (1 + L (P / 4 + 1)) floats, N = L (dense) or 2 L (ds) BatchNorms (each BatchNorm's mean and invstd as
+ *   doubles, the preprocessing output, per block its pre-BatchNorm tensors and its output).  d_workspace:
+ *   wekws_tcn_train_workspace_bytes(m, B, T, save) = 32 * 128 hdim + (save ? 0 : 16 B T hdim) bytes.
+ *   wekws_tcn_train_forward_launches(m) = 2 + L (dense) or 2 + 2 L (ds) launches either way.
+ * wekws_tcn_backward: from d_feats, the same h_params / CMVN buffers / seed / h_p, d_saved and d_out of a save != 0
+ *   forward and d_grad_out (B, T, odim), writes every element of the gradient buffers h_grads.  Batch statistics are
+ *   formed in double over 128 fixed row slices; each weight gradient over Z fixed row ranges (FP32 over 256 rows,
+ *   double across them), Z = min(64, max(1, B T / 256), ceil(264 / tiles)) with tiles = ceil(N / 64) ceil((Q + 1) / 64)
+ *   for an N x Q weight and its bias; the partials are added in order: no atomics, equal inputs give equal bits.
+ *   d_workspace: wekws_tcn_backward_workspace_bytes(m, B, T) = 32 * 128 hdim + 16 B T hdim + 8 (sum of Z N (Q + 1)
+ *   over the weights, + 128 hdim (K + 1) per ds block) bytes.  wekws_tcn_backward_launches(m) = 4 + 2 L (dense) or
+ *   4 + 3 L (ds) launches.
+ * wekws_dropout_mask (test hook): d_out (B, T, C) bytes, 1 where block `layer` keeps the element, for theta.       */
+WEKWS_API int wekws_tcn_num_params(const wekws_model* m);
+WEKWS_API int64_t wekws_tcn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int64_t wekws_tcn_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save);
+WEKWS_API int wekws_tcn_train_forward_launches(const wekws_model* m);
+WEKWS_API int wekws_tcn_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                      const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
+                                      const double* h_bn, uint64_t seed, const double* h_p, float* d_out,
+                                      float* d_out_cache, float* d_saved, int save, void* d_workspace, int64_t B,
+                                      int64_t T, void* stream);
+WEKWS_API int64_t wekws_tcn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_tcn_backward_launches(const wekws_model* m);
+WEKWS_API int wekws_tcn_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                 const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                 const float* d_out, const float* d_grad_out, uint64_t seed, const double* h_p,
+                                 int64_t B, int64_t T, float* const* h_grads, void* d_workspace, void* stream);
+WEKWS_API int wekws_dropout_mask(uint64_t seed, int64_t B, int64_t T, int64_t C, int layer, uint32_t theta,
+                                 uint8_t* d_out, void* stream);
 
 /* Resampling: torchaudio.transforms.Resample(orig_freq, new_freq) with sinc_interp_hann (the resampling of
  * wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py:50-53), for B waveforms of their own lengths.

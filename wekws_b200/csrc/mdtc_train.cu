@@ -20,93 +20,16 @@
 
 #include "common.cuh"
 #include "mdtc_train.h"
+#include "train_common.cuh"
 
 namespace wekws {
 
 namespace {
 
+using namespace train;
 constexpr int S = MDTC_TRAIN_SLICES;
-constexpr int NT = 256;
-
-struct Rows {
-  long long r0, r1;
-};
-__device__ inline Rows slice_rows(long long M) {
-  const long long rs = (M + S - 1) / S;
-  const long long r0 = min(M, (long long)blockIdx.x * rs);
-  return {r0, min(M, r0 + rs)};
-}
-
-// ---------------------------------------------------------------------------------------------------- batch norm
-struct BnFold {
-  const double* part;              // [S][2][C]: slice sums of x and x^2
-  const float* gamma;
-  const float* beta;
-  float* run_mean;                 // updated by CTA 0
-  float* run_var;
-  double momentum, eps;
-  double* stats;                   // [2][C] mean, invstd, written by CTA 0 for the backward; nullptr: not kept
-};
-
-// BN(x) = (x - mean) * scale + beta with mean and scale = gamma * invstd rounded once from double: torch's order (the
-// subtraction first keeps a channel whose mean is far from 0 exact), and the same bits in the forward and in the
-// backward's recomputation
-__device__ inline void bn_affine(double mean, double invstd, float gamma, float& sc, float& sm) {
-  sc = (float)((double)gamma * invstd);
-  sm = (float)mean;
-}
-__device__ inline float bn_apply(float x, float sm, float sc, float beta) { return fmaf(x - sm, sc, beta); }
-
-// the slice sums of `part` ([S][2][C]) in slice order, into tmp[2C]
-template <int C>
-__device__ inline void sum_slices(const double* part, double* tmp) {
-  const int t = threadIdx.x;
-  if (t < 2 * C) {
-    double s = 0.0;
-    for (int z = 0; z < S; ++z) s += part[z * 2 * C + t];
-    tmp[t] = s;
-  }
-  __syncthreads();
-}
-
-// the batch statistics of a BatchNorm's input -> its scale / mean / beta; CTA 0 also updates the running statistics
-// (torch: running_var with the unbiased variance) and stores mean / invstd
-template <int C>
-__device__ void fold_bn(const BnFold& f, long long M, float* sc, float* sh, float* sb, double* tmp) {
-  sum_slices<C>(f.part, tmp);
-  const int c = threadIdx.x;
-  if (c < C) {
-    const double mean = tmp[c] / (double)M;
-    const double var = fmax(tmp[C + c] / (double)M - mean * mean, 0.0);
-    const double invstd = 1.0 / sqrt(var + f.eps);
-    bn_affine(mean, invstd, f.gamma[c], sc[c], sh[c]);
-    sb[c] = f.beta[c];
-    if (blockIdx.x == 0) {
-      if (f.stats != nullptr) {
-        f.stats[c] = mean;
-        f.stats[C + c] = invstd;
-      }
-      const double m = f.momentum;
-      f.run_mean[c] = (float)((1.0 - m) * (double)f.run_mean[c] + m * mean);
-      f.run_var[c] = (float)((1.0 - m) * (double)f.run_var[c] + m * var * (double)M / (double)(M - 1));
-    }
-  }
-  __syncthreads();
-}
-
-// the row groups' per-channel (s1, s2) in group order -> this slice's partial part[blockIdx.x][2][C]
-template <int C, int G>
-__device__ inline void write_slice_stats(double (*red)[2][C], int g, int c, double s1, double s2, double* part) {
-  red[g][0][c] = s1;
-  red[g][1][c] = s2;
-  __syncthreads();
-  const int t = threadIdx.x;
-  if (t < 2 * C) {
-    double s = 0.0;
-    for (int q = 0; q < G; ++q) s += red[q][t / C][t % C];
-    part[(long long)blockIdx.x * 2 * C + t] = s;
-  }
-}
+constexpr int NT = TRAIN_NT;
+static_assert(S == TRAIN_SLICES, "the MDTC slices are the shared scheme's");
 
 // ---------------------------------------------------------------------------------------------------- forward
 // preprocessing Linear(idim, C) + ReLU of the CMVN-normalised features
@@ -417,42 +340,6 @@ __global__ void __launch_bounds__(NT) mdtc_train_gstat_kernel(const GStatArgs a)
     s2 += (double)gv * (((double)a.a[i] - mean) * inv);
   }
   write_slice_stats<C, G>(red, g, c, s1, s2, a.part);
-}
-
-// BatchNorm backward from the gradient statistics, and gamma / beta's gradients (CTA 0)
-struct BnGrad {
-  const float* a; const double* stats; const float* gamma; const double* gpart;
-  float* dgamma; float* dbeta;
-};
-
-// per channel, in double: k1 = gamma invstd, mg = Sigma g / M, mgx = Sigma g x_hat / M, mean, invstd.  The batch
-// statistics' backward, da = k1 (g - mg - x_hat mgx), is formed in double with x_hat in double as in the statistics'
-// sums, so that Sigma da -- the gradient of a bias in front of a BatchNorm, zero in exact arithmetic -- stays at
-// double round-off
-template <int C>
-__device__ inline double bn_grad(float g, float a, int c, const double* k1, const double* mg, const double* mgx,
-                                 const double* mean, const double* inv) {
-  const double xh = ((double)a - mean[c]) * inv[c];
-  return k1[c] * ((double)g - mg[c] - xh * mgx[c]);
-}
-
-template <int C>
-__device__ void fold_bn_grad(const BnGrad& b, long long M, double* k1, double* mg, double* mgx, double* mean,
-                             double* inv, double* tmp) {
-  sum_slices<C>(b.gpart, tmp);
-  const int c = threadIdx.x;
-  if (c < C) {
-    if (blockIdx.x == 0) {
-      b.dbeta[c] = (float)tmp[c];
-      b.dgamma[c] = (float)tmp[C + c];
-    }
-    k1[c] = (double)b.gamma[c] * b.stats[C + c];
-    mg[c] = tmp[c] / (double)M;
-    mgx[c] = tmp[C + c] / (double)M;
-    mean[c] = b.stats[c];
-    inv[c] = b.stats[C + c];
-  }
-  __syncthreads();
 }
 
 // The backward of a = W n + bias, n = [relu](BN_in(a_in)), from the gradient into BN_out(a) (g = up [* (ymask > 0)]):

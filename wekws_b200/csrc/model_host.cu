@@ -24,6 +24,7 @@
 #include "dstcn_tc.h"
 #include "fsmn.h"
 #include "mdtc_train.h"
+#include "tcn_train.h"
 #include "linear_tc.h"
 #include "cls_head.h"
 #include "tc_common.cuh"
@@ -1088,6 +1089,148 @@ extern "C" int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, c
                   "null", i);
   return mdtc_backward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B, (int)T,
                               h_grads, d_workspace, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------- TCN / DS-TCN training
+namespace {
+
+// the dimensions of a TCN / DS-TCN model with the per-frame linear classifier, as the training kernels take them
+int tcn_train_dims(const wekws_model* m, const char* what, TcnTrainDims* d) {
+  WEKWS_REQUIRE(m, "%s: null handle", what);
+  const wekws_model_config& c = m->cfg;
+  WEKWS_REQUIRE(c.backbone == WEKWS_BACKBONE_TCN || c.backbone == WEKWS_BACKBONE_DSTCN,
+                "%s: a TCN or DS-TCN model is required", what);
+  WEKWS_REQUIRE(m->head == WEKWS_HEAD_LINEAR, "%s: the TCN model trains with the per-frame linear classifier", what);
+  WEKWS_REQUIRE((c.hdim == 64 || c.hdim == 256) && c.kernel_size >= 2 && c.kernel_size <= TCN_TRAIN_MAX_K &&
+                    c.num_layers >= 1 && c.num_layers <= TCN_TRAIN_MAX_LAYERS && c.idim >= 1 &&
+                    c.idim <= TCN_TRAIN_MAX_IDIM && c.odim >= 1 && c.odim <= TCN_TRAIN_MAX_ODIM,
+                "%s: TCN training supports hidden_dim 64 or 256, kernel_size 2..%d, 1..%d layers, input_dim <= %d and "
+                "output_dim <= %d; got hidden %d, kernel %d, %d layers, input %d, output %d", what, TCN_TRAIN_MAX_K,
+                TCN_TRAIN_MAX_LAYERS, TCN_TRAIN_MAX_IDIM, TCN_TRAIN_MAX_ODIM, c.hdim, c.kernel_size, c.num_layers,
+                c.idim, c.odim);
+  memset(d, 0, sizeof(*d));
+  d->C = c.hdim; d->idim = c.idim; d->odim = c.odim; d->K = c.kernel_size; d->L = c.num_layers;
+  d->ds = c.backbone == WEKWS_BACKBONE_DSTCN ? 1 : 0;
+  d->act = c.activation == WEKWS_ACT_SIGMOID ? 1 : 0;
+  d->norm_var = c.norm_var;
+  d->pad_total = (c.kernel_size - 1) * ((1 << c.num_layers) - 1);
+  return WEKWS_OK;
+}
+
+// theta = ceil(p 2^24) in double, scale = 1 / (float)(1 - p), torch's scale
+int tcn_dropout(const TcnTrainDims& d, uint64_t seed, const double* h_p, const char* what, TcnDropout* o) {
+  WEKWS_REQUIRE(h_p, "%s: null dropout probabilities", what);
+  memset(o, 0, sizeof(*o));
+  o->seed = seed;
+  for (int l = 0; l < d.L; ++l) {
+    WEKWS_REQUIRE(h_p[l] >= 0.0 && h_p[l] <= 1.0, "%s: dropout probability %g of block %d is outside [0, 1]", what,
+                  h_p[l], l);
+    o->theta[l] = (uint32_t)ceil(h_p[l] * 16777216.0);
+    o->scale[l] = 1.0f / (float)(1.0 - h_p[l]);
+  }
+  return WEKWS_OK;
+}
+
+}  // namespace
+
+extern "C" int wekws_tcn_num_params(const wekws_model* m) {
+  TcnTrainDims d;
+  return tcn_train_dims(m, "wekws_tcn_num_params", &d) ? 0 : tcn_train_num_params(d);
+}
+
+extern "C" int64_t wekws_tcn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
+  TcnTrainDims d;
+  int rc = tcn_train_dims(m, "wekws_tcn_train_saved_floats", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_tcn_train_saved_floats: B, T >= 0 are required");
+  return tcn_train_saved_floats(d, B * T);
+}
+
+extern "C" int64_t wekws_tcn_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save) {
+  TcnTrainDims d;
+  int rc = tcn_train_dims(m, "wekws_tcn_train_workspace_bytes", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_tcn_train_workspace_bytes: B, T >= 0 are required");
+  return tcn_train_workspace_bytes(d, B * T, save != 0);
+}
+
+extern "C" int64_t wekws_tcn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
+  TcnTrainDims d;
+  int rc = tcn_train_dims(m, "wekws_tcn_backward_workspace_bytes", &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_tcn_backward_workspace_bytes: B, T >= 0 are required");
+  return tcn_backward_workspace_bytes(d, B * T);
+}
+
+extern "C" int wekws_tcn_train_forward_launches(const wekws_model* m) {
+  TcnTrainDims d;
+  return tcn_train_dims(m, "wekws_tcn_train_forward_launches", &d) ? 0 : tcn_train_forward_launches(d);
+}
+
+extern "C" int wekws_tcn_backward_launches(const wekws_model* m) {
+  TcnTrainDims d;
+  return tcn_train_dims(m, "wekws_tcn_backward_launches", &d) ? 0 : tcn_train_backward_launches(d);
+}
+
+extern "C" int wekws_tcn_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                       const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
+                                       const double* h_bn, uint64_t seed, const double* h_p, float* d_out,
+                                       float* d_out_cache, float* d_saved, int save, void* d_workspace, int64_t B,
+                                       int64_t T, void* stream) {
+  TcnTrainDims d;
+  TcnDropout drop;
+  int rc = tcn_train_dims(m, "wekws_tcn_train_forward", &d);
+  if (rc) return rc;
+  if ((rc = tcn_dropout(d, seed, h_p, "wekws_tcn_train_forward", &drop))) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31) && B * T * d.odim < (1LL << 31),
+                "wekws_tcn_train_forward: B = %lld, T = %lld unsupported (B * T >= 2 frames are needed for batch "
+                "statistics)", (long long)B, (long long)T);
+  WEKWS_REQUIRE(n == tcn_train_num_params(d), "wekws_tcn_train_forward: expected %d parameters, got %d",
+                tcn_train_num_params(d), n);
+  WEKWS_REQUIRE(d_feats && h_params && h_running && h_bn && d_out && d_out_cache && d_workspace && (!save || d_saved),
+                "wekws_tcn_train_forward: null argument");
+  WEKWS_REQUIRE((d_cmvn_mean == nullptr) == (d_cmvn_istd == nullptr),
+                "wekws_tcn_train_forward: pass both CMVN buffers or neither");
+  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_params[i] != nullptr, "wekws_tcn_train_forward: parameter %d is null", i);
+  const int nbn = tcn_train_num_bns(d);
+  for (int i = 0; i < 2 * nbn; ++i)
+    WEKWS_REQUIRE(h_running[i] != nullptr, "wekws_tcn_train_forward: running statistic %d is null", i);
+  for (int i = 0; i < nbn; ++i)
+    WEKWS_REQUIRE(h_bn[2 * i] >= 0.0 && h_bn[2 * i] <= 1.0 && h_bn[2 * i + 1] > 0.0,
+                  "wekws_tcn_train_forward: BatchNorm %d has momentum %g, eps %g", i, h_bn[2 * i], h_bn[2 * i + 1]);
+  return tcn_train_forward_launch(d, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out,
+                                  d_out_cache, save ? d_saved : nullptr, d_workspace, (int)B, (int)T,
+                                  (cudaStream_t)stream);
+}
+
+extern "C" int wekws_tcn_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                  const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                  const float* d_out, const float* d_grad_out, uint64_t seed, const double* h_p,
+                                  int64_t B, int64_t T, float* const* h_grads, void* d_workspace, void* stream) {
+  TcnTrainDims d;
+  TcnDropout drop;
+  int rc = tcn_train_dims(m, "wekws_tcn_backward", &d);
+  if (rc) return rc;
+  if ((rc = tcn_dropout(d, seed, h_p, "wekws_tcn_backward", &drop))) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31) && B * T * d.odim < (1LL << 31),
+                "wekws_tcn_backward: bad B/T");
+  WEKWS_REQUIRE(n == tcn_train_num_params(d), "wekws_tcn_backward: expected %d parameters, got %d",
+                tcn_train_num_params(d), n);
+  WEKWS_REQUIRE(d_feats && h_params && d_saved && d_out && d_grad_out && h_grads && d_workspace,
+                "wekws_tcn_backward: null argument");
+  for (int i = 0; i < n; ++i)
+    WEKWS_REQUIRE(h_params[i] != nullptr && h_grads[i] != nullptr, "wekws_tcn_backward: parameter or gradient %d is "
+                  "null", i);
+  return tcn_backward_launch(d, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_out, d_grad_out, (int)B,
+                             (int)T, h_grads, d_workspace, (cudaStream_t)stream);
+}
+
+extern "C" int wekws_dropout_mask(uint64_t seed, int64_t B, int64_t T, int64_t C, int layer, uint32_t theta,
+                                  uint8_t* d_out, void* stream) {
+  WEKWS_REQUIRE(B >= 0 && T >= 0 && C >= 0 && B < (1LL << 31) && T < (1LL << 31) && C < (1LL << 31) && layer >= 0 &&
+                    theta <= (1u << 24), "wekws_dropout_mask: bad arguments");
+  WEKWS_REQUIRE(B * T * C == 0 || d_out, "wekws_dropout_mask: null output");
+  return dropout_mask_launch(seed, B, T, (int)C, layer, theta, d_out, (cudaStream_t)stream);
 }
 
 extern "C" int wekws_pipeline_forward(wekws_fbank* fb, wekws_model* m, const void* d_pcm, int pcm_dtype,

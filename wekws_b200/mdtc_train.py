@@ -12,7 +12,7 @@ version counters' back, so each training forward marks the packed eval model sta
 
 The opt-in exists because a BatchNorm model in training mode gives other outputs than in eval mode and overwrites its
 running statistics: a model left in ``train()`` by accident keeps refusing to run.  The MDTC backbone has no Dropout;
-the TCN / DS-TCN backbones and the ``global`` / ``last`` heads do, and are not supported.
+the TCN / DS-TCN backbones train through tcn_train.py, and the ``global`` / ``last`` heads are not supported.
 
 Refused: a non-empty streaming cache, features that require grad, ``forward_softmax``, ``momentum=None``, non-contiguous
 or non-float32 parameters, and double backward.
@@ -69,8 +69,9 @@ def check_trainable(model) -> None:
     bb = model.backbone
     kind = "gru" if isinstance(bb, nn.GRU) else getattr(bb, "kind", None)
     if kind in ("tcn", "ds_tcn"):
-        raise NotImplementedError(f"wekws_b200: training is not implemented for the {kind.upper().replace('_', '-')} "
-                                  "backbone (its Dropout inside the backbone needs random masks)")
+        raise NotImplementedError(f"wekws_b200: training the {kind.upper().replace('_', '-')} backbone applies Dropout "
+                                  "masks made on the device, not torch's Bernoulli draws: opt in with "
+                                  "model.enable_training(device_dropout=True)")
     if kind != "mdtc":
         raise NotImplementedError(f"wekws_b200: training is not implemented for the {str(kind).upper()} backbone")
     if model.head is not None:
@@ -98,29 +99,33 @@ def _pointers(tensors) -> C.Array:
     return (C.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
 
 
-def _params(model, dev: torch.device) -> List[torch.Tensor]:
+def _params(model, dev: torch.device, names: List[str] = None, what: str = "MDTC") -> List[torch.Tensor]:
+    """The parameters in native order (``names``, default the MDTC order), checked for the kernels."""
     named = dict(model.named_parameters())
-    names = param_names(model.backbone.num_stack, model.backbone.stack_size)
+    if names is None:
+        names = param_names(model.backbone.num_stack, model.backbone.stack_size)
     if list(named) != names:
-        raise RuntimeError("wekws_b200: MDTC training expects the parameters of wekws/model/kws_model.py with the MDTC "
-                           f"backbone and the linear classifier, in named_parameters order {names}; got {list(named)}")
+        raise RuntimeError(f"wekws_b200: {what} training expects the parameters of wekws/model/kws_model.py with the "
+                           f"{what} backbone and the linear classifier, in named_parameters order {names}; got "
+                           f"{list(named)}")
     params = [named[n] for n in names]
     for n, p in zip(names, params):
         if p.device != dev or p.dtype != torch.float32 or not p.is_contiguous():
-            raise ValueError(f"wekws_b200: MDTC training needs every parameter as a contiguous float32 tensor on "
+            raise ValueError(f"wekws_b200: {what} training needs every parameter as a contiguous float32 tensor on "
                              f"{dev}; {n} is {p.dtype} on {p.device}{'' if p.is_contiguous() else ', not contiguous'}")
     return params
 
 
-def _buffers(model, dev: torch.device):
-    """(CMVN mean / istd or Nones, running statistics in native order, (momentum, eps) per BatchNorm, counters)."""
+def _buffers(model, dev: torch.device, bns: List[nn.BatchNorm1d] = None, what: str = "MDTC"):
+    """(CMVN mean / istd or Nones, running statistics in native order, (momentum, eps) per BatchNorm, counters) of
+    the BatchNorms ``bns`` (default the MDTC ones)."""
     running, hyper, counters = [], [], []
-    for bn in batch_norms(model):
+    for bn in batch_norms(model) if bns is None else bns:
         if not bn.track_running_stats or bn.running_mean is None or not bn.affine:
-            raise ValueError("wekws_b200: MDTC training needs affine BatchNorms that track running statistics")
+            raise ValueError(f"wekws_b200: {what} training needs affine BatchNorms that track running statistics")
         for t in (bn.running_mean, bn.running_var):
             if t.device != dev or t.dtype != torch.float32 or not t.is_contiguous():
-                raise ValueError(f"wekws_b200: MDTC training needs the BatchNorm running statistics as contiguous "
+                raise ValueError(f"wekws_b200: {what} training needs the BatchNorm running statistics as contiguous "
                                  f"float32 tensors on {dev}")
         running += [bn.running_mean, bn.running_var]
         hyper += [float(bn.momentum), float(bn.eps)]
@@ -199,22 +204,23 @@ def wants_grad(model) -> bool:
     return torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters())
 
 
-def check_call(model, x: torch.Tensor, in_cache: torch.Tensor) -> None:
+def check_call(model, x: torch.Tensor, in_cache: torch.Tensor, bns: List[nn.BatchNorm1d] = None,
+               what: str = "MDTC") -> None:
     """The refusals that need no device: a streaming cache, features that require grad, a batch of one frame (torch's
-    own error), a BatchNorm with momentum=None."""
+    own error), a BatchNorm (of ``bns``, default the MDTC ones) with momentum=None."""
     if in_cache is not None and in_cache.numel() > 0:
-        raise ValueError("wekws_b200: MDTC training runs from empty caches (as Executor.train does); a streaming cache "
-                         "is not supported in training mode -- pass no in_cache, or call model.eval()")
+        raise ValueError(f"wekws_b200: {what} training runs from empty caches (as Executor.train does); a streaming "
+                         "cache is not supported in training mode -- pass no in_cache, or call model.eval()")
     if x.requires_grad:
-        raise ValueError("wekws_b200: MDTC training computes parameter gradients only; features that require grad "
+        raise ValueError(f"wekws_b200: {what} training computes parameter gradients only; features that require grad "
                          "are not supported (detach them)")
     if x.dim() == 3 and x.shape[0] * x.shape[1] <= 1:
         raise ValueError("Expected more than 1 value per channel when training, got input size "
                          f"{torch.Size([x.shape[0], model.hdim, x.shape[1]])}")
-    for bn in batch_norms(model):
+    for bn in batch_norms(model) if bns is None else bns:
         if bn.momentum is None:
             raise ValueError("wekws_b200: BatchNorm momentum=None (a cumulative moving average) is not supported in "
-                             "MDTC training; set a momentum")
+                             f"{what} training; set a momentum")
 
 
 def forward(model, x: torch.Tensor, in_cache: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
