@@ -14,8 +14,8 @@
 //     only keeps the weight ring and the loader's barriers in step.
 //
 // One CTA per SM holds ALL of its streams (up to 7 x 40 frames) resident for the whole network.  The residual stream is
-// CHANNEL-MINOR: X[col][64 ch] (256 B per frame column, every stream's cache slice in the columns directly in front of
-// its frames, so a dilated tap is a column offset), 16-byte chunks XOR-swizzled by (col & 7).
+// CHANNEL-MINOR: X[col][64 ch] (272 B per frame column: 256 B of channels and one 16-byte pad chunk that staggers the
+// banks; every stream's cache slice in the columns directly in front of its frames, so a dilated tap is a column offset).
 //
 // 19 warps: 16 compute (2 groups x 2 warpgroups), 1 weight ring warp, 2 loaders (cache slices by 2-D TMA tensor copies
 // into landing slots, transposed into X).
@@ -25,7 +25,7 @@
 #include "mdtc_tc.h"
 #include "tc_common.cuh"
 
-// per-phase cycle counters of the loaders (debug builds with -DMDTC_TIMING=1 only)
+// per-phase cycle counters of the loaders and of one compute warp per group (debug builds with -DMDTC_TIMING=1 only)
 #ifndef MDTC_TIMING
 #define MDTC_TIMING 0
 #endif
@@ -49,19 +49,21 @@ constexpr int W_LD = W_WGT + 1;            // warps 17..18: cache loaders, one p
 constexpr int NT_TC = (W_LD + NG) * 32;    // 608 threads -> up to 104 registers per thread (accumulator 32 + A 32)
 constexpr int C = 64;
 constexpr int XCOLS = 504;                 // frame columns of X (n_streams * Lw <= XCOLS)
-constexpr int X_BYTES = XCOLS * 256;       // 129024: X[col][64] fp32
+constexpr int X_COL = 272;                 // bytes per frame column of X: 64 fp32 + one 16-byte pad chunk
+constexpr int X_BYTES = XCOLS * X_COL;     // 137088
 constexpr int STG_FLOATS = 64 * 32;        // TMA landing slot: one stream's cache slice [64][pad <= 32]
 constexpr int NSLOT = 7;                   // TMA landing slots, shared out among the tiles' loaders by stream count
+constexpr int NSLOT_HEAD = 6;              // the head variant gives one slot's room to its pool
 constexpr int W_SLOT = 16384;              // hi + lo image of one 64x64 matrix
-constexpr int OFF_X = 0;
-constexpr int OFF_STG = OFF_X + X_BYTES;                   // 129024
-constexpr int OFF_W = OFF_STG + NSLOT * STG_FLOATS * 4;    // 186368 (1024-aligned: SWIZZLE_128B images)
-constexpr int OFF_END = OFF_W + 2 * W_SLOT;                // 219136
-constexpr int SMEM_TOTAL = OFF_END + 1024;                 // incl. alignment slack
+constexpr int OFF_W = 0;                                   // 1024-aligned: SWIZZLE_128B images
+constexpr int OFF_X = OFF_W + 2 * W_SLOT;                  // 32768
+constexpr int OFF_STG = OFF_X + X_BYTES;                   // 169856 (128-aligned: TMA destination)
+constexpr int OFF_WC = OFF_STG + NSLOT * STG_FLOATS * 4;            // per-frame classifier weights [64][odim <= 8]
+constexpr int SMEM_TOTAL = OFF_WC + C * 8 * 4 + 1024;                // 230272, incl. alignment slack
 constexpr int POOL_SPT = 16;                               // streams per tile at the shortest chunk (T = 8)
-constexpr int OFF_POOL = OFF_END;                          // head variant: pooled sums [NG][POOL_SPT][64]
-constexpr int SMEM_TOTAL_HEAD = OFF_POOL + NG * POOL_SPT * C * 4 + 1024;
-static_assert(OFF_W % 1024 == 0, "weight images must be 1024-byte aligned");
+constexpr int OFF_POOL = OFF_STG + NSLOT_HEAD * STG_FLOATS * 4;       // head variant: pooled sums [NG][POOL_SPT][64]
+constexpr int SMEM_TOTAL_HEAD = OFF_POOL + NG * POOL_SPT * C * 4 + 1024;   // 228224
+static_assert(OFF_W % 1024 == 0 && OFF_X % 128 == 0 && OFF_STG % 128 == 0, "misaligned shared-memory region");
 static_assert(SMEM_TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 static_assert(SMEM_TOTAL_HEAD <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 
@@ -77,9 +79,15 @@ __device__ __forceinline__ float2 lds_f2(uint32_t addr) {
 __device__ __forceinline__ void sts_f2(uint32_t addr, float x, float y) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
 }
-// Layout of X: frame column col holds its 64 channels in 256 bytes; the 16-byte chunk with channels 8m..8m+3 sits at
-// chunk (m ^ (col & 7)) of the first 128 bytes, channels 8m+4..8m+7 at the same chunk of the second 128 bytes:
-//   address(col, 8m + 4h + u) = xs + ((col << 8) | ((col & 7) << 4)) ^ (m << 4)  +  128 h  +  4 u
+// Layout of X: frame column col holds its 64 channels in the first 256 of its X_COL = 272 bytes; the 16-byte chunk with
+// channels 8m..8m+3 sits at byte 16 m, channels 8m+4..8m+7 at 128 + 16 m:
+//   address(col, 8m + 4h + u) = xs + 272 col + 16 m + 128 h + 4 u
+// Chunk m of column col falls in bank group (col + m) mod 8, so for a fixed m the columns spread over the banks as they
+// would under an XOR swizzle (tests/test_mdtc_x_layout.py counts every access pattern), while the chunk offset 16 m
+// stays an immediate of the load: x_addr(xs, col, 8 m + r) == x_addr(xs, col, r) + 16 m for r < 8.
+__device__ __forceinline__ uint32_t x_addr(uint32_t xs, int col, int ch) {
+  return xs + (uint32_t)col * X_COL + 16u * (uint32_t)(ch >> 3) + 128u * (uint32_t)((ch >> 2) & 1) + 4u * (uint32_t)(ch & 3);
+}
 // 2-D TMA tensor copy global -> shared (box given by the tensor map), completion on an mbarrier
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, int c0, int c1, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
@@ -125,7 +133,7 @@ __device__ __noinline__ void weights_role(const TcArgs& a, uint8_t* base, Bars B
 // time on halo_bar with two loaders walking the tiles in order).  The tile's ring of `nsl` landing slots is refilled
 // the moment a slot is drained, i.e. the copy for the same stream of the NEXT block is in flight a whole block ahead.
 __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B, int i, int lane, int K, int ns, int b0,
-                                         int ntile, uint32_t& hf_par) {
+                                         int ntile, int nslot, uint32_t& hf_par) {
   if (i >= ntile) return;
   float* STG = reinterpret_cast<float*>(base + OFF_STG);
   const uint32_t xs = smem_u32(base) + OFF_X;
@@ -133,14 +141,14 @@ __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B,
   const int nst = min(spt, ns - i * spt), sg0 = i * spt;          // my streams: sg0 .. sg0 + nst
   const int njobs = a.nblocks * nst;
   const bool have_cache = a.in_cache != nullptr;
-  // landing slots of tile t: the streams' share of the NSLOT slots (each tile at least one; ns <= NSLOT: one per stream)
+  // landing slots of tile t: the streams' share of the nslot slots (each tile at least one; ns <= nslot: one per stream)
   int slot0 = 0, nsl = 1;
   {
     int used = 0;
     for (int t = 0; t < ntile; ++t) {
       const int n_t = min(spt, ns - t * spt);
-      int want = ns <= NSLOT ? n_t : max(1, (NSLOT * n_t) / ns);
-      const int left = NSLOT - used - (ntile - 1 - t);               // keep one slot for every later tile
+      int want = ns <= nslot ? n_t : max(1, (nslot * n_t) / ns);
+      const int left = nslot - used - (ntile - 1 - t);               // keep one slot for every later tile
       if (want > left) want = left;
       if (t == i) { slot0 = used; nsl = want; }
       used += want;
@@ -177,12 +185,11 @@ __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B,
       const int cq = r >> lgg, jg = r & ((1 << lgg) - 1);
       const float4* s4 = reinterpret_cast<const float4*>(slotp + 4 * cq * pad + 4 * jg);
       const float4 r0 = s4[0], r1 = s4[pad >> 2], r2 = s4[2 * (pad >> 2)], r3 = s4[3 * (pad >> 2)];
-      const uint32_t sw = ((uint32_t)(cq >> 1) << 4), hi = (uint32_t)(cq & 1) * 128u;
-      uint32_t col = (uint32_t)(colb + 4 * jg);
-      sts_2x2(((xs + (col << 8) + ((col & 7u) << 4)) ^ sw) + hi, pack2(r0.x, r1.x), pack2(r2.x, r3.x)); ++col;
-      sts_2x2(((xs + (col << 8) + ((col & 7u) << 4)) ^ sw) + hi, pack2(r0.y, r1.y), pack2(r2.y, r3.y)); ++col;
-      sts_2x2(((xs + (col << 8) + ((col & 7u) << 4)) ^ sw) + hi, pack2(r0.z, r1.z), pack2(r2.z, r3.z)); ++col;
-      sts_2x2(((xs + (col << 8) + ((col & 7u) << 4)) ^ sw) + hi, pack2(r0.w, r1.w), pack2(r2.w, r3.w));
+      const uint32_t d = x_addr(xs, colb + 4 * jg, 4 * cq);
+      sts_2x2(d, pack2(r0.x, r1.x), pack2(r2.x, r3.x));
+      sts_2x2(d + X_COL, pack2(r0.y, r1.y), pack2(r2.y, r3.y));
+      sts_2x2(d + 2 * X_COL, pack2(r0.z, r1.z), pack2(r2.z, r3.z));
+      sts_2x2(d + 3 * X_COL, pack2(r0.w, r1.w), pack2(r2.w, r3.w));
     };
     if (have_cache && nsl >= nst) {
       // every stream of the tile has its own landing slot: wait for all of them (they were requested a block ago), move
@@ -224,7 +231,7 @@ __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B,
         }
       } else {
         const f32x2 z = 0ull;
-        for (int e = lane; e < pad * 16; e += 32) sts_2x2(xs + ((uint32_t)colb << 8) + 16u * (uint32_t)e, z, z);
+        for (int e = lane; e < pad * 16; e += 32) sts_2x2(x_addr(xs, colb + (e >> 4), 4 * (e & 15)), z, z);
       }
     }
     __syncwarp();
@@ -248,6 +255,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
   uint8_t* base = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);
   __shared__ uint64_t halo_bar[NG], h_free[NG];
   __shared__ uint64_t w_bar[2], w_free[2], stg_bar[NSLOT];
+  constexpr int nslot = HEAD ? NSLOT_HEAD : NSLOT;
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform for the compiler too (no divergence regions around the roles)
@@ -262,6 +270,12 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
     for (int i = 0; i < NG; ++i) { mbar_init(&halo_bar[i], 1); mbar_init(&h_free[i], WPG); }
     for (int i = 0; i < 2; ++i) { mbar_init(&w_bar[i], 1); mbar_init(&w_free[i], NCW); }
     mbar_fence_init();
+  }
+  if constexpr (!HEAD) {
+    // the classifier weights in shared memory: the stack-end partial sums read them right after each residual store,
+    // where a global load's latency is exposed once per fragment column (measured: 15 % of the flagship step)
+    float* wcs = reinterpret_cast<float*>(base + OFF_WC);
+    for (int i = tid; i < C * a.odim; i += NT_TC) wcs[i] = __ldg(vec + a.v_wc + i);
   }
   __syncthreads();
   const Bars bars{halo_bar, h_free, w_bar, w_free, stg_bar};
@@ -289,7 +303,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
 
     // the landing slots are dealt out per pass (by stream count): their barriers start every pass from phase 0
     if (tid == 0) {
-      for (int i = 0; i < NSLOT; ++i) mbar_init(&stg_bar[i], 1);
+      for (int i = 0; i < nslot; ++i) mbar_init(&stg_bar[i], 1);
       mbar_fence_init();
     }
     __syncthreads();
@@ -306,10 +320,9 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
       if (grp < ntile && wq < nlw) {
         const int nst = tile_streams(grp), rows = nst * T;
         const int q4 = lane & 3, r0 = 64 * (wq >> 2) + 16 * (wq & 3) + (lane >> 2);
-        const uint32_t qoff = 128u * (uint32_t)(q4 >> 1) + 8u * (uint32_t)(q4 & 1);   // channel pair 2 q4 inside a chunk
         bool live[2];
         int col[2], sgr[2], ttr[2];
-        uint32_t t_own[2];
+        uint32_t t_own[2];                                 // X address of the row's channel pair 2 q4 (chunk 0)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = r0 + 8 * h;
@@ -318,7 +331,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           ttr[h] = live[h] ? row - s * T : 0;
           sgr[h] = grp * spt + s;                          // stream index inside the pass
           col[h] = sgr[h] * Lw + PADR + ttr[h];            // this row's frame column (dead rows alias a valid one)
-          t_own[h] = xs + ((uint32_t)col[h] << 8) + (((uint32_t)col[h] & 7u) << 4);
+          t_own[h] = x_addr(xs, col[h], 2 * q4);
         }
         const float* cwf = reinterpret_cast<const float*>(&a.cw[0][0]);
         constexpr int CWS = 7 * 64;                        // floats per block in cw
@@ -390,10 +403,16 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
 #pragma unroll
           for (int h = 0; h < 2; ++h)
             if (live[h])
-              sts_f2(((t_own[h] ^ ((uint32_t)j << 4)) + qoff), fmaxf(acc[4 * j + 2 * h] + b.x, 0.f), fmaxf(acc[4 * j + 2 * h + 1] + b.y, 0.f));
+              sts_f2(t_own[h] + 16u * j, fmaxf(acc[4 * j + 2 * h] + b.x, 0.f), fmaxf(acc[4 * j + 2 * h + 1] + b.y, 0.f));
         }
         group_barrier(grp, nlw);                // X of the tile complete before the first depthwise conv reads across rows
 
+#if MDTC_TIMING
+        // halo wait, depthwise conv, cache stores, GEMM1 (incl. weight wait), epilogue 1, GEMM2, first barrier,
+        // epilogue 2, second barrier
+        long long t_halo = 0, t_dw = 0, t_cache = 0, t_g1 = 0, t_e1 = 0, t_g2 = 0, t_bar1 = 0, t_e2 = 0, t_bar2 = 0;
+        long long t_last_ = clock64();
+#endif
         // ---- blocks
         for (int blk = 0; blk < a.nblocks; ++blk) {
           const int d = a.dil[blk], pad = d * (K - 1);
@@ -402,14 +421,14 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           // ---------------- depthwise dilated conv (+folded BN) -> A fragments                 (mdtc.py:56-57)
           mbar_wait(&halo_bar[grp], halo_par);
           halo_par ^= 1;
+          TPH(t_halo)
           {
             uint32_t tj[2][5];
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
               for (int j = 0; j < 5; ++j) {
-                const uint32_t cj = (uint32_t)(col[h] - pad + j * d);
-                tj[h][j] = xs + (cj << 8) + ((cj & 7u) << 4);
+                tj[h][j] = x_addr(xs, col[h] - pad + j * d, 2 * q4);
               }
 #pragma unroll
             for (int k = 0; k < 4; ++k)
@@ -422,7 +441,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
 #pragma unroll
                 for (int j = 0; j < 5; ++j) {
                   if (KT ? j < KT : j < K) {
-                    const float2 x = lds_f2((tj[h][j] ^ ((uint32_t)m << 4)) + qoff);
+                    const float2 x = lds_f2(tj[h][j] + 16u * m);
                     s0 = fmaf(x.x, cwb[64 * j + ch], s0);
                     s1 = fmaf(x.y, cwb[64 * j + ch + 1], s1);
                   }
@@ -433,22 +452,24 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           // this warp is done with the block's cache columns in front of the frames: when the new cache slice is made of
           // frame columns only (T >= pad) the loader may start transposing the next block's slices now, not after the
           // stores below (which read those columns when T < pad)
+          TPH(t_dw)
           const bool early_free = T >= pad;
           __syncwarp();
           if (early_free && lane == 0) mbar_arrive(&h_free[grp]);
           // ---------------- new cache slices of this tile: out_cache[b][c][off + j] = cat[c][T + j] (mdtc.py:113).
-          // A warp reads 8 columns x 4 channels per request (conflict-free in the swizzled layout); 8 lanes write 32
-          // contiguous bytes of one cache row.
+          // A warp reads jpl columns x 32 / jpl channel quads per request; 8 lanes write 32 contiguous bytes of one
+          // cache row.  Quad cq = 2 m + h takes the chunk index m = q >> 1 rotated left by one bit, so the chunks of one
+          // request spread over the bank groups (col + m) mod 8: conflict-free for 4- and 8-column slices too.
           {
             const int off = a.coff[blk];
             const int jpl = pad < 32 ? pad : 32, lgj = 31 - __clz(jpl), qstep = 32 >> lgj;
             const int j = lane & (jpl - 1), qs = lane >> lgj, per = 16 >> (5 - lgj);      // quads passes per stream
             const int nitem = nst * per;
             for (int it = wq; it < nitem; it += nlw) {
-              const int s2 = it / per, cq = (it - s2 * per) * qstep + qs;
+              const int s2 = it / per, q = (it - s2 * per) * qstep + qs, mq = q >> 1;
+              const int cq = 2 * (((mq << 1) | (mq >> 2)) & 7) + (q & 1);
               const int sg2 = grp * spt + s2;
-              const uint32_t cc = (uint32_t)(sg2 * Lw + PADR + T - pad + j);
-              const uint32_t src = ((xs + (cc << 8) + ((cc & 7u) << 4)) ^ ((uint32_t)(cq >> 1) << 4)) + (uint32_t)(cq & 1) * 128u;
+              const uint32_t src = x_addr(xs, sg2 * Lw + PADR + T - pad + j, 4 * cq);
               f32x2 v01, v23;
               lds_2x2(src, v01, v23);
               float v0, v1, v2, v3;
@@ -462,8 +483,10 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
               if (lane == 0) mbar_arrive(&h_free[grp]);    // the tile's cache columns may be overwritten
             }
           }
+          TPH(t_cache)
           // ---------------- pointwise-1 GEMM, h = relu(D + b1) -> A fragments                 (mdtc.py:115)
           gemm(0, 4, true);
+          TPH(t_g1)
 #pragma unroll
           for (int k = 0; k < 4; ++k)
 #pragma unroll
@@ -472,28 +495,33 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
               split_pair_rz_relu(pack2(acc[i] + cwb[5 * 64 + ch], acc[i + 1] + cwb[5 * 64 + ch + 1]), ahi[k][p], alo[k][p]);
             }
           // ---------------- pointwise-2 GEMM; x' = relu(D + b2 + x) -> X; classifier partial sums at the end of a stack
+          TPH(t_e1)
           gemm(1, 4, true);                                                    // (mdtc.py:116-118, 266-273)
+          TPH(t_g2)
           group_barrier(grp, nlw);              // every row's depthwise taps and cache stores have read x
+          TPH(t_bar1)
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int ch = 8 * j + 2 * q4;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              const uint32_t ax = (t_own[h] ^ ((uint32_t)j << 4)) + qoff;
+              const uint32_t ax = t_own[h] + 16u * j;
               const float2 r = lds_f2(ax);
               const float o0 = fmaxf(acc[4 * j + 2 * h] + cwb[6 * 64 + ch] + r.x, 0.f);
               const float o1 = fmaxf(acc[4 * j + 2 * h + 1] + cwb[6 * 64 + ch + 1] + r.y, 0.f);
               if (live[h]) sts_f2(ax, o0, o1);
               if (!HEAD && stack_end) {
                 // the classifier is linear: W_c (sum of stack outputs) = sum of W_c (stack output)
-                const float* wc = vec + a.v_wc + ch * a.odim;
+                const float* wc = reinterpret_cast<const float*>(base + OFF_WC) + ch * a.odim;
 #pragma unroll
                 for (int jo = 0; jo < 8; ++jo)
-                  if (jo < a.odim) part[h][jo] = fmaf(__ldg(wc + a.odim + jo), o1, fmaf(__ldg(wc + jo), o0, part[h][jo]));
+                  if (jo < a.odim) part[h][jo] = fmaf(wc[a.odim + jo], o1, fmaf(wc[jo], o0, part[h][jo]));
               }
             }
           }
+          TPH(t_e2)
           group_barrier(grp, nlw);              // x' of every row of the tile complete before the next block's conv
+          TPH(t_bar2)
           if constexpr (HEAD) {
             // X now holds the stack output of every frame of the tile, and stays so until the next block's second
             // group barrier.  Warp wq sums channels 8 wq .. 8 wq + 7; lane = 8 q + channel, q = frame phase mod 4:
@@ -501,16 +529,13 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             // over the stacks in the shared pool buffer (always the same thread: no barrier, no atomics)
             if (stack_end && a.pool_t1 > a.pool_t0) {
               const int c = 8 * wq + (lane & 7), q = lane >> 3;
-              const uint32_t cofs = 128u * (uint32_t)((c >> 2) & 1) + 4u * (uint32_t)(c & 3);
               float* pl = reinterpret_cast<float*>(base + OFF_POOL) + grp * POOL_SPT * C;
               for (int s2 = 0; s2 < nst; ++s2) {
                 const int colb = (grp * spt + s2) * Lw + PADR;
                 float v = 0.f;
                 for (int t = a.pool_t0 + q; t < a.pool_t1; t += 4) {
-                  const uint32_t cc = (uint32_t)(colb + t);
                   float x;
-                  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
-                               : "r"(((xs + (cc << 8) + ((cc & 7u) << 4)) ^ ((uint32_t)(c >> 3) << 4)) + cofs));
+                  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(x_addr(xs, colb + t, c)));
                   v += x;
                 }
                 v += __shfl_xor_sync(0xffffffffu, v, 8);
@@ -520,6 +545,12 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             }
           }
         }
+#if MDTC_TIMING
+        if (blockIdx.x == 0 && wq == 0 && lane == 0)
+          printf("group %d (%d rows, pass at stream %d): halo %lld dw %lld cache %lld gemm1 %lld epi1 %lld gemm2 %lld "
+                 "bar1 %lld epi2 %lld bar2 %lld\n", grp, rows, b0, t_halo, t_dw, t_cache, t_g1, t_e1, t_g2, t_bar1, t_e2,
+                 t_bar2);
+#endif
         if constexpr (HEAD) {
           // the stream's pooled vector: the first time-chunk of the call stores, later ones add (stream-ordered launches)
           if (a.pool_t1 > a.pool_t0 && lane < 8) {
@@ -578,7 +609,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
     } else if (warp == W_WGT) {
       if (lane == 0) weights_role(a, base, bars, K, natoms, wf_par, b0 == sb);
     } else {
-      loader_role(a, base, bars, warp - W_LD, lane, K, ns, b0, ntile, hf_par);
+      loader_role(a, base, bars, warp - W_LD, lane, K, ns, b0, ntile, nslot, hf_par);
     }
     __syncthreads();       // pass boundary: X, the landing slots and the rings are reused
   }
