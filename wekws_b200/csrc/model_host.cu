@@ -1005,6 +1005,40 @@ int mdtc_train_dims(const wekws_model* m, const char* what, MdtcTrainDims* d) {
   return WEKWS_OK;
 }
 
+// The arguments of a batch-statistics training forward (MDTC, TCN / DS-TCN) of a model of width C and output width
+// odim with n_expected parameters and nbn BatchNorms.
+int batch_stats_forward_check(const char* what, int64_t B, int64_t T, int C, int odim, int n, int n_expected, int nbn,
+                              const float* d_feats, const float* const* h_params, const float* d_cmvn_mean,
+                              const float* d_cmvn_istd, float* const* h_running, const double* h_bn,
+                              const float* d_out, const float* d_out_cache, const float* d_saved, int save,
+                              const void* d_workspace) {
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * C < (1LL << 31) && B * T * odim < (1LL << 31),
+                "%s: B = %lld, T = %lld unsupported (B * T >= 2 frames are needed for batch statistics)", what,
+                (long long)B, (long long)T);
+  WEKWS_REQUIRE(n == n_expected, "%s: expected %d parameters, got %d", what, n_expected, n);
+  WEKWS_REQUIRE(d_feats && h_params && h_running && h_bn && d_out && d_out_cache && d_workspace && (!save || d_saved),
+                "%s: null argument", what);
+  WEKWS_REQUIRE((d_cmvn_mean == nullptr) == (d_cmvn_istd == nullptr), "%s: pass both CMVN buffers or neither", what);
+  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_params[i] != nullptr, "%s: parameter %d is null", what, i);
+  for (int i = 0; i < 2 * nbn; ++i) WEKWS_REQUIRE(h_running[i] != nullptr, "%s: running statistic %d is null", what, i);
+  for (int i = 0; i < nbn; ++i)
+    WEKWS_REQUIRE(h_bn[2 * i] >= 0.0 && h_bn[2 * i] <= 1.0 && h_bn[2 * i + 1] > 0.0,
+                  "%s: BatchNorm %d has momentum %g, eps %g", what, i, h_bn[2 * i], h_bn[2 * i + 1]);
+  return WEKWS_OK;
+}
+
+// The arguments of its backward; args_present: every pointer argument but the parameters and gradients is non-null.
+int batch_stats_backward_check(const char* what, int64_t B, int64_t T, int C, int odim, int n, int n_expected,
+                               const float* const* h_params, float* const* h_grads, bool args_present) {
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * C < (1LL << 31) && B * T * odim < (1LL << 31),
+                "%s: bad B/T", what);
+  WEKWS_REQUIRE(n == n_expected, "%s: expected %d parameters, got %d", what, n_expected, n);
+  WEKWS_REQUIRE(args_present && h_params && h_grads, "%s: null argument", what);
+  for (int i = 0; i < n; ++i)
+    WEKWS_REQUIRE(h_params[i] != nullptr && h_grads[i] != nullptr, "%s: parameter or gradient %d is null", what, i);
+  return WEKWS_OK;
+}
+
 }  // namespace
 
 extern "C" int wekws_mdtc_num_params(const wekws_model* m) {
@@ -1051,23 +1085,13 @@ extern "C" int wekws_mdtc_train_forward(const wekws_model* m, const float* d_fea
                                         const double* h_bn, float* d_out, float* d_out_cache, float* d_saved, int save,
                                         void* d_workspace, int64_t B, int64_t T, void* stream) {
   MdtcTrainDims d;
-  int rc = mdtc_train_dims(m, "wekws_mdtc_train_forward", &d);
+  const char* what = "wekws_mdtc_train_forward";
+  int rc = mdtc_train_dims(m, what, &d);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31),
-                "wekws_mdtc_train_forward: B = %lld, T = %lld unsupported (B * T >= 2 frames are needed for batch "
-                "statistics)", (long long)B, (long long)T);
-  WEKWS_REQUIRE(n == mdtc_train_num_params(d.L), "wekws_mdtc_train_forward: expected %d parameters, got %d",
-                mdtc_train_num_params(d.L), n);
-  WEKWS_REQUIRE(d_feats && h_params && h_running && h_bn && d_out && d_out_cache && d_workspace && (!save || d_saved),
-                "wekws_mdtc_train_forward: null argument");
-  WEKWS_REQUIRE((d_cmvn_mean == nullptr) == (d_cmvn_istd == nullptr),
-                "wekws_mdtc_train_forward: pass both CMVN buffers or neither");
-  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_params[i] != nullptr, "wekws_mdtc_train_forward: parameter %d is null", i);
-  for (int i = 0; i < 6 * d.L; ++i)
-    WEKWS_REQUIRE(h_running[i] != nullptr, "wekws_mdtc_train_forward: running statistic %d is null", i);
-  for (int i = 0; i < 3 * d.L; ++i)
-    WEKWS_REQUIRE(h_bn[2 * i] >= 0.0 && h_bn[2 * i] <= 1.0 && h_bn[2 * i + 1] > 0.0,
-                  "wekws_mdtc_train_forward: BatchNorm %d has momentum %g, eps %g", i, h_bn[2 * i], h_bn[2 * i + 1]);
+  if ((rc = batch_stats_forward_check(what, B, T, d.C, d.odim, n, mdtc_train_num_params(d.L), 3 * d.L, d_feats,
+                                      h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache, d_saved,
+                                      save, d_workspace)))
+    return rc;
   return mdtc_train_forward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache,
                                    save ? d_saved : nullptr, d_workspace, (int)B, (int)T, (cudaStream_t)stream);
 }
@@ -1077,16 +1101,12 @@ extern "C" int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, c
                                    const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads,
                                    void* d_workspace, void* stream) {
   MdtcTrainDims d;
-  int rc = mdtc_train_dims(m, "wekws_mdtc_backward", &d);
+  const char* what = "wekws_mdtc_backward";
+  int rc = mdtc_train_dims(m, what, &d);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31), "wekws_mdtc_backward: bad B/T");
-  WEKWS_REQUIRE(n == mdtc_train_num_params(d.L), "wekws_mdtc_backward: expected %d parameters, got %d",
-                mdtc_train_num_params(d.L), n);
-  WEKWS_REQUIRE(d_feats && h_params && d_saved && d_grad_out && h_grads && d_workspace,
-                "wekws_mdtc_backward: null argument");
-  for (int i = 0; i < n; ++i)
-    WEKWS_REQUIRE(h_params[i] != nullptr && h_grads[i] != nullptr, "wekws_mdtc_backward: parameter or gradient %d is "
-                  "null", i);
+  if ((rc = batch_stats_backward_check(what, B, T, d.C, d.odim, n, mdtc_train_num_params(d.L), h_params, h_grads,
+                                       d_feats && d_saved && d_grad_out && d_workspace)))
+    return rc;
   return mdtc_backward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B, (int)T,
                               h_grads, d_workspace, (cudaStream_t)stream);
 }
@@ -1179,25 +1199,14 @@ extern "C" int wekws_tcn_train_forward(const wekws_model* m, const float* d_feat
                                        int64_t T, void* stream) {
   TcnTrainDims d;
   TcnDropout drop;
-  int rc = tcn_train_dims(m, "wekws_tcn_train_forward", &d);
+  const char* what = "wekws_tcn_train_forward";
+  int rc = tcn_train_dims(m, what, &d);
   if (rc) return rc;
-  if ((rc = tcn_dropout(d, seed, h_p, "wekws_tcn_train_forward", &drop))) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31) && B * T * d.odim < (1LL << 31),
-                "wekws_tcn_train_forward: B = %lld, T = %lld unsupported (B * T >= 2 frames are needed for batch "
-                "statistics)", (long long)B, (long long)T);
-  WEKWS_REQUIRE(n == tcn_train_num_params(d), "wekws_tcn_train_forward: expected %d parameters, got %d",
-                tcn_train_num_params(d), n);
-  WEKWS_REQUIRE(d_feats && h_params && h_running && h_bn && d_out && d_out_cache && d_workspace && (!save || d_saved),
-                "wekws_tcn_train_forward: null argument");
-  WEKWS_REQUIRE((d_cmvn_mean == nullptr) == (d_cmvn_istd == nullptr),
-                "wekws_tcn_train_forward: pass both CMVN buffers or neither");
-  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_params[i] != nullptr, "wekws_tcn_train_forward: parameter %d is null", i);
-  const int nbn = tcn_train_num_bns(d);
-  for (int i = 0; i < 2 * nbn; ++i)
-    WEKWS_REQUIRE(h_running[i] != nullptr, "wekws_tcn_train_forward: running statistic %d is null", i);
-  for (int i = 0; i < nbn; ++i)
-    WEKWS_REQUIRE(h_bn[2 * i] >= 0.0 && h_bn[2 * i] <= 1.0 && h_bn[2 * i + 1] > 0.0,
-                  "wekws_tcn_train_forward: BatchNorm %d has momentum %g, eps %g", i, h_bn[2 * i], h_bn[2 * i + 1]);
+  if ((rc = tcn_dropout(d, seed, h_p, what, &drop))) return rc;
+  if ((rc = batch_stats_forward_check(what, B, T, d.C, d.odim, n, tcn_train_num_params(d), tcn_train_num_bns(d),
+                                      d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache,
+                                      d_saved, save, d_workspace)))
+    return rc;
   return tcn_train_forward_launch(d, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out,
                                   d_out_cache, save ? d_saved : nullptr, d_workspace, (int)B, (int)T,
                                   (cudaStream_t)stream);
@@ -1209,18 +1218,13 @@ extern "C" int wekws_tcn_backward(const wekws_model* m, const float* d_feats, co
                                   int64_t B, int64_t T, float* const* h_grads, void* d_workspace, void* stream) {
   TcnTrainDims d;
   TcnDropout drop;
-  int rc = tcn_train_dims(m, "wekws_tcn_backward", &d);
+  const char* what = "wekws_tcn_backward";
+  int rc = tcn_train_dims(m, what, &d);
   if (rc) return rc;
-  if ((rc = tcn_dropout(d, seed, h_p, "wekws_tcn_backward", &drop))) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B * T >= 2 && B * T * d.C < (1LL << 31) && B * T * d.odim < (1LL << 31),
-                "wekws_tcn_backward: bad B/T");
-  WEKWS_REQUIRE(n == tcn_train_num_params(d), "wekws_tcn_backward: expected %d parameters, got %d",
-                tcn_train_num_params(d), n);
-  WEKWS_REQUIRE(d_feats && h_params && d_saved && d_out && d_grad_out && h_grads && d_workspace,
-                "wekws_tcn_backward: null argument");
-  for (int i = 0; i < n; ++i)
-    WEKWS_REQUIRE(h_params[i] != nullptr && h_grads[i] != nullptr, "wekws_tcn_backward: parameter or gradient %d is "
-                  "null", i);
+  if ((rc = tcn_dropout(d, seed, h_p, what, &drop))) return rc;
+  if ((rc = batch_stats_backward_check(what, B, T, d.C, d.odim, n, tcn_train_num_params(d), h_params, h_grads,
+                                       d_feats && d_saved && d_out && d_grad_out && d_workspace)))
+    return rc;
   return tcn_backward_launch(d, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_out, d_grad_out, (int)B,
                              (int)T, h_grads, d_workspace, (cudaStream_t)stream);
 }

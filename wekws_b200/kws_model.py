@@ -11,9 +11,9 @@ The modules in here are parameter HOLDERS only.  ``forward`` hands raw device po
 the C-ABI library (include/wekws_b200.h) whose fused sm_90a kernels do all the work:
 CMVN -> Linear+ReLU -> backbone with streaming cache -> classifier -> activation
 (kws_model.py:65-76).  There is no PyTorch / CPU fallback: CPU tensors, training mode or a missing native library
-raise.  Training runs on the device for the FSMN model (fsmn_train.py), after ``enable_training()`` for the MDTC
-model with the per-frame linear classifier (mdtc_train.py), and after ``enable_training(device_dropout=True)`` for the
-TCN / DS-TCN models with the per-frame linear classifier (tcn_train.py).
+raise.  Training runs on the device (training.py) for the FSMN model, after ``enable_training()`` for the MDTC model
+with the per-frame linear classifier, and after ``enable_training(device_dropout=True)`` for the TCN / DS-TCN models
+with the per-frame linear classifier.
 """
 from __future__ import annotations
 
@@ -24,7 +24,7 @@ from typing import Optional, Tuple
 import torch
 import torch.nn as nn
 
-from . import _native, fsmn_train, mdtc_train, tcn_train
+from . import _native, training
 from .cmvn import load_cmvn, load_kaldi_cmvn
 
 _EMPTY = torch.zeros(0, 0, 0, dtype=torch.float)
@@ -352,8 +352,8 @@ class KWSModel(nn.Module):
 
     # ------------------------------------------------------------------------- training
     def enable_training(self, device_dropout: bool = False) -> "KWSModel":
-        """Lets ``train()`` mode run the training forward of the MDTC model (mdtc_train.py) or, with
-        ``device_dropout=True``, of the TCN / DS-TCN model (tcn_train.py), each with the per-frame linear classifier:
+        """Lets ``train()`` mode run the training forward (training.py) of the MDTC model or, with
+        ``device_dropout=True``, of the TCN / DS-TCN model, each with the per-frame linear classifier:
         batch statistics, running-statistics updates, gradients for ``loss.backward()``.  Without it a BatchNorm model
         in training mode refuses to run, so a model left in ``train()`` by accident cannot silently give training-mode
         outputs or overwrite its running statistics.  ``device_dropout=True`` accepts Dropout masks made on the device
@@ -361,14 +361,9 @@ class KWSModel(nn.Module):
         (NotImplementedError without), and it changes nothing for the MDTC and FSMN models.  A no-op for the FSMN
         model, whose training needs no opt-in; NotImplementedError for the ``global`` / ``last`` heads and for the
         GRU.  Not part of the state_dict; kept by copies and pickles."""
-        kind = getattr(self.backbone, "kind", None)
-        if kind in ("tcn", "ds_tcn") and device_dropout:
-            tcn_train.check_trainable(self)
-            self._training_enabled = self._device_dropout = True
-        elif kind != "fsmn":
-            mdtc_train.check_trainable(self)
-            self._training_enabled = True
-            self._device_dropout = bool(device_dropout)
+        training.check_trainable(self, device_dropout)
+        if getattr(self.backbone, "kind", None) != "fsmn":
+            self._training_enabled, self._device_dropout = True, bool(device_dropout)
         return self
 
     # ------------------------------------------------------------------------- forward
@@ -381,29 +376,7 @@ class KWSModel(nn.Module):
         return self._handle
 
     def _run(self, x: torch.Tensor, in_cache: torch.Tensor, flags: int) -> Tuple[torch.Tensor, torch.Tensor]:
-        train_fsmn = train_mdtc = train_tcn = False
-        if self.training:
-            kind = getattr(self.backbone, "kind", None)
-            # FSMN: the training-mode forward is the eval forward (no BatchNorm; its Dropout is never called), so under
-            # no_grad it takes the eval path; with grad it builds the graph (fsmn_train.py).  MDTC after
-            # enable_training(), TCN / DS-TCN after enable_training(device_dropout=True): the batch-statistics forward,
-            # with or without grad (mdtc_train.py, tcn_train.py).
-            enabled = self.__dict__.get("_training_enabled", False)
-            train_mdtc = kind == "mdtc" and enabled
-            train_tcn = kind in ("tcn", "ds_tcn") and enabled and self.__dict__.get("_device_dropout", False)
-            if kind != "fsmn" and not (train_mdtc or train_tcn):
-                hint = (" -- or call model.enable_training() to train this MDTC model" if kind == "mdtc" else
-                        " -- or call model.enable_training(device_dropout=True) to train this model"
-                        if kind in ("tcn", "ds_tcn") else "")
-                raise RuntimeError("wekws_b200.KWSModel is inference-only: call model.eval() first "
-                                   "(training-mode BatchNorm/Dropout are not implemented)" + hint)
-            train_fsmn = kind == "fsmn" and fsmn_train.wants_grad(self)
-            if (train_fsmn or train_mdtc or train_tcn) and flags != 0:
-                raise RuntimeError("wekws_b200: forward_softmax has no training path; call forward() for training")
-            if train_mdtc:
-                mdtc_train.check_call(self, x, in_cache)
-            if train_tcn:
-                tcn_train.check_call(self, x, in_cache)
+        train = self.training and training.route(self, x, in_cache, flags)
         if not x.is_cuda:
             raise RuntimeError("wekws_b200.KWSModel runs on CUDA (sm_90a) only; got a CPU tensor. "
                                "There is no CPU fallback -- move the model and inputs to an H100.")
@@ -411,12 +384,8 @@ class KWSModel(nn.Module):
             raise TypeError(f"wekws_b200.KWSModel expects float32 features, got {x.dtype}")
         if x.dim() != 3 or x.size(2) != self.idim:
             raise ValueError(f"features must be (B, T, {self.idim}), got {tuple(x.shape)}")
-        if train_fsmn:
-            return fsmn_train.forward(self, x, in_cache)
-        if train_mdtc:
-            return mdtc_train.forward(self, x, in_cache)
-        if train_tcn:
-            return tcn_train.forward(self, x, in_cache)
+        if train:
+            return training.forward(self, x, in_cache)
         dev = x.device
         B, T = x.size(0), x.size(1)
         if not x.is_contiguous():
