@@ -500,13 +500,21 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           TPH(t_g2)
           group_barrier(grp, nlw);              // every row's depthwise taps and cache stores have read x
           TPH(t_bar1)
+          // the rows' residual x, read before the first x' store: the loads are volatile asm like the stores, so read
+          // column by column each load would wait for the previous column's store and every column would pay a full
+          // shared-memory round trip.  Each address is the thread's own, so the order changes no value.
+          float2 res[8][2];
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) res[j][h] = lds_f2(t_own[h] + 16u * j);
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int ch = 8 * j + 2 * q4;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const uint32_t ax = t_own[h] + 16u * j;
-              const float2 r = lds_f2(ax);
+              const float2 r = res[j][h];
               const float o0 = fmaxf(acc[4 * j + 2 * h] + cwb[6 * 64 + ch] + r.x, 0.f);
               const float o1 = fmaxf(acc[4 * j + 2 * h + 1] + cwb[6 * 64 + ch + 1] + r.y, 0.f);
               if (live[h]) sts_f2(ax, o0, o1);
