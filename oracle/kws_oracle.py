@@ -91,13 +91,28 @@ def num_frames(num_samples: int, frame_len: int = 400, frame_shift: int = 160) -
     return 1 + (num_samples - frame_len) // frame_shift
 
 
+def feature_window(window_type: str, n: int, dtype=torch.float32) -> Tensor:
+    """kaldi.py:86-113 without blackman: povey, hanning, hamming or rectangular."""
+    if window_type == "povey":
+        return povey_window(n, dtype)
+    if window_type == "hanning":
+        return torch.hann_window(n, periodic=False, dtype=dtype)
+    if window_type == "hamming":
+        return hamming_window(n, dtype)
+    if window_type == "rectangular":
+        return torch.ones(n, dtype=dtype)
+    raise ValueError("Invalid window type " + window_type)
+
+
 def fbank(waveform: Tensor, num_mel_bins: int = 80, frame_length: float = 25.0,
           frame_shift: float = 10.0, sample_frequency: float = 16000.0,
-          window_type: str = "povey", preemphasis: float = 0.97, dtype=torch.float32) -> Tensor:
+          window_type: str = "povey", preemphasis: float = 0.97, dtype=torch.float32,
+          remove_dc_offset: bool = True, low_freq: float = 20.0, high_freq: float = 0.0) -> Tensor:
     """Kaldi log-mel filterbank of one waveform (N,) in int16-scale floats, with
-    the arguments the reference passes (dither=0, energy_floor=0, rest default).
-    Returns (m, num_mel_bins).  dtype=float64 evaluates the same formulas in double
-    (the 'exact arithmetic' yardstick tests use to rank fp32 implementations)."""
+    dither=0, energy_floor=0 and the rest of kaldi.fbank's options at their defaults
+    unless given here.  Returns (m, num_mel_bins).  dtype=float64 evaluates the same
+    formulas in double (the 'exact arithmetic' yardstick tests use to rank fp32
+    implementations)."""
     wav = waveform.to(dtype).reshape(-1)
     win = int(sample_frequency * frame_length * 0.001)
     shift = int(sample_frequency * frame_shift * 0.001)
@@ -106,14 +121,15 @@ def fbank(waveform: Tensor, num_mel_bins: int = 80, frame_length: float = 25.0,
     if m == 0:
         return torch.empty(0, num_mel_bins)
     frames = wav.as_strided((m, win), (shift, 1))                         # kaldi.py:82-83
-    frames = frames - frames.mean(dim=1, keepdim=True)                    # :183-186
-    prev = F.pad(frames.unsqueeze(0), (1, 0), mode="replicate").squeeze(0)[:, :-1]
-    frames = frames - preemphasis * prev                                  # :193-198
-    w = povey_window(win, dtype) if window_type == "povey" else hamming_window(win, dtype)
-    frames = frames * w.unsqueeze(0)                                      # :201-204
+    if remove_dc_offset:
+        frames = frames - frames.mean(dim=1, keepdim=True)                # :183-186
+    if preemphasis != 0.0:
+        prev = F.pad(frames.unsqueeze(0), (1, 0), mode="replicate").squeeze(0)[:, :-1]
+        frames = frames - preemphasis * prev                              # :193-198
+    frames = frames * feature_window(window_type, win, dtype).unsqueeze(0)   # :201-204
     frames = F.pad(frames, (0, n_fft - win))                              # :207-211
     spec = torch.fft.rfft(frames).abs().pow(2.0)                          # :616-618
-    mel = mel_banks(num_mel_bins, n_fft, sample_frequency, dtype=dtype)   # :621-627
+    mel = mel_banks(num_mel_bins, n_fft, sample_frequency, low_freq, high_freq, dtype=dtype)   # :621-627
     e = torch.mm(spec, mel.T)                                             # :630
     return torch.max(e, torch.tensor(EPS, dtype=dtype)).log()             # :633
 
@@ -133,13 +149,16 @@ def dct_matrix(num_ceps: int, num_mel_bins: int, dtype=torch.float32) -> Tensor:
 
 def mfcc(waveform: Tensor, num_ceps: int = 80, num_mel_bins: int = 80, cepstral_lifter: float = 22.0,
          frame_length: float = 25.0, frame_shift: float = 10.0, sample_frequency: float = 16000.0,
-         window_type: str = "povey", dtype=torch.float32) -> Tensor:
+         window_type: str = "povey", dtype=torch.float32, preemphasis: float = 0.97,
+         remove_dc_offset: bool = True, low_freq: float = 20.0, high_freq: float = 0.0) -> Tensor:
     """Kaldi MFCC of one waveform with the arguments the reference passes (wekws/dataset/processor.py:157-166:
     kaldi.mfcc(num_ceps, num_mel_bins, frame_length, frame_shift, dither=0, energy_floor=0, sample_frequency);
-    use_energy False, htk_compat False, subtract_mean False by default): log-mel fbank -> matmul with the DCT
-    matrix -> cepstral lifter (torchaudio kaldi.py mfcc body).  Returns (m, num_ceps)."""
+    use_energy False, htk_compat False, subtract_mean False by default), plus the front-end options of ``fbank``:
+    log-mel fbank -> matmul with the DCT matrix -> cepstral lifter, none when cepstral_lifter is 0 (torchaudio
+    kaldi.py mfcc body).  Returns (m, num_ceps)."""
     assert num_ceps <= num_mel_bins
-    f = fbank(waveform, num_mel_bins, frame_length, frame_shift, sample_frequency, window_type, dtype=dtype)
+    f = fbank(waveform, num_mel_bins, frame_length, frame_shift, sample_frequency, window_type, preemphasis, dtype,
+              remove_dc_offset, low_freq, high_freq)
     if f.shape[0] == 0:
         return torch.empty(0, num_ceps)
     out = f.matmul(dct_matrix(num_ceps, num_mel_bins, dtype))

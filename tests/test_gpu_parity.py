@@ -11,12 +11,12 @@ import torch
 from oracle import kws_oracle as O
 from tests.cases import CASE_NAMES, CHUNKS, build_model
 from tests.conftest import ROOT, golden
+from tests.feature_gates import TOL_FEAT_MAX, TOL_FEAT_MEAN, check_feats, check_mfcc
 from wekws_b200 import Fbank, init_model, model_config, synth
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 TOL_POST = 1e-4
-TOL_FEAT_MAX, TOL_FEAT_MEAN = 1e-3, 1e-5
 
 
 def _tol(ref):
@@ -139,24 +139,6 @@ def test_full_size_batch_properties(name, models):
     assert (y_full[rows].cpu() - y_ref).abs().max() <= TOL_POST
 
 
-def _check_feats(out, ref, what, wav=None, **kw):
-    """Direct agreement with the reference's fp32 output within the SURVEY 8c gate, OR -- for
-    signals where the reference's own fp32 rounding exceeds that gate (pure tones: energy in a
-    few bins, the rest is rounding noise) -- at least as close to the float64 evaluation of the
-    same formulas as the reference itself is (x1.5 slack)."""
-    assert out.shape == ref.shape, what
-    if not ref.size:
-        return
-    d = np.abs(out - ref)
-    if d.max() <= TOL_FEAT_MAX and d.mean() <= TOL_FEAT_MEAN:
-        return
-    assert wav is not None, (what, d.max(), d.mean())
-    truth = O.fbank(wav, dtype=torch.float64, **kw).numpy()
-    e_ref, e_out = np.abs(ref - truth), np.abs(out - truth)
-    assert e_out.max() <= max(TOL_FEAT_MAX, 1.5 * e_ref.max()), (what, e_out.max(), e_ref.max())
-    assert e_out.mean() <= max(TOL_FEAT_MEAN, 1.5 * e_ref.mean()), (what, e_out.mean(), e_ref.mean())
-
-
 def test_fbank_matches_reference_golden():
     g = golden("fbank")
     names = [k[4:] for k in g.files if k.startswith("wav_")]
@@ -165,29 +147,14 @@ def test_fbank_matches_reference_golden():
         for name in names:
             wav = torch.from_numpy(g["wav_" + name])
             ref = g[f"fbank{nmel}_{name}"]
-            _check_feats(fb(wav.to(DEV)).cpu().numpy(), ref, (name, nmel, "f32"), wav, num_mel_bins=nmel)
-            _check_feats(fb(wav.to(torch.int16).to(DEV)).cpu().numpy(), ref, (name, nmel, "s16"), wav,
-                         num_mel_bins=nmel)
+            check_feats(fb(wav.to(DEV)).cpu().numpy(), ref, (name, nmel, "f32"), wav, num_mel_bins=nmel)
+            check_feats(fb(wav.to(torch.int16).to(DEV)).cpu().numpy(), ref, (name, nmel, "s16"), wav,
+                        num_mel_bins=nmel)
     wav = torch.from_numpy(g["wav_gauss3000_a"])
     ham = Fbank(80, window_type="hamming")(wav.to(DEV)).cpu().numpy()
-    _check_feats(ham, g["fbank80_hamming_gauss3000_a"], "hamming", wav, window_type="hamming")
+    check_feats(ham, g["fbank80_hamming_gauss3000_a"], "hamming", wav, window_type="hamming")
     z = Fbank(80)(torch.zeros(2, 1200, device=DEV))
     assert torch.all(z == float(np.log(np.float32(O.EPS))))
-
-
-def _check_mfcc(out, ref, what, wav, nc, nmel):
-    """The reference's own fp32 MFCC sits 3.5e-3 max / 3.5e-4 mean from the float64 evaluation (sgemm over 80
-    log-mels of magnitude ~16); the kernel must agree with it to that order, or be at least as close to float64."""
-    assert out.shape == ref.shape, what
-    if not ref.size:
-        return
-    d = np.abs(out - ref)
-    if d.max() <= 6e-3 and d.mean() <= 6e-4:
-        return
-    truth = O.mfcc(wav, nc, nmel, dtype=torch.float64).numpy()
-    e_ref, e_out = np.abs(ref - truth), np.abs(out - truth)
-    assert e_out.max() <= max(6e-3, 1.5 * e_ref.max()), (what, e_out.max(), e_ref.max())
-    assert e_out.mean() <= max(6e-4, 1.5 * e_ref.mean()), (what, e_out.mean(), e_ref.mean())
 
 
 def test_mfcc_matches_reference_golden():
@@ -200,13 +167,13 @@ def test_mfcc_matches_reference_golden():
         nc, nmel = int(head[4:]), int(nmel)
         fe = fes.setdefault((nc, nmel), Mfcc(nc, nmel))
         wav = torch.from_numpy(fbg["wav_" + name])
-        _check_mfcc(fe(wav.to(DEV)).cpu().numpy(), g[k], (k, "f32"), wav, nc, nmel)
-        _check_mfcc(fe(wav.to(torch.int16).to(DEV)).cpu().numpy(), g[k], (k, "s16"), wav, nc, nmel)
+        check_mfcc(fe(wav.to(DEV)).cpu().numpy(), g[k], (k, "f32"), wav, nc, nmel)
+        check_mfcc(fe(wav.to(torch.int16).to(DEV)).cpu().numpy(), g[k], (k, "s16"), wav, nc, nmel)
     # the functional form with the reference's call signature, (1, N) -> (m, num_ceps)
     wav = torch.from_numpy(fbg["wav_gauss3000_a"])
     f = mfcc(wav.unsqueeze(0).to(DEV), num_ceps=80, num_mel_bins=80, frame_length=25, frame_shift=10, dither=0.0,
              energy_floor=0.0, sample_frequency=16000)
-    _check_mfcc(f.cpu().numpy(), g["mfcc80_80_gauss3000_a"], "functional", wav, 80, 80)
+    check_mfcc(f.cpu().numpy(), g["mfcc80_80_gauss3000_a"], "functional", wav, 80, 80)
     assert Mfcc(80, 80)(torch.zeros(399, device=DEV)).shape == (0, 80)
     with pytest.raises(AssertionError):
         Mfcc(81, 80)

@@ -11,6 +11,7 @@ import torch
 
 from oracle import kws_train_oracle as T
 from tests.conftest import golden
+from tests.feature_gates import check_feats
 from tests.test_train_features_host import chain_f64
 from wekws_b200 import Fbank, Mfcc, TrainFeatures, spec_aug, _native
 from wekws_b200.frontend import draw_seed
@@ -68,10 +69,11 @@ def _batch(dtype, B=5, N=16000 + 777):
 
 
 @pytest.mark.parametrize("dtype", ["int16", "float32"])
-@pytest.mark.parametrize("kind", ["fbank40", "fbank80", "mfcc80", "mfcc40x13"])
+@pytest.mark.parametrize("kind", ["fbank40", "fbank80", "mfcc80", "mfcc40x13", "fbank23", "fbank128", "mfcc128x128"])
 def test_dithered_features_match_oracle_with_dumped_noise(dtype, kind):
     pcm, lens = _batch(dtype)
-    fe = Fbank(int(kind[5:])) if kind.startswith("fbank") else (Mfcc(80, 80) if kind == "mfcc80" else Mfcc(13, 40))
+    mfccs = {"mfcc80": (80, 80), "mfcc40x13": (13, 40), "mfcc128x128": (128, 128)}
+    fe = Fbank(int(kind[5:])) if kind.startswith("fbank") else Mfcc(*mfccs[kind])
     seed = draw_seed(torch.Generator().manual_seed(5))
     out = fe(pcm.to(DEV), lengths=torch.tensor(lens, dtype=torch.int32), dither=1.0,
              generator=torch.Generator().manual_seed(5)).cpu()
@@ -158,6 +160,22 @@ def test_train_features_match_reference_chain(name, dtype):
     e_ref, e_out = np.abs(want - truth), np.abs(got - truth)
     assert e_out.max() <= max(tmax, 1.5 * e_ref.max()), (e_out.max(), e_ref.max())
     assert e_out.mean() <= max(tmean, 1.5 * e_ref.mean()), (e_out.mean(), e_ref.mean())
+
+
+def test_train_features_default_conf_is_fbank23():
+    """TrainFeatures with an empty feat_conf takes compute_fbank's defaults: 23 mel bins, no dither; its features are
+    the Fbank(23) kernel's, bit for bit, in padding()'s order."""
+    pcm, lens = _batch("int16")
+    tf = TrainFeatures(feat_conf={})
+    assert tf.frontend.feature_dim == 23 and tf.dither == 0.0
+    batch = tf(pcm.to(DEV), lens, 16000, [0] * len(lens), [str(i) for i in range(len(lens))])
+    want = Fbank(23)(pcm.to(DEV), lengths=torch.tensor(lens, dtype=torch.int32)).cpu()
+    order = [int(k) for k in batch["keys"]]
+    T_max = int(batch["feats_lengths"][0])
+    assert torch.equal(batch["feats"].cpu(), want[order, :T_max])
+    for b, n in enumerate(lens):
+        ref = T.fbank(pcm[b, :n].float(), 23)
+        check_feats(want[b, :ref.shape[0]].numpy(), ref.numpy(), ("fbank23", b), pcm[b, :n].float(), num_mel_bins=23)
 
 
 def test_train_features_cv_split_and_resampled_input():
