@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 15  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask */
+#define WEKWS_B200_ABI_VERSION 16  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask; 16: + wekws_mdtc_head_* (MDTC training with the global / last head) */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -586,6 +586,50 @@ WEKWS_API int wekws_tcn_backward(const wekws_model* m, const float* d_feats, con
                                  int64_t B, int64_t T, float* const* h_grads, void* d_workspace, void* stream);
 WEKWS_API int wekws_dropout_mask(uint64_t seed, int64_t B, int64_t T, int64_t C, int layer, uint32_t theta,
                                  uint8_t* d_out, void* stream);
+
+/* Training the speech-command MDTC model (Executor.train with examples/speechcommand_v1/s0/conf/mdtc.yaml): the MDTC
+ * backbone's training forward and backward as in MDTC training above, with the utterance-level head of
+ * wekws/model/classifier.py in place of the per-frame linear classifier: GlobalClassifier (the mean over all T frames,
+ * padding included) or LastClassifier (frame T - 1) around Linear(hdim, 64) -> ReLU -> Dropout(p) -> Linear(64, odim),
+ * the Identity activation.  The handle only supplies the config plus wekws_model_set_head (GLOBAL or LAST): an MDTC
+ * model within the limits of MDTC training above except output_dim, here 1..4096, and the Identity activation.  The
+ * wekws_mdtc_* entry points above refuse a head model; these refuse a linear-classifier model.
+ *   h_params: wekws_mdtc_head_num_params(m) = 6 + 12 L device pointers, named_parameters order: the MDTC parameters
+ *     above with classifier.classifier.0.{weight,bias} (64, hdim), (64) and classifier.classifier.3.{weight,bias}
+ *     (odim, 64), (odim) in place of classifier.linear.{weight,bias}.  h_running / h_bn / CMVN buffers: as above.
+ *   Dropout: p in [0, 1] and a 64-bit seed.  Element (b, j) of the head's ReLU output (B, 64) is kept iff
+ *     (word >> 8) >= theta, theta = ceil(p 2^24) (in double), word = component j % 4 of Philox4x32-10(counter =
+ *     (j / 4, 0, b, 256), key = (seed lo, seed hi)): wekws_dropout_mask(seed, B, 1, 64, 255, theta) gives the mask.
+ *     Counter word 3 = 256 keeps the stream apart from the dither's (0) and the TCN blocks' (1..8).  A kept element is
+ *     multiplied by 1.0f / (float)(1 - p), a dropped one is 0 (selected: p = 1 gives exact zeros).  The backward
+ *     recomputes the mask from the same seed and p.
+ * wekws_mdtc_head_train_forward: B utterances of T frames (B * T >= 2) from empty caches: d_out (B, odim), d_out_cache
+ *   (B, hdim, padding).  save != 0: also writes d_saved, wekws_mdtc_head_train_saved_floats(m, B, T) = 12 L hdim +
+ *   B T hdim (4 L + 2) + B (hdim + 64) floats (MDTC training's, then the pooled vectors and the head's pre-ReLU
+ *   hidden vectors).  d_workspace: wekws_mdtc_head_train_workspace_bytes(m, B, T, save) = 48 * 128 hdim + (save ? 0 :
+ *   24 B T hdim) bytes.  wekws_mdtc_head_train_forward_launches(m) = 3 + 3 L launches either way.
+ * wekws_mdtc_head_backward: from d_feats, the same h_params / CMVN buffers / seed / p and d_saved of a save != 0
+ *   forward and d_grad_out (B, odim), writes every element of the 6 + 12 L gradient buffers h_grads.  The head's weight
+ *   gradients are sums over the utterances in utterance order, in double, rounded once; the backbone's as above.
+ *   d_workspace: wekws_mdtc_head_backward_workspace_bytes(m, B, T) = 32 * 128 hdim + 24 B T hdim + 8 * 128 P + 512 B
+ *   bytes, P the number of weight and bias elements of the preprocessing Linear and the convolutions.
+ *   wekws_mdtc_head_backward_launches(m) = 4 + 4 L launches.
+ * The size and launch queries return a negative status (0 for the counts) for a model they do not accept.        */
+WEKWS_API int wekws_mdtc_head_num_params(const wekws_model* m);
+WEKWS_API int64_t wekws_mdtc_head_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int64_t wekws_mdtc_head_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save);
+WEKWS_API int wekws_mdtc_head_train_forward_launches(const wekws_model* m);
+WEKWS_API int wekws_mdtc_head_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params,
+                                            int n, const float* d_cmvn_mean, const float* d_cmvn_istd,
+                                            float* const* h_running, const double* h_bn, uint64_t seed, double p,
+                                            float* d_out, float* d_out_cache, float* d_saved, int save,
+                                            void* d_workspace, int64_t B, int64_t T, void* stream);
+WEKWS_API int64_t wekws_mdtc_head_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_mdtc_head_backward_launches(const wekws_model* m);
+WEKWS_API int wekws_mdtc_head_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                       const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                       const float* d_grad_out, uint64_t seed, double p, int64_t B, int64_t T,
+                                       float* const* h_grads, void* d_workspace, void* stream);
 
 /* Resampling: torchaudio.transforms.Resample(orig_freq, new_freq) with sinc_interp_hann (the resampling of
  * wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py:50-53), for B waveforms of their own lengths.

@@ -23,7 +23,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 # limits (include/wekws_b200.h #defines)
 CTC_MAX_PREFIX, CTC_MAX_PATH_BEAM, CTC_MAX_SCORE_BEAM = 64, 20, 3
@@ -160,6 +160,19 @@ SIGNATURES = {
     "wekws_mdtc_backward_launches": (C.c_int, [C.c_void_p]),
     "wekws_mdtc_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_mdtc_head_num_params": (C.c_int, [C.c_void_p]),
+    "wekws_mdtc_head_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
+    "wekws_mdtc_head_train_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64, C.c_int]),
+    "wekws_mdtc_head_train_forward_launches": (C.c_int, [C.c_void_p]),
+    "wekws_mdtc_head_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_uint64, C.c_double, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64,
+                                                C.c_void_p]),
+    "wekws_mdtc_head_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
+    "wekws_mdtc_head_backward_launches": (C.c_int, [C.c_void_p]),
+    "wekws_mdtc_head_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_uint64, C.c_double, C.c_int64, C.c_int64,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
     "wekws_tcn_num_params": (C.c_int, [C.c_void_p]),
     "wekws_tcn_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
     "wekws_tcn_train_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64, C.c_int]),

@@ -701,7 +701,8 @@ int forward_t(const MdtcTrainDims& d, const float* feats, const float* const* P,
   FinalArgs f{};
   f.a2 = a2(L - 1); f.res = y(L - 2); f.f2 = fold(L - 1, 2, part[2]);
   f.y_out = saved ? y(L - 1) : nullptr; f.ssum = ssum; f.ssum_mode = ssum_mode(L - 1);
-  f.Wc = P[2 + 12 * L]; f.bc = P[3 + 12 * L]; f.out = out; f.O = d.odim; f.act = d.act; f.M = M;
+  if (d.odim > 0) { f.Wc = P[2 + 12 * L]; f.bc = P[3 + 12 * L]; }     // odim 0: the stack sum is the output
+  f.out = out; f.O = d.odim; f.act = d.act; f.M = M;
   mdtc_train_final_kernel<C><<<S, NT, 0, st>>>(f);
   return check_launch("mdtc_train_final_kernel");
 }
@@ -724,15 +725,16 @@ int backward_t(const MdtcTrainDims& d, const float* feats, const float* const* P
   // workspace: [gradient statistics x 2][ds][dy x 2][t1][t2][slice partials of every sliced gradient, in order, as
   // doubles]
   double* gpart[2] = {(double*)workspace, (double*)workspace + 2LL * S * C};
-  float* ds = (float*)((double*)workspace + 4LL * S * C);
-  float* dyr[2] = {ds + MC, ds + 2 * MC};
-  float* t1 = ds + 3 * MC;
-  float* t2 = ds + 4 * MC;
+  float* ds_ws = (float*)((double*)workspace + 4LL * S * C);
+  const float* ds = d.odim > 0 ? ds_ws : grad_out;            // odim 0: grad_out is the stack sum's gradient
+  float* dyr[2] = {ds_ws + MC, ds_ws + 2 * MC};
+  float* t1 = ds_ws + 3 * MC;
+  float* t2 = ds_ws + 4 * MC;
   const std::vector<long long> sizes = sliced_sizes(d);
   std::vector<double*> part(sizes.size());
-  double* w = (double*)(ds + 5 * MC);
+  double* w = (double*)(ds_ws + 5 * MC);
   for (size_t i = 0; i < sizes.size(); ++i) { part[i] = w; w += S * sizes[i]; }
-  auto dy = [&](int b) { return b == L - 1 ? ds : dyr[b % 2]; };    // the last block is a stack end: dy = ds
+  auto dy = [&](int b) -> const float* { return b == L - 1 ? ds : dyr[b % 2]; };   // the last block is a stack end
   auto bng = [&](int b, int which, const float* a, const double* gp) {
     BnGrad g{};
     g.a = a; g.stats = bstats(b, which); g.gamma = P[pidx(b, which == 0 ? 2 : which == 1 ? 6 : 10)]; g.gpart = gp;
@@ -741,10 +743,10 @@ int backward_t(const MdtcTrainDims& d, const float* feats, const float* const* P
     return g;
   };
   int rc;
-  {
+  if (d.odim > 0) {
     ClsBwdArgs c{};
     c.g = grad_out; c.ssum = ssum; c.Wc = P[2 + 12 * L]; c.bc = P[3 + 12 * L]; c.O = d.odim; c.act = d.act;
-    c.ds = ds; c.dW_part = part[2 + 6 * L]; c.db_part = part[3 + 6 * L]; c.M = M;
+    c.ds = ds_ws; c.dW_part = part[2 + 6 * L]; c.db_part = part[3 + 6 * L]; c.M = M;
     mdtc_train_cls_bwd_kernel<C><<<S, NT, 0, st>>>(c);
     if ((rc = check_launch("mdtc_train_cls_bwd_kernel"))) return rc;
   }
@@ -779,7 +781,7 @@ int backward_t(const MdtcTrainDims& d, const float* feats, const float* const* P
     a.dy = dy(b); a.y = y(b);
     a.ds = b > 0 && mdtc_stack_end(b - 1, d.stack_size) ? ds : nullptr;
     a.mask_in = b == 0;
-    a.d_in = b > 0 ? dy(b - 1) : dyr[1];
+    a.d_in = dyr[b > 0 ? (b - 1) % 2 : 1];                   // dy(b - 1): block b - 1 < L - 1 is no last block
     a.dw_part = part[q]; a.db_part = part[q + 1];
     a.M = M; a.T = T; a.K = d.K; a.dil = d.dil[b];
     mdtc_train_dw_bwd_kernel<C><<<S, NT, 0, st>>>(a);
@@ -806,7 +808,7 @@ int backward_t(const MdtcTrainDims& d, const float* feats, const float* const* P
     job(q, pidx(b, 0)); job(q + 1, pidx(b, 1)); job(q + 2, pidx(b, 4)); job(q + 3, pidx(b, 5));
     job(q + 4, pidx(b, 8)); job(q + 5, pidx(b, 9));
   }
-  job(2 + 6 * L, 2 + 12 * L); job(3 + 6 * L, 3 + 12 * L);
+  if (d.odim > 0) { job(2 + 6 * L, 2 + 12 * L); job(3 + 6 * L, 3 + 12 * L); }
   const int bx = (int)std::min<long long>((most + 255) / 256, 32);
   mdtc_train_reduce_kernel<<<dim3(bx, nj), 256, 0, st>>>(r);
   return check_launch("mdtc_train_reduce_kernel");
@@ -816,6 +818,12 @@ int backward_t(const MdtcTrainDims& d, const float* feats, const float* const* P
 
 long long mdtc_train_saved_floats(const MdtcTrainDims& d, long long M) {
   return 12LL * d.L * d.C + M * d.C * (4LL * d.L + 2);
+}
+
+float* mdtc_train_stack_sum(const MdtcTrainDims& d, long long M, float* saved, void* workspace) {
+  const long long MC = M * d.C;
+  if (saved) return saved + 12LL * d.L * d.C + MC * (1 + 4LL * d.L);
+  return (float*)((double*)workspace + 3LL * S * 2 * d.C) + 5 * MC;
 }
 
 long long mdtc_train_workspace_bytes(const MdtcTrainDims& d, long long M, bool save) {

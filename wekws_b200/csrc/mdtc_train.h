@@ -17,6 +17,9 @@ constexpr int MDTC_TRAIN_MAX_IDIM = 128;
 //     +0 conv1.conv.weight (C, 1, K), +1 .bias, +2 conv1.bn.weight, +3 .bias, +4 conv1.pointwise.weight (C, C, 1),
 //     +5 .bias, +6 bn1.weight, +7 .bias, +8 conv2.weight (C, C, 1), +9 .bias, +10 bn2.weight, +11 .bias
 //   2 + 12 L classifier.linear.weight (O, C), 3 + 12 L .bias
+// odim = 0: no classifier (mdtc_head_train.cu).  The forward's output is the stack sum, kept where
+// mdtc_train_stack_sum says, and `out` is not written; the backward's grad_out is the stack sum's gradient (B, T, C),
+// and the classifier parameters and gradients are neither read nor written.
 struct MdtcTrainDims {
   int C, idim, odim, K, L, stack_size, act, norm_var;
   int dil[MDTC_TRAIN_MAX_BLOCKS], coff[MDTC_TRAIN_MAX_BLOCKS];   // per block: dilation, offset in the cache
@@ -32,6 +35,8 @@ inline bool mdtc_stack_end(int b, int stack_size) { return b > 0 && b % stack_si
 long long mdtc_train_saved_floats(const MdtcTrainDims& d, long long M);
 long long mdtc_train_workspace_bytes(const MdtcTrainDims& d, long long M, bool save);
 long long mdtc_backward_workspace_bytes(const MdtcTrainDims& d, long long M);
+// where the forward leaves the stack sum (B, T, C): in `saved` when it is kept, else in `workspace`
+float* mdtc_train_stack_sum(const MdtcTrainDims& d, long long M, float* saved, void* workspace);
 
 // running: 2 per BatchNorm (running_mean, running_var) in block order bn0, bn1, bn2; bn: (momentum, eps) per BatchNorm.
 // saved == nullptr: nothing is kept for a backward.

@@ -23,6 +23,7 @@
 #include "tcn_tc.h"
 #include "dstcn_tc.h"
 #include "fsmn.h"
+#include "mdtc_head_train.h"
 #include "mdtc_train.h"
 #include "tcn_train.h"
 #include "linear_tc.h"
@@ -974,25 +975,34 @@ extern "C" int wekws_fsmn_backward_launches(const wekws_model* m) {
 // ------------------------------------------------------------------------------- MDTC training
 namespace {
 
-// the dimensions of an MDTC model with the per-frame linear classifier, as the training kernels take them
-int mdtc_train_dims(const wekws_model* m, const char* what, MdtcTrainDims* d) {
+// the dimensions of an MDTC model with the per-frame linear classifier (head == false) or with the global / last head
+// (head == true: odim 0, the backbone alone), as the training kernels take them
+int mdtc_dims(const wekws_model* m, const char* what, bool head, MdtcTrainDims* d) {
   WEKWS_REQUIRE(m, "%s: null handle", what);
   const wekws_model_config& c = m->cfg;
   WEKWS_REQUIRE(c.backbone == WEKWS_BACKBONE_MDTC, "%s: an MDTC model is required", what);
-  WEKWS_REQUIRE(m->head == WEKWS_HEAD_LINEAR, "%s: the MDTC model trains with the per-frame linear classifier", what);
+  if (!head) {
+    WEKWS_REQUIRE(m->head == WEKWS_HEAD_LINEAR, "%s: the MDTC model trains with the per-frame linear classifier", what);
+  } else {
+    WEKWS_REQUIRE(m->head != WEKWS_HEAD_LINEAR, "%s: a model with the global or last head is required (the per-frame "
+                  "linear classifier trains through wekws_mdtc_train_forward)", what);
+    WEKWS_REQUIRE(c.activation == WEKWS_ACT_IDENTITY, "%s: the head trains with the Identity activation", what);
+  }
   WEKWS_REQUIRE(c.hdim == 32 || c.hdim == 64, "%s: hidden_dim %d unsupported in training (32 or 64)", what, c.hdim);
   WEKWS_REQUIRE(c.kernel_size >= 2 && c.kernel_size <= MDTC_TRAIN_MAX_K, "%s: kernel_size %d unsupported (2..%d)", what,
                 c.kernel_size, MDTC_TRAIN_MAX_K);
   WEKWS_REQUIRE(c.idim >= 1 && c.idim <= MDTC_TRAIN_MAX_IDIM, "%s: input_dim %d unsupported (1..%d)", what, c.idim,
                 MDTC_TRAIN_MAX_IDIM);
-  WEKWS_REQUIRE(c.odim >= 1 && c.odim <= MDTC_TRAIN_MAX_ODIM, "%s: output_dim %d unsupported in training (1..%d)", what,
-                c.odim, MDTC_TRAIN_MAX_ODIM);
+  const int max_odim = head ? MDTC_HEAD_TRAIN_MAX_ODIM : MDTC_TRAIN_MAX_ODIM;
+  WEKWS_REQUIRE(c.odim >= 1 && c.odim <= max_odim, "%s: output_dim %d unsupported in training (1..%d)", what, c.odim,
+                max_odim);
   const int L = 1 + c.num_stack * c.stack_size;
   WEKWS_REQUIRE(c.num_stack >= 1 && c.stack_size >= 1 && L <= MDTC_TRAIN_MAX_BLOCKS,
                 "%s: %d stacks of %d blocks unsupported (at most %d blocks)", what, c.num_stack, c.stack_size,
                 MDTC_TRAIN_MAX_BLOCKS);
   memset(d, 0, sizeof(*d));
-  d->C = c.hdim; d->idim = c.idim; d->odim = c.odim; d->K = c.kernel_size; d->L = L; d->stack_size = c.stack_size;
+  d->C = c.hdim; d->idim = c.idim; d->odim = head ? 0 : c.odim; d->K = c.kernel_size; d->L = L;
+  d->stack_size = c.stack_size;
   d->act = c.activation == WEKWS_ACT_SIGMOID ? 1 : 0;
   d->norm_var = c.norm_var;
   int off = 0;
@@ -1002,6 +1012,20 @@ int mdtc_train_dims(const wekws_model* m, const char* what, MdtcTrainDims* d) {
     off += d->dil[b] * (c.kernel_size - 1);
   }
   d->pad_total = off;
+  return WEKWS_OK;
+}
+
+int mdtc_train_dims(const wekws_model* m, const char* what, MdtcTrainDims* d) { return mdtc_dims(m, what, false, d); }
+
+// the head of one call: theta = ceil(p 2^24) in double, scale = 1 / (float)(1 - p), torch's scale
+int mdtc_head(const wekws_model* m, uint64_t seed, double p, const char* what, MdtcHead* h) {
+  WEKWS_REQUIRE(p >= 0.0 && p <= 1.0, "%s: dropout probability %g is outside [0, 1]", what, p);
+  memset(h, 0, sizeof(*h));
+  h->last = m->head == WEKWS_HEAD_LAST ? 1 : 0;
+  h->odim = m->cfg.odim;
+  h->seed = seed;
+  h->theta = (uint32_t)ceil(p * 16777216.0);
+  h->scale = 1.0f / (float)(1.0 - p);
   return WEKWS_OK;
 }
 
@@ -1109,6 +1133,83 @@ extern "C" int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, c
     return rc;
   return mdtc_backward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B, (int)T,
                               h_grads, d_workspace, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------- MDTC training, global / last head
+extern "C" int wekws_mdtc_head_num_params(const wekws_model* m) {
+  MdtcTrainDims d;
+  return mdtc_dims(m, "wekws_mdtc_head_num_params", true, &d) ? 0 : mdtc_head_train_num_params(d.L);
+}
+
+extern "C" int64_t wekws_mdtc_head_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
+  MdtcTrainDims d;
+  int rc = mdtc_dims(m, "wekws_mdtc_head_train_saved_floats", true, &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_head_train_saved_floats: B, T >= 0 are required");
+  return mdtc_head_train_saved_floats(d, B, T);
+}
+
+extern "C" int64_t wekws_mdtc_head_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save) {
+  MdtcTrainDims d;
+  int rc = mdtc_dims(m, "wekws_mdtc_head_train_workspace_bytes", true, &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_head_train_workspace_bytes: B, T >= 0 are required");
+  return mdtc_head_train_workspace_bytes(d, B, T, save != 0);
+}
+
+extern "C" int64_t wekws_mdtc_head_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
+  MdtcTrainDims d;
+  int rc = mdtc_dims(m, "wekws_mdtc_head_backward_workspace_bytes", true, &d);
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_head_backward_workspace_bytes: B, T >= 0 are required");
+  return mdtc_head_backward_workspace_bytes(d, B, T);
+}
+
+extern "C" int wekws_mdtc_head_train_forward_launches(const wekws_model* m) {
+  MdtcTrainDims d;
+  return mdtc_dims(m, "wekws_mdtc_head_train_forward_launches", true, &d) ? 0 : mdtc_head_train_forward_launches(d.L);
+}
+
+extern "C" int wekws_mdtc_head_backward_launches(const wekws_model* m) {
+  MdtcTrainDims d;
+  return mdtc_dims(m, "wekws_mdtc_head_backward_launches", true, &d) ? 0 : mdtc_head_backward_launches(d.L);
+}
+
+extern "C" int wekws_mdtc_head_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params,
+                                             int n, const float* d_cmvn_mean, const float* d_cmvn_istd,
+                                             float* const* h_running, const double* h_bn, uint64_t seed, double p,
+                                             float* d_out, float* d_out_cache, float* d_saved, int save,
+                                             void* d_workspace, int64_t B, int64_t T, void* stream) {
+  MdtcTrainDims d;
+  MdtcHead h;
+  const char* what = "wekws_mdtc_head_train_forward";
+  int rc = mdtc_dims(m, what, true, &d);
+  if (rc) return rc;
+  if ((rc = mdtc_head(m, seed, p, what, &h))) return rc;
+  if ((rc = batch_stats_forward_check(what, B, T, d.C, h.odim, n, mdtc_head_train_num_params(d.L), 3 * d.L, d_feats,
+                                      h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache, d_saved,
+                                      save, d_workspace)))
+    return rc;
+  return mdtc_head_train_forward_launch(d, h, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out,
+                                        d_out_cache, save ? d_saved : nullptr, d_workspace, (int)B, (int)T,
+                                        (cudaStream_t)stream);
+}
+
+extern "C" int wekws_mdtc_head_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                        const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                        const float* d_grad_out, uint64_t seed, double p, int64_t B, int64_t T,
+                                        float* const* h_grads, void* d_workspace, void* stream) {
+  MdtcTrainDims d;
+  MdtcHead h;
+  const char* what = "wekws_mdtc_head_backward";
+  int rc = mdtc_dims(m, what, true, &d);
+  if (rc) return rc;
+  if ((rc = mdtc_head(m, seed, p, what, &h))) return rc;
+  if ((rc = batch_stats_backward_check(what, B, T, d.C, h.odim, n, mdtc_head_train_num_params(d.L), h_params, h_grads,
+                                       d_feats && d_saved && d_grad_out && d_workspace)))
+    return rc;
+  return mdtc_head_backward_launch(d, h, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B,
+                                   (int)T, h_grads, d_workspace, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------- TCN / DS-TCN training

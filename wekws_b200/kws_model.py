@@ -13,7 +13,7 @@ CMVN -> Linear+ReLU -> backbone with streaming cache -> classifier -> activation
 (kws_model.py:65-76).  There is no PyTorch / CPU fallback: CPU tensors, training mode or a missing native library
 raise.  Training runs on the device (training.py) for the FSMN model, after ``enable_training()`` for the MDTC model
 with the per-frame linear classifier, and after ``enable_training(device_dropout=True)`` for the TCN / DS-TCN models
-with the per-frame linear classifier.
+with the per-frame linear classifier and for the MDTC model with the ``global`` / ``last`` head.
 """
 from __future__ import annotations
 
@@ -352,15 +352,16 @@ class KWSModel(nn.Module):
 
     # ------------------------------------------------------------------------- training
     def enable_training(self, device_dropout: bool = False) -> "KWSModel":
-        """Lets ``train()`` mode run the training forward (training.py) of the MDTC model or, with
-        ``device_dropout=True``, of the TCN / DS-TCN model, each with the per-frame linear classifier:
-        batch statistics, running-statistics updates, gradients for ``loss.backward()``.  Without it a BatchNorm model
-        in training mode refuses to run, so a model left in ``train()`` by accident cannot silently give training-mode
-        outputs or overwrite its running statistics.  ``device_dropout=True`` accepts Dropout masks made on the device
-        from a seed drawn from torch's generator, not torch's own Bernoulli values; the TCN / DS-TCN backbones need it
-        (NotImplementedError without), and it changes nothing for the MDTC and FSMN models.  A no-op for the FSMN
-        model, whose training needs no opt-in; NotImplementedError for the ``global`` / ``last`` heads and for the
-        GRU.  Not part of the state_dict; kept by copies and pickles."""
+        """Lets ``train()`` mode run the training forward (training.py) of the MDTC model with the per-frame linear
+        classifier or, with ``device_dropout=True``, of the TCN / DS-TCN model with the per-frame linear classifier and
+        of the MDTC model with the ``global`` / ``last`` head: batch statistics, running-statistics updates, gradients
+        for ``loss.backward()``.  Without it a BatchNorm model in training mode refuses to run, so a model left in
+        ``train()`` by accident cannot silently give training-mode outputs or overwrite its running statistics.
+        ``device_dropout=True`` accepts Dropout masks made on the device from a seed drawn from torch's generator, not
+        torch's own Bernoulli values; the TCN / DS-TCN backbones and the MDTC heads need it (NotImplementedError
+        without), and it changes nothing for the MDTC model with the linear classifier and the FSMN model.  A no-op
+        for the FSMN model, whose training needs no opt-in; NotImplementedError for the heads behind TCN / DS-TCN and
+        for the GRU.  Not part of the state_dict; kept by copies and pickles."""
         training.check_trainable(self, device_dropout)
         if getattr(self.backbone, "kind", None) != "fsmn":
             self._training_enabled, self._device_dropout = True, bool(device_dropout)

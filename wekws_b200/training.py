@@ -21,14 +21,20 @@ Which models train, and how they opt in:
   the next eval call repacks.  The opt-in exists because a BatchNorm model in training mode gives other outputs than in
   eval mode and overwrites its running statistics: a model left in ``train()`` by accident keeps refusing to run.
 
-TCN / DS-TCN Dropout: no device generator reproduces torch's Bernoulli stream, so every block's ``nn.Dropout`` applies
-a mask that is a documented pure function of a 64-bit seed (include/wekws_b200.h, ``wekws_tcn_train_forward``).  The
-seed is one draw from torch's default CPU generator per training forward (``frontend.draw_seed``), so
-``torch.manual_seed`` makes a run reproducible; when every block's ``p`` is 0 nothing is drawn.  ``p`` is read from each
-block's own ``nn.Dropout`` at call time.  The backward recomputes the masks from the seed; they are never stored.
-``device_dropout=True`` is the caller's acceptance of these masks in place of torch's.
+* MDTC with the ``global`` / ``last`` head (the speech-command recipe), after
+  ``model.enable_training(device_dropout=True)``: the same backbone forward, then the head's training forward
+  (Linear, ReLU, Dropout, Linear on the mean over the frames or on the last frame), logits (B, odim); the backward
+  runs the head's kernels (csrc/mdtc_head_train.cu) and then the backbone's from the stack sum's gradient.
 
-Refused: GRU training and the ``global`` / ``last`` heads (at ``enable_training``); per call, ``forward_softmax``, a
+Dropout (TCN / DS-TCN blocks, the MDTC heads): no device generator reproduces torch's Bernoulli stream, so every
+``nn.Dropout`` applies a mask that is a documented pure function of a 64-bit seed (include/wekws_b200.h,
+``wekws_tcn_train_forward``, ``wekws_mdtc_head_train_forward``).  The seed is one draw from torch's default CPU
+generator per training forward (``frontend.draw_seed``), so ``torch.manual_seed`` makes a run reproducible; when every
+``p`` is 0 nothing is drawn.  ``p`` is read from the model's own ``nn.Dropout`` modules at call time.  The backward
+recomputes the masks from the seed; they are never stored.  ``device_dropout=True`` is the caller's acceptance of these
+masks in place of torch's.
+
+Refused: GRU training and the heads behind TCN / DS-TCN (at ``enable_training``); per call, ``forward_softmax``, a
 non-empty streaming cache, features that require grad, ``momentum=None``, non-contiguous or non-float32 parameters,
 and double backward.  The per-model names, orders, formulas and limits are in mdtc_train.py, tcn_train.py and
 fsmn_train.py.
@@ -70,8 +76,16 @@ def check_trainable(model, device_dropout: bool) -> None:
     if kind not in ("mdtc", "tcn", "ds_tcn"):
         raise NotImplementedError(f"wekws_b200: training is not implemented for the {label} backbone")
     if model.head is not None:
-        raise NotImplementedError(f"wekws_b200: {label} training runs with the per-frame linear classifier; the "
-                                  f"'{model.head}' head has Dropout, which is not implemented")
+        if kind != "mdtc":
+            raise NotImplementedError(f"wekws_b200: {label} training runs with the per-frame linear classifier; the "
+                                      f"'{model.head}' head has Dropout and trains behind the MDTC backbone only")
+        if not device_dropout:
+            raise NotImplementedError(f"wekws_b200: the '{model.head}' head has Dropout, whose masks are made on the "
+                                      "device, not torch's Bernoulli draws: opt in with "
+                                      "model.enable_training(device_dropout=True)")
+        if not isinstance(model.activation, nn.Identity):
+            raise NotImplementedError(f"wekws_b200: MDTC training with the '{model.head}' head needs the Identity "
+                                      "activation")
     if not isinstance(model.activation, (nn.Sigmoid, nn.Identity)):
         raise NotImplementedError(f"wekws_b200: {label} training needs the Sigmoid or Identity activation")
     (mdtc_train if kind == "mdtc" else tcn_train).check_limits(model)
@@ -99,10 +113,10 @@ def route(model, x: torch.Tensor, in_cache: torch.Tensor, flags: int) -> bool:
         train = wants_grad(model)
     else:
         enabled = model.__dict__.get("_training_enabled", False)
-        if not (enabled and (kind == "mdtc" or kind in ("tcn", "ds_tcn") and model.__dict__.get("_device_dropout"))):
-            hint = (" -- or call model.enable_training() to train this MDTC model" if kind == "mdtc" else
-                    " -- or call model.enable_training(device_dropout=True) to train this model"
-                    if kind in ("tcn", "ds_tcn") else "")
+        dropout = kind in ("tcn", "ds_tcn") or kind == "mdtc" and model.head is not None
+        if not (enabled and kind in ("mdtc", "tcn", "ds_tcn") and (not dropout or model.__dict__.get("_device_dropout"))):
+            hint = (" -- or call model.enable_training(device_dropout=True) to train this model" if dropout else
+                    " -- or call model.enable_training() to train this MDTC model" if kind == "mdtc" else "")
             raise RuntimeError("wekws_b200.KWSModel is inference-only: call model.eval() first "
                                "(training-mode BatchNorm/Dropout are not implemented)" + hint)
         train = True
@@ -129,8 +143,9 @@ def _params(model, dev: torch.device, names: List[str], label: str) -> List[torc
     """The parameters in native order `names`, checked for the kernels."""
     named = dict(model.named_parameters())
     if list(named) != names:
+        head = "the linear classifier" if model.head is None else f"the '{model.head}' head"
         expects = ("the parameters of wekws/model/fsmn.py FSMN, in state_dict order" if label == "FSMN" else
-                   f"the parameters of wekws/model/kws_model.py with the {label} backbone and the linear classifier, in "
+                   f"the parameters of wekws/model/kws_model.py with the {label} backbone and {head}, in "
                    "named_parameters order")
         raise RuntimeError(f"wekws_b200: {label} training expects {expects} {names}; got {list(named)}")
     params = [named[n] for n in names]
@@ -170,10 +185,14 @@ def _grad_out(g_out: torch.Tensor, dev: torch.device) -> torch.Tensor:
 
 
 class _Config:
-    """A config-only native model (the batch-statistics entry points read nothing else from it), destroyed on exit."""
+    """A config-only native model with its head (the batch-statistics entry points read nothing else from it),
+    destroyed on exit.  `net` is (config, HEAD_* id)."""
 
-    def __init__(self, cfg: _native.ModelConfig):
+    def __init__(self, net):
+        cfg, head = net
         self.h = _native.create("wekws_model_create", C.byref(cfg))
+        if head != _native.HEAD_LINEAR:
+            _native.invoke("wekws_model_set_head", self.h, head)
 
     def __enter__(self):
         return self.h
@@ -182,14 +201,17 @@ class _Config:
         _native.lib().wekws_model_destroy(self.h)
 
 
-def _run_forward(fam, cfg, x, params, cmvn, running, hyper, drop, cache_shape, save: bool):
-    """(logits, out_cache, saved activations -- empty without `save`) of the ``wekws_{fam}_train_forward`` call."""
+def _run_forward(fam, net, x, params, cmvn, running, hyper, drop, cache_shape, save: bool):
+    """(logits, out_cache, saved activations -- empty without `save`) of the ``wekws_{fam}_train_forward`` call:
+    logits (B, T, odim), or (B, odim) with a head."""
     dev = x.device
     B, T = x.shape[0], x.shape[1]
     lib = _native.lib()
-    out = torch.empty(B, T, cfg.odim, device=dev, dtype=torch.float32)
+    cfg, head = net
+    out = torch.empty((B, T, cfg.odim) if head == _native.HEAD_LINEAR else (B, cfg.odim), device=dev,
+                      dtype=torch.float32)
     out_cache = torch.empty(cache_shape, device=dev, dtype=torch.float32)
-    with _Config(cfg) as h:
+    with _Config(net) as h:
         saved = torch.empty(int(getattr(lib, f"wekws_{fam}_train_saved_floats")(h, B, T)) if save else 0, device=dev,
                             dtype=torch.float32)
         ws = torch.empty(int(getattr(lib, f"wekws_{fam}_train_workspace_bytes")(h, B, T, int(save))), device=dev,
@@ -201,15 +223,16 @@ def _run_forward(fam, cfg, x, params, cmvn, running, hyper, drop, cache_shape, s
 
 
 class _BatchStatsTrain(torch.autograd.Function):
-    """(logits, out_cache) of an MDTC (`fam` "mdtc") or TCN / DS-TCN (`fam` "tcn") training forward, whose Dropout
-    arguments `drop` are (seed, per-block p) or, for MDTC, empty; the backward returns one gradient per parameter."""
+    """(logits, out_cache) of an MDTC (`fam` "mdtc"), MDTC with a head ("mdtc_head") or TCN / DS-TCN ("tcn")
+    training forward of the native model `net` (config, head id), whose Dropout arguments `drop` are (seed, per-block
+    p), (seed, p) or, for MDTC, empty; the backward returns one gradient per parameter."""
 
     @staticmethod
-    def forward(ctx, fam, cfg, x, cmvn, running, hyper, drop, cache_shape, *params):
-        out, out_cache, saved = _run_forward(fam, cfg, x, params, cmvn, running, hyper, drop, cache_shape, True)
+    def forward(ctx, fam, net, x, cmvn, running, hyper, drop, cache_shape, *params):
+        out, out_cache, saved = _run_forward(fam, net, x, params, cmvn, running, hyper, drop, cache_shape, True)
         kept = (out,) if fam == "tcn" else ()         # only the TCN backward reads the logits
         ctx.save_for_backward(x, saved, *kept, *params)  # the version check: no in-place change before backward
-        ctx.fam, ctx.cfg, ctx.cmvn, ctx.drop, ctx.nkept = fam, cfg, cmvn, drop, len(kept)
+        ctx.fam, ctx.net, ctx.cmvn, ctx.drop, ctx.nkept = fam, net, cmvn, drop, len(kept)
         ctx.mark_non_differentiable(out_cache)
         return out, out_cache
 
@@ -222,7 +245,7 @@ class _BatchStatsTrain(torch.autograd.Function):
         B, T = x.shape[0], x.shape[1]
         g_out = _grad_out(g_out, dev)
         grads = [torch.empty_like(p) for p in params]
-        with _Config(ctx.cfg) as h:
+        with _Config(ctx.net) as h:
             ws = torch.empty(int(getattr(_native.lib(), f"wekws_{ctx.fam}_backward_workspace_bytes")(h, B, T)),
                              device=dev, dtype=torch.uint8)
             _native.call(f"wekws_{ctx.fam}_backward", h, x, _pointers(params), len(params), ctx.cmvn[0], ctx.cmvn[1],
@@ -292,23 +315,30 @@ def forward(model, x: torch.Tensor, in_cache: torch.Tensor) -> Tuple[torch.Tenso
         params = _params(model, dev, fsmn_train.param_names(bb.fsmn_layers), "FSMN")
         return _FsmnTrain.apply(model, x.contiguous(), *params)
     label = _label(bb.kind)
-    if bb.kind == "mdtc":
+    head = _native.HEAD_LINEAR
+    if bb.kind == "mdtc" and model.head is not None:
+        fam, names = "mdtc_head", mdtc_train.head_param_names(bb.num_stack, bb.stack_size)
+        head = {"global": _native.HEAD_GLOBAL, "last": _native.HEAD_LAST}[model.head]
+    elif bb.kind == "mdtc":
         fam, names = "mdtc", mdtc_train.param_names(bb.num_stack, bb.stack_size)
     else:
         fam, names = "tcn", tcn_train.param_names(bb.num_layers, bb.ds)
     params = _params(model, dev, names, label)
     cmvn, running, hyper, counters = _buffers(model, dev, _batch_norms(model), label)
-    cfg = model._native_config()
+    net = (model._native_config(), head)
     x = x.contiguous()
     drop = ()
     if fam == "tcn":
         seed, ps = tcn_train.draw_dropout(model)
         drop = (seed, (C.c_double * len(ps))(*ps))
+    elif fam == "mdtc_head":
+        seed, p = mdtc_train.draw_head_dropout(model)
+        drop = (seed, C.c_double(p))
     B = x.shape[0]
     if wants_grad(model):
-        out, out_cache = _BatchStatsTrain.apply(fam, cfg, x, cmvn, running, hyper, drop, model.cache_shape(B), *params)
+        out, out_cache = _BatchStatsTrain.apply(fam, net, x, cmvn, running, hyper, drop, model.cache_shape(B), *params)
     else:
-        out, out_cache, _ = _run_forward(fam, cfg, x, params, cmvn, running, hyper, drop, model.cache_shape(B), False)
+        out, out_cache, _ = _run_forward(fam, net, x, params, cmvn, running, hyper, drop, model.cache_shape(B), False)
     torch._foreach_add_(counters, 1)
     model.invalidate()           # the running statistics changed without a version-counter bump: repack for eval
     return out, out_cache
