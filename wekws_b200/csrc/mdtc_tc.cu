@@ -17,8 +17,10 @@
 // CHANNEL-MINOR: X[col][64 ch] (272 B per frame column: 256 B of channels and one 16-byte pad chunk that staggers the
 // banks; every stream's cache slice in the columns directly in front of its frames, so a dilated tap is a column offset).
 //
-// 19 warps: 16 compute (2 groups x 2 warpgroups), 1 weight ring warp, 2 loaders (cache slices by 2-D TMA tensor copies
-// into landing slots, transposed into X).
+// 20 warps = 5 warpgroups: 16 compute (2 groups x 2 warpgroups), then the service warpgroup: 1 weight ring warp,
+// 2 loaders (cache slices by 2-D TMA tensor copies into landing slots, transposed into X) and one warp that only keeps
+// the warpgroup whole.  The CTA launches at 96 registers per thread; after the prologue the service warpgroup gives
+// all but 40 of its registers to the compute warpgroups (setmaxnreg), which then hold 104.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -46,7 +48,11 @@ constexpr int WPG = 8;                     // warps per group (tile): two warpgr
 constexpr int NCW = NG * WPG;              // compute warps (16)
 constexpr int W_WGT = NCW;                 // warp 16: weight ring
 constexpr int W_LD = W_WGT + 1;            // warps 17..18: cache loaders, one per tile
-constexpr int NT_TC = (W_LD + NG) * 32;    // 608 threads -> up to 104 registers per thread (accumulator 32 + A 32)
+constexpr int NT_TC = (NCW + 4) * 32;      // 640 threads: five whole warpgroups, launched at 96 registers per thread
+constexpr int REG_SERVICE = 40;            // registers per thread after the handoff: service warpgroup ...
+constexpr int REG_COMPUTE = 104;           // ... and compute warpgroups (4 x 104 + 40 <= 5 x 96)
+static_assert(W_LD + NG <= NCW + 4, "the service roles must fit in the service warpgroup");
+static_assert(4 * REG_COMPUTE + REG_SERVICE <= 5 * 96, "the handoff must not take more registers than the CTA holds");
 constexpr int C = 64;
 constexpr int XCOLS = 504;                 // frame columns of X (n_streams * Lw <= XCOLS)
 constexpr int X_COL = 272;                 // bytes per frame column of X: 64 fp32 + one 16-byte pad chunk
@@ -96,17 +102,18 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, in
 }
 
 
-// The service roles are separate NON-INLINED functions: compiled on their own, their state does not add to the register
-// pressure of the compute code.  (Under the wgmma fragment layout the per-block tap / bias constants are read with
-// lane-indexed LDC from the parameter bank, four distinct addresses per warp.  Reading them instead from a
+// The service roles run in the service warpgroup's own pass loop, after its setmaxnreg.dec.  They are inlined there:
+// as __noinline__ functions the call ABI pinned registers, and at 40 registers the loader spilled 128-136 bytes.
+// Inlined, with its transpose loops kept rolled, it fits (KT = 5) or keeps 1-3 spill instructions (KT = 0).
+// (Under the wgmma fragment layout the per-block tap / bias constants are read with lane-indexed LDC from the parameter bank, four distinct addresses per warp.  Reading them instead from a
 // fragment-ordered global array with __ldg was measured 11 % slower on H100: see DESIGN.md section 3.)
 struct Bars {
   uint64_t *halo_bar, *h_free, *w_bar, *w_free, *stg_bar;
 };
 
 // WEIGHT RING (one thread): slot 0 carries Linear atom 0, W1(0), W1(1), ...; slot 1 [Linear atom 1], W2(0), ...
-__device__ __noinline__ void weights_role(const TcArgs& a, uint8_t* base, Bars B, int K, int natoms, uint32_t& wf_par,
-                                          bool first_pass) {
+__device__ __forceinline__ void weights_role(const TcArgs& a, uint8_t* base, Bars B, int K, int natoms, uint32_t& wf_par,
+                                             bool first_pass) {
   uint8_t* Wslot[2] = {base + OFF_W, base + OFF_W + W_SLOT};
   auto load_w = [&](int slot, const uint8_t* src) {
     mbar_arrive_expect_tx(&B.w_bar[slot], W_SLOT);
@@ -132,8 +139,8 @@ __device__ __noinline__ void weights_role(const TcArgs& a, uint8_t* base, Bars B
 // means a group never queues behind another tile's slices (the round-2 profile showed the groups waiting 14 % of the
 // time on halo_bar with two loaders walking the tiles in order).  The tile's ring of `nsl` landing slots is refilled
 // the moment a slot is drained, i.e. the copy for the same stream of the NEXT block is in flight a whole block ahead.
-__device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B, int i, int lane, int K, int ns, int b0,
-                                         int ntile, int nslot, uint32_t& hf_par) {
+__device__ __forceinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B, int i, int lane, int K, int ns,
+                                            int b0, int ntile, int nslot, uint32_t& hf_par) {
   if (i >= ntile) return;
   float* STG = reinterpret_cast<float*>(base + OFF_STG);
   const uint32_t xs = smem_u32(base) + OFF_X;
@@ -201,6 +208,7 @@ __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B,
       }
       TPH(t_stg)
       const int per = 16 << lgg;
+#pragma unroll 1
       for (int it = lane; it < nst * per; it += 32) {
         const int m = it >> (4 + lgg);
         move_item(STG + (slot0 + (uint32_t)(k + m) % nsl) * STG_FLOATS, (sg0 + m) * Lw + PADR - pad, it & (per - 1));
@@ -223,6 +231,7 @@ __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B,
         if (lane == 0) mbar_wait_backoff(&B.stg_bar[slot], (use / nsl) & 1);
         __syncwarp();
         const float* slotp = STG + slot * STG_FLOATS;
+#pragma unroll 1
         for (int it = lane; it < (16 << lgg); it += 32) move_item(slotp, colb, it);
         __syncwarp();                              // every lane has read the slot
         if (lane == 0 && k + nsl < njobs) {        // refill it: the same ring position, nsl jobs ahead
@@ -231,6 +240,7 @@ __device__ __noinline__ void loader_role(const TcArgs& a, uint8_t* base, Bars B,
         }
       } else {
         const f32x2 z = 0ull;
+#pragma unroll 1
         for (int e = lane; e < pad * 16; e += 32) sts_2x2(x_addr(xs, colb + (e >> 4), 4 * (e & 15)), z, z);
       }
     }
@@ -290,24 +300,30 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
   // balanced contiguous partition of the streams over the grid
   const int sb = (int)(((long long)a.B * blockIdx.x) / gridDim.x);
   const int se = (int)(((long long)a.B * (blockIdx.x + 1)) / gridDim.x);
-  int done = sb;
-
-  while (done < se) {
+  int done = sb, b0 = 0, ns = 0, ntile = 0;
+  // opens the next pass: every thread of the CTA calls it once per pass, so the __syncthreads stay in step
+  auto begin_pass = [&]() {
     const int remaining = se - done;
     const int passes_left = (remaining + a.smax - 1) / a.smax;
-    const int ns = (remaining + passes_left - 1) / passes_left;      // streams of this pass (resident in X)
-    const int b0 = done;
+    ns = (remaining + passes_left - 1) / passes_left;                 // streams of this pass (resident in X)
+    b0 = done;
     done += ns;
-    const int ntile = (ns + spt - 1) / spt;
-    auto tile_streams = [&](int i) { return min(spt, ns - i * spt); };  // streams of tile i (sequential fill)
-
+    ntile = (ns + spt - 1) / spt;
     // the landing slots are dealt out per pass (by stream count): their barriers start every pass from phase 0
     if (tid == 0) {
       for (int i = 0; i < nslot; ++i) mbar_init(&stg_bar[i], 1);
       mbar_fence_init();
     }
     __syncthreads();
-    if (warp < NCW) {
+  };
+  auto tile_streams = [&](int i) { return min(spt, ns - i * spt); };  // streams of tile i (sequential fill)
+
+  // The register handoff is warpgroup-collective: every warp of a warpgroup executes it once, before its pass loop.
+  // ptxas honours the new limits only in code that the other side never runs, so each side has its own pass loop.
+  if (warp < NCW) {
+    setmaxnreg_inc<REG_COMPUTE>();
+    while (done < se) {
+      begin_pass();
       // ================================================================== COMPUTE GROUPS (WPG warps per tile)
       // warp = grp * WPG + 4 wg + w: warpgroup wg of the tile owns rows [64 wg, 64 wg + 64) and runs their GEMMs; a thread
       // holds the wgmma fragment of rows r0 and r0 + 8 (r0 = 64 wg + 16 w + lane / 4), channel pairs 8 m + 2 (lane % 4)
@@ -353,8 +369,16 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           dW_hi[sl] = make_sdesc_sw128(sbase + OFF_W + sl * W_SLOT);
           dW_lo[sl] = make_sdesc_sw128(sbase + OFF_W + sl * W_SLOT + 8192);
         }
-        // 3-pass bf16x3 GEMM acc (+)= A * W^T over weight slot `slot` (waited for here, released when the MMAs are done)
-        auto gemm = [&](int slot, int ksteps, bool fresh) {
+        // waits for this warpgroup's MMAs and releases their weight slot
+        auto gemm_finish = [&](int slot) {
+          wgmma_wait<0>();
+          wgmma_reg_fence(acc);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&w_free[slot]);
+        };
+        // 3-pass bf16x3 GEMM acc (+)= A * W^T over weight slot `slot` (waited for here); with finish == false the MMAs
+        // are left in flight, and the caller runs gemm_finish once its own work under them is done
+        auto gemm = [&](int slot, int ksteps, bool fresh, bool finish = true) {
           mbar_wait(&w_bar[slot], (w_par >> slot) & 1);
           w_par ^= 1u << slot;
           wgmma_fence();
@@ -368,10 +392,7 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           for (int k = 0; k < 4; ++k)
             if (k < ksteps) wgmma_m64n64k16_rs(acc, ahi[k][0], ahi[k][1], ahi[k][2], ahi[k][3], dW_lo[slot] + 2 * k, 1u);
           wgmma_commit();
-          wgmma_wait<0>();
-          wgmma_reg_fence(acc);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&w_free[slot]);
+          if (finish) gemm_finish(slot);
         };
 
         // ---- features (+CMVN) -> bf16x3 A fragments, first Linear over slot 0 (K 0..63) and slot 1 (K 64..)
@@ -485,21 +506,32 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           }
           TPH(t_cache)
           // ---------------- pointwise-1 GEMM, h = relu(D + b1) -> A fragments                 (mdtc.py:115)
+          // The per-block biases are lane-indexed reads of the parameter bank (four addresses per warp).  Each wait in
+          // gemm clobbers memory, so a read written after it cannot move above it and its latency is exposed; read
+          // before the GEMM, it completes under the MMAs (measured: 2.6 % of the flagship step).
+          float2 b1[8];                         // pointwise-1 bias of channels 8 j + 2 q4, + 1
+#pragma unroll
+          for (int j = 0; j < 8; ++j) b1[j] = make_float2(cwb[5 * 64 + 8 * j + 2 * q4], cwb[5 * 64 + 8 * j + 2 * q4 + 1]);
           gemm(0, 4, true);
           TPH(t_g1)
 #pragma unroll
           for (int k = 0; k < 4; ++k)
 #pragma unroll
             for (int p = 0; p < 4; ++p) {
-              const int ch = 16 * k + 8 * (p >> 1) + 2 * q4, i = 8 * k + 2 * p;
-              split_pair_rz_relu(pack2(acc[i] + cwb[5 * 64 + ch], acc[i + 1] + cwb[5 * 64 + ch + 1]), ahi[k][p], alo[k][p]);
+              const int i = 8 * k + 2 * p;
+              const float2 b = b1[2 * k + (p >> 1)];      // channels 16 k + 8 (p >> 1) + 2 q4, + 1
+              split_pair_rz_relu(pack2(acc[i] + b.x, acc[i + 1] + b.y), ahi[k][p], alo[k][p]);
             }
           // ---------------- pointwise-2 GEMM; x' = relu(D + b2 + x) -> X; classifier partial sums at the end of a stack
           TPH(t_e1)
-          gemm(1, 4, true);                                                    // (mdtc.py:116-118, 266-273)
+          float2 b2[8];                         // pointwise-2 bias of channels 8 j + 2 q4, + 1
+#pragma unroll
+          for (int j = 0; j < 8; ++j) b2[j] = make_float2(cwb[6 * 64 + 8 * j + 2 * q4], cwb[6 * 64 + 8 * j + 2 * q4 + 1]);
+          gemm(1, 4, true, false);                                             // (mdtc.py:116-118, 266-273)
           TPH(t_g2)
-          group_barrier(grp, nlw);              // every row's depthwise taps and cache stores have read x
+          group_barrier(grp, nlw);              // every row's depthwise taps and cache stores have read x (under the MMAs)
           TPH(t_bar1)
+          gemm_finish(1);
           // the rows' residual x, read before the first x' store: the loads are volatile asm like the stores, so read
           // column by column each load would wait for the previous column's store and every column would pay a full
           // shared-memory round trip.  Each address is the thread's own, so the order changes no value.
@@ -515,8 +547,8 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
             for (int h = 0; h < 2; ++h) {
               const uint32_t ax = t_own[h] + 16u * j;
               const float2 r = res[j][h];
-              const float o0 = fmaxf(acc[4 * j + 2 * h] + cwb[6 * 64 + ch] + r.x, 0.f);
-              const float o1 = fmaxf(acc[4 * j + 2 * h + 1] + cwb[6 * 64 + ch + 1] + r.y, 0.f);
+              const float o0 = fmaxf(acc[4 * j + 2 * h] + b2[j].x + r.x, 0.f);
+              const float o1 = fmaxf(acc[4 * j + 2 * h + 1] + b2[j].y + r.y, 0.f);
               if (live[h]) sts_f2(ax, o0, o1);
               if (!HEAD && stack_end) {
                 // the classifier is linear: W_c (sum of stack outputs) = sum of W_c (stack output)
@@ -614,12 +646,19 @@ __global__ void __launch_bounds__(NT_TC, 1) mdtc_tc_kernel(const __grid_constant
           }
         if (in_tile) halo_par ^= (uint32_t)a.nblocks & 1u;   // the tile's halo_bar went through nblocks phases
       }
-    } else if (warp == W_WGT) {
-      if (lane == 0) weights_role(a, base, bars, K, natoms, wf_par, b0 == sb);
-    } else {
-      loader_role(a, base, bars, warp - W_LD, lane, K, ns, b0, ntile, nslot, hf_par);
+      __syncthreads();     // pass boundary: X, the landing slots and the rings are reused
     }
-    __syncthreads();       // pass boundary: X, the landing slots and the rings are reused
+  } else {
+    setmaxnreg_dec<REG_SERVICE>();
+    while (done < se) {
+      begin_pass();
+      if (warp == W_WGT) {
+        if (lane == 0) weights_role(a, base, bars, K, natoms, wf_par, b0 == sb);
+      } else if (warp < W_LD + NG) {
+        loader_role(a, base, bars, warp - W_LD, lane, K, ns, b0, ntile, nslot, hf_par);
+      }
+      __syncthreads();     // pass boundary
+    }
   }
 }
 

@@ -157,6 +157,12 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Hopper register reallocation between the warpgroups of a CTA (warpgroup-collective): dec gives registers back to the
+// CTA's pool, inc waits until the pool can raise this warpgroup to N registers per thread
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 // keeps the compiler from moving accesses of an accumulator across the asynchronous MMAs that own it
 template <int R>
 __device__ __forceinline__ void wgmma_reg_fence(float (&d)[R]) {
