@@ -126,7 +126,13 @@ def _config(name, ov):
 
 def build_row(row_id, factory, seed=777):
     """-> (cfg, model): `factory` (the reference's or this package's init_model) with the synthetic weights."""
-    cfg, cleanup = row_config(row_id)
+    _, name, ov, _ = _ROW[row_id]
+    return build_config(name, ov, factory, seed)
+
+
+def build_config(name, ov, factory, seed=777):
+    """build_row for a recipe config `name` with the overrides `ov` of a ROWS entry ({} for the shipped shape)."""
+    cfg, cleanup = _config(name, ov)
     try:
         with contextlib.redirect_stdout(io.StringIO()):
             torch.manual_seed(seed)
