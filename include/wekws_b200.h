@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 16  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask; 16: + wekws_mdtc_head_* (MDTC training with the global / last head) */
+#define WEKWS_B200_ABI_VERSION 17  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask; 16: + wekws_mdtc_head_* (MDTC training with the global / last head); 17: + wekws_gru_* (GRU training) */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -491,6 +491,41 @@ WEKWS_API int64_t wekws_fsmn_backward_workspace_bytes(const wekws_model* m, int6
 WEKWS_API int wekws_fsmn_backward_launches(const wekws_model* m);
 WEKWS_API int wekws_fsmn_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_grad_out,
                                   int64_t B, int64_t T, float* const* h_grads, int n, void* d_workspace, void* stream);
+
+/* Training the GRU model (Executor.train with examples/hi_xiaowen/s0/conf/gru.yaml): the training-mode forward keeps
+ * every step's gates, the backward through time gives the gradient of every parameter of wekws/model/kws_model.py
+ * with the GRU backbone (preprocessing Linear + ReLU, torch.nn.GRU, linear classifier).  The handle is a GRU model
+ * made by wekws_model_create / _set_tensor / _finalize (hidden_dim 128, 1..4 layers, input_dim 1..128, the linear
+ * classifier, Sigmoid or Identity).  Parameters and gradients travel as host arrays of wekws_gru_num_params(m) =
+ * 4 + 4 L device pointers in named_parameters order, each contiguous float32 in the parameter's own shape:
+ *   preprocessing.out.0.{weight,bias}, per layer k: backbone.{weight_ih,weight_hh,bias_ih,bias_hh}_l{k},
+ *   classifier.linear.{weight,bias}
+ *
+ * wekws_gru_load_params: the handle's packed FP32 weights from those tensors, on the device (1 launch): the
+ *   optimiser's updates reach the kernels without a host round trip.  The CMVN buffers keep what _finalize packed;
+ *   the tensor-core weight image is not updated (the training forward does not read it).
+ * wekws_gru_train_forward: the FP32 kernel of wekws_model_forward (whatever the precision mode) over B utterances of T
+ *   frames from empty caches, one launch, the same d_out / d_out_cache bits, also writing d_saved:
+ *   wekws_gru_train_saved_floats(m, B, T) = (1 + 5 L) B T hidden_dim floats, (B T, hidden_dim) row-major blocks with
+ *   row b T + t: x0 = ReLU(Linear(CMVN(feats))), then per layer h_t, r, z, n and W_hn h_{t-1} + b_hn.
+ * wekws_gru_backward: from d_feats, d_saved and d_out (the logits) of that forward and d_grad_out = d loss / d out
+ *   (B, T, odim), writes every element of every gradient buffer, all B T frames as rows (padding included, as torch
+ *   does).  Per layer one sequential kernel runs the recurrence backwards in time; the weight gradients are summed in
+ *   32 fixed row slices, then the slices in order: no atomics, equal inputs give equal bits.  d_workspace:
+ *   wekws_gru_backward_workspace_bytes(m, B, T) = 4 * (32 P + B T (8 hidden_dim + odim)) bytes, P the number of
+ *   parameter elements.  wekws_gru_backward_launches(m) = 5 + 4 L launches.
+ * The size and launch queries read the config only; they return a negative status (0 for the counts) for another
+ * backbone.                                                                                                       */
+WEKWS_API int wekws_gru_num_params(const wekws_model* m);
+WEKWS_API int wekws_gru_load_params(wekws_model* m, const float* const* h_params, int n, void* stream);
+WEKWS_API int64_t wekws_gru_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_gru_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
+                                      float* d_saved, int64_t B, int64_t T, void* stream);
+WEKWS_API int64_t wekws_gru_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_gru_backward_launches(const wekws_model* m);
+WEKWS_API int wekws_gru_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_out,
+                                 const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads, int n,
+                                 void* d_workspace, void* stream);
 
 /* Training the MDTC model (wekws/utils/executor.py Executor.train with an mdtc.yaml / mdtc_small.yaml model): the
  * training-mode forward, every BatchNorm normalising with the biased variance of the batch (all B * T frames, padding

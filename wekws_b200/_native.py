@@ -23,7 +23,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 # limits (include/wekws_b200.h #defines)
 CTC_MAX_PREFIX, CTC_MAX_PATH_BEAM, CTC_MAX_SCORE_BEAM = 64, 20, 3
@@ -149,6 +149,15 @@ SIGNATURES = {
     "wekws_fsmn_backward_launches": (C.c_int, [C.c_void_p]),
     "wekws_fsmn_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
                                       C.c_int, C.c_void_p, C.c_void_p]),
+    "wekws_gru_num_params": (C.c_int, [C.c_void_p]),
+    "wekws_gru_load_params": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "wekws_gru_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
+    "wekws_gru_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.c_int64, C.c_void_p]),
+    "wekws_gru_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
+    "wekws_gru_backward_launches": (C.c_int, [C.c_void_p]),
+    "wekws_gru_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wekws_mdtc_num_params": (C.c_int, [C.c_void_p]),
     "wekws_mdtc_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
     "wekws_mdtc_train_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64, C.c_int]),

@@ -12,6 +12,9 @@
 // so every step streams them from L2 through a double-buffered shared-memory ring of 48 KB chunks
 // (16 k-rows of [W_ih | W_hh], one cp.async.bulk each, mbarrier-signalled): the TMA engine keeps
 // ~96 KB in flight per SM, which is what hides the L2 latency -- register-staged loads could not.
+//
+// The training forward (SAVE) is the same kernel that also stores what the backward (gru_train.cu) reads: the layer-0
+// input and, per layer and step, h_t, r, z, n and W_hn h_{t-1} + b_hn (GruArgs::saved).
 #include "common.cuh"
 #include "gru.h"
 #include "tc_common.cuh"
@@ -27,7 +30,7 @@ constexpr int KCH = 16;                          // k-rows per weight chunk
 constexpr int CHUNK_FLOATS = KCH * 2 * GG;       // 12288 floats = 48 KB
 constexpr int NCHUNK = GH / KCH;                 // 8 chunks per layer
 
-template <int S>
+template <int S, bool SAVE>
 __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
   extern __shared__ __align__(128) float sm[];
   float* ring = sm;                               // [2][CHUNK_FLOATS]
@@ -40,6 +43,7 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
   const int tid = threadIdx.x;
   const int idim = a.idim, idimP = (idim + 3) & ~3;
   const float* vec = a.vec;
+  const long long M = (long long)a.B * a.T;        // rows of a saved block
   if (tid == 0) {
     mbar_init(&full[0], 1); mbar_init(&full[1], 1);
     mbar_fence_init();
@@ -102,6 +106,9 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
         const int s = i / GH, j = i - s * GH;
         const float v = gi[s * GH + j] + gi[(S + s) * GH + j] + gi[(2 * S + s) * GH + j] + __ldg(vec + a.v_bp + j);
         xin[i] = fmaxf(v, 0.f);
+        if constexpr (SAVE) {
+          if (s < Sv) a.saved[((long long)(b0 + s) * a.T + t) * GH + j] = xin[i];
+        }
       }
       __syncthreads();
       for (int l = 0; l < a.L; ++l) {
@@ -154,6 +161,16 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
           const float hn = (1.f - z) * n + z * hp;
           hst[(l * S + s) * GH + j] = hn;
           xin[s * GH + j] = hn;
+          if constexpr (SAVE) {
+            if (s < Sv) {
+              float* dst = a.saved + M * GH * (1 + 5 * l) + ((long long)(b0 + s) * a.T + t) * GH + j;
+              dst[0] = hn;
+              dst[M * GH] = r;
+              dst[2 * M * GH] = z;
+              dst[3 * M * GH] = n;
+              dst[4 * M * GH] = gh[s * GG + 2 * GH + j];
+            }
+          }
         }
         __syncthreads();
       }
@@ -185,32 +202,33 @@ __global__ void __launch_bounds__(GG, 1) gru_kernel(const GruArgs a) {
   }
 }
 
-template <int S>
+template <int S, bool SAVE>
 int launch_s(const GruArgs& a, cudaStream_t st) {
   GruArgs b = a;
   b.n_tiles = (a.B + S - 1) / S;
   const int idimP = (a.idim + 3) & ~3;
   const size_t smem = (size_t)(2 * CHUNK_FLOATS + S * GH + a.L * S * GH + 2 * S * GG + S * idimP) * sizeof(float);
   const int sms = device_sm_count();
-  WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_kernel<S, SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = b.n_tiles < sms ? b.n_tiles : sms;
-  gru_kernel<S><<<grid, GG, smem, st>>>(b);
-  return check_launch("gru_kernel");
+  gru_kernel<S, SAVE><<<grid, GG, smem, st>>>(b);
+  return check_launch(SAVE ? "gru_kernel<save>" : "gru_kernel");
 }
 
 }  // namespace
 
-int gru_launch(const GruArgs& a, cudaStream_t st) {
+int gru_launch(const GruArgs& a, cudaStream_t st, bool save) {
   WEKWS_REQUIRE(a.H == 128, "GRU hidden_dim %d unsupported (128 only)", a.H);
   WEKWS_REQUIRE(a.L >= 1 && a.L <= 4, "GRU num_layers %d unsupported (1..4)", a.L);
   const int sms = device_sm_count();
   // streams per CTA: keep the grid within one wave
   const int S = a.B <= sms ? 1 : a.B <= 2 * sms ? 2 : a.B <= 4 * sms ? 4 : 8;
+  WEKWS_REQUIRE(!save || (a.saved != nullptr && a.in_cache == nullptr), "gru_launch: bad training-forward arguments");
   switch (S) {
-    case 1: return launch_s<1>(a, st);
-    case 2: return launch_s<2>(a, st);
-    case 4: return launch_s<4>(a, st);
-    default: return launch_s<8>(a, st);
+    case 1: return save ? launch_s<1, true>(a, st) : launch_s<1, false>(a, st);
+    case 2: return save ? launch_s<2, true>(a, st) : launch_s<2, false>(a, st);
+    case 4: return save ? launch_s<4, true>(a, st) : launch_s<4, false>(a, st);
+    default: return save ? launch_s<8, true>(a, st) : launch_s<8, false>(a, st);
   }
 }
 

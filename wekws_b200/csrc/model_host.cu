@@ -972,6 +972,104 @@ extern "C" int wekws_fsmn_backward_launches(const wekws_model* m) {
   return m && m->cfg.backbone == WEKWS_BACKBONE_FSMN ? fsmn_backward_launches(m->cfg.num_layers) : 0;
 }
 
+// ------------------------------------------------------------------------------- GRU training
+namespace {
+
+bool is_gru(const wekws_model* m) { return m && m->cfg.backbone == WEKWS_BACKBONE_GRU; }
+
+// the dimensions of a GRU model's config (the fields the saved-activation and workspace sizes depend on)
+GruArgs gru_dims(const wekws_model_config& c) {
+  GruArgs a{};
+  a.L = c.num_layers; a.H = c.hdim; a.idim = c.idim; a.odim = c.odim;
+  return a;
+}
+
+int gru_train_check(const wekws_model* m, const char* what) {
+  WEKWS_REQUIRE(m, "%s: null handle", what);
+  WEKWS_REQUIRE(is_gru(m), "%s: a GRU model is required", what);
+  if (!m->finalized) { set_error("%s called before wekws_model_finalize", what); return WEKWS_ERR_STATE; }
+  int dev = 0;
+  WEKWS_CUDA_OK(cudaGetDevice(&dev));
+  WEKWS_REQUIRE(dev == m->device, "model was finalized on device %d but current device is %d", m->device, dev);
+  return WEKWS_OK;
+}
+
+}  // namespace
+
+extern "C" int wekws_gru_num_params(const wekws_model* m) {
+  return is_gru(m) ? gru_num_params(m->cfg.num_layers) : 0;
+}
+
+extern "C" int wekws_gru_load_params(wekws_model* m, const float* const* h_params, int n, void* stream) {
+  int rc = gru_train_check(m, "wekws_gru_load_params");
+  if (rc) return rc;
+  const GruArgs& a = m->gru;
+  const int H = a.H, G = 3 * H;
+  WEKWS_REQUIRE(h_params && n == gru_num_params(a.L), "wekws_gru_load_params: expected the %d parameters of a "
+                "%d-layer GRU model, got %d", gru_num_params(a.L), a.L, n);
+  FsmnPackArgs p{};
+  p.packed = m->d_vec;
+  p.n = n;
+  int k = 0;                                   // each parameter [rows][cols] into its place in pack_gru's layout
+  auto put = [&](int rows, int cols, long long dst, int ld) {
+    FsmnParamCopy& c = p.p[k];
+    c.src = h_params[k]; c.dst = dst; c.rows = rows; c.cols = cols; c.ld = ld;
+    ++k;
+  };
+  put(H, a.idim, a.v_wp, H); put(H, 1, a.v_bp, 1);
+  for (int l = 0; l < a.L; ++l) {
+    const long long base = a.v_layers + (long long)l * a.v_layer_stride;
+    put(G, H, base, 2 * G); put(G, H, base + G, 2 * G);
+    put(G, 1, base + 2LL * H * G, 1); put(G, 1, base + 2LL * H * G + G, 1);
+  }
+  put(a.odim, H, a.v_wc, a.odim); put(a.odim, 1, a.v_bc, 1);
+  for (int i = 0; i < p.n; ++i)
+    WEKWS_REQUIRE(p.p[i].src != nullptr, "wekws_gru_load_params: parameter %d is null", i);
+  return fsmn_pack_launch(p, (cudaStream_t)stream);
+}
+
+extern "C" int64_t wekws_gru_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
+  WEKWS_REQUIRE(is_gru(m) && B >= 0 && T >= 0, "wekws_gru_train_saved_floats: a GRU model and B, T >= 0 are required");
+  return B * T * gru_saved_per_frame(m->cfg.num_layers, m->cfg.hdim);
+}
+
+extern "C" int64_t wekws_gru_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
+  WEKWS_REQUIRE(is_gru(m) && B >= 0 && T >= 0,
+                "wekws_gru_backward_workspace_bytes: a GRU model and B, T >= 0 are required");
+  return (int64_t)sizeof(float) * gru_backward_workspace_floats(gru_dims(m->cfg), B * T);
+}
+
+extern "C" int wekws_gru_backward_launches(const wekws_model* m) {
+  return is_gru(m) ? gru_backward_launches(m->cfg.num_layers) : 0;
+}
+
+extern "C" int wekws_gru_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
+                                       float* d_saved, int64_t B, int64_t T, void* stream) {
+  int rc = gru_train_check(m, "wekws_gru_train_forward");
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_gru_train_forward: bad B/T");
+  WEKWS_REQUIRE(d_feats && d_out && d_out_cache && d_saved, "wekws_gru_train_forward: null tensor");
+  GruArgs a = m->gru;                          // the FP32 kernel whatever the precision mode
+  a.feats = d_feats; a.in_cache = nullptr; a.out = d_out; a.out_cache = d_out_cache;
+  a.B = (int)B; a.T = (int)T; a.saved = d_saved;
+  return gru_launch(a, (cudaStream_t)stream, true);
+}
+
+extern "C" int wekws_gru_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_out,
+                                  const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads, int n,
+                                  void* d_workspace, void* stream) {
+  int rc = gru_train_check(m, "wekws_gru_backward");
+  if (rc) return rc;
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_gru_backward: bad B/T");
+  WEKWS_REQUIRE(d_feats && d_saved && d_out && d_grad_out && d_workspace && h_grads,
+                "wekws_gru_backward: null argument");
+  const int np = gru_num_params(m->gru.L);
+  WEKWS_REQUIRE(n == np, "wekws_gru_backward: expected %d gradient buffers, got %d", np, n);
+  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_grads[i] != nullptr, "wekws_gru_backward: gradient buffer %d is null", i);
+  return gru_backward_launch(m->gru, d_feats, d_saved, d_out, d_grad_out, (int)B, (int)T, h_grads,
+                             (float*)d_workspace, (cudaStream_t)stream);
+}
+
 // ------------------------------------------------------------------------------- MDTC training
 namespace {
 

@@ -13,7 +13,8 @@ CMVN -> Linear+ReLU -> backbone with streaming cache -> classifier -> activation
 (kws_model.py:65-76).  There is no PyTorch / CPU fallback: CPU tensors, training mode or a missing native library
 raise.  Training runs on the device (training.py) for the FSMN model, after ``enable_training()`` for the MDTC model
 with the per-frame linear classifier, and after ``enable_training(device_dropout=True)`` for the TCN / DS-TCN models
-with the per-frame linear classifier and for the MDTC model with the ``global`` / ``last`` head.
+with the per-frame linear classifier and for the MDTC model with the ``global`` / ``last`` head, and after
+``enable_training(bptt=True)`` for the GRU model.
 """
 from __future__ import annotations
 
@@ -178,6 +179,7 @@ class KWSModel(nn.Module):
         self._precision_applied = None
         self._training_enabled = False   # enable_training(): BatchNorm models run training mode only after opting in
         self._device_dropout = False     # enable_training(device_dropout=True): Dropout masks made on the device
+        self._bptt = False               # enable_training(bptt=True): GRU training, its gates kept for the backward
 
     # ---------------------------------------------------------------- weight life-cycle
     def invalidate(self) -> None:
@@ -351,7 +353,7 @@ class KWSModel(nn.Module):
         return cache, out, out_cache
 
     # ------------------------------------------------------------------------- training
-    def enable_training(self, device_dropout: bool = False) -> "KWSModel":
+    def enable_training(self, device_dropout: bool = False, bptt: bool = False) -> "KWSModel":
         """Lets ``train()`` mode run the training forward (training.py) of the MDTC model with the per-frame linear
         classifier or, with ``device_dropout=True``, of the TCN / DS-TCN model with the per-frame linear classifier and
         of the MDTC model with the ``global`` / ``last`` head: batch statistics, running-statistics updates, gradients
@@ -359,12 +361,16 @@ class KWSModel(nn.Module):
         ``train()`` by accident cannot silently give training-mode outputs or overwrite its running statistics.
         ``device_dropout=True`` accepts Dropout masks made on the device from a seed drawn from torch's generator, not
         torch's own Bernoulli values; the TCN / DS-TCN backbones and the MDTC heads need it (NotImplementedError
-        without), and it changes nothing for the MDTC model with the linear classifier and the FSMN model.  A no-op
-        for the FSMN model, whose training needs no opt-in; NotImplementedError for the heads behind TCN / DS-TCN and
-        for the GRU.  Not part of the state_dict; kept by copies and pickles."""
-        training.check_trainable(self, device_dropout)
+        without), and it changes nothing for the MDTC model with the linear classifier and the FSMN model.
+        ``bptt=True`` lets the GRU model train: with grad, its forward keeps every step's gates ((1 + 5 num_layers)
+        * B * T * 128 floats) and ``loss.backward()`` runs the backward through time; without grad a training-mode
+        call takes the eval path.  The GRU model needs it (NotImplementedError without), and it changes nothing for
+        the other backbones.  A no-op for the FSMN model, whose training needs no opt-in; NotImplementedError for the
+        heads behind TCN / DS-TCN and for a GRU with inter-layer Dropout or outside the kernels' limits
+        (gru_train.py).  Not part of the state_dict; kept by copies and pickles."""
+        training.check_trainable(self, device_dropout, bptt)
         if getattr(self.backbone, "kind", None) != "fsmn":
-            self._training_enabled, self._device_dropout = True, bool(device_dropout)
+            self._training_enabled, self._device_dropout, self._bptt = True, bool(device_dropout), bool(bptt)
         return self
 
     # ------------------------------------------------------------------------- forward

@@ -10,6 +10,13 @@ Which models train, and how they opt in:
   csrc/fsmn_grad.cu.  Each forward first packs the parameters' current values into the model's native handle on the
   device (one launch), so ``optimizer.step()`` needs no host round trip; when the handle was rebuilt between the
   forward and the backward, the backward packs the same values again.
+* GRU, after ``model.enable_training(bptt=True)``: as FSMN, with grad mode on and a parameter requiring grad the
+  logits are attached to the autograd graph and ``loss.backward()`` fills ``.grad`` of every parameter (the
+  preprocessing Linear, every layer of ``nn.GRU``, the classifier); without grad the call takes the eval path (the GRU
+  model has no BatchNorm and no Dropout).  The forward is the FP32 kernel of csrc/gru.cu in its storing instantiation,
+  whatever ``model.precision`` is (its logits and cache are the FP32 eval kernel's, bit for bit); the backward through
+  time is csrc/gru_train.cu.  Parameters are packed into the handle on the device as for FSMN.  The opt-in is the
+  caller's acceptance of the memory the forward keeps: (1 + 5 L) B T 128 floats.
 * MDTC, after ``model.enable_training()``, and TCN / DS-TCN, after ``model.enable_training(device_dropout=True)``, each
   with the per-frame linear classifier: the training-mode forward of the reference's wekws/model/kws_model.py, with or
   without grad.  Every BatchNorm normalises with the biased variance of the batch (all B * T frames, padding included),
@@ -34,10 +41,10 @@ generator per training forward (``frontend.draw_seed``), so ``torch.manual_seed`
 recomputes the masks from the seed; they are never stored.  ``device_dropout=True`` is the caller's acceptance of these
 masks in place of torch's.
 
-Refused: GRU training and the heads behind TCN / DS-TCN (at ``enable_training``); per call, ``forward_softmax``, a
-non-empty streaming cache, features that require grad, ``momentum=None``, non-contiguous or non-float32 parameters,
-and double backward.  The per-model names, orders, formulas and limits are in mdtc_train.py, tcn_train.py and
-fsmn_train.py.
+Refused: GRU training without ``bptt=True``, a GRU with inter-layer Dropout or outside the kernels' limits, and the
+heads behind TCN / DS-TCN (at ``enable_training``); per call, ``forward_softmax``, a non-empty streaming cache,
+features that require grad, ``momentum=None``, non-contiguous or non-float32 parameters, and double backward.  The
+per-model names, orders, formulas and limits are in mdtc_train.py, tcn_train.py, fsmn_train.py and gru_train.py.
 """
 from __future__ import annotations
 
@@ -48,7 +55,7 @@ import torch
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
-from . import _native, fsmn_train, mdtc_train, tcn_train
+from . import _native, fsmn_train, gru_train, mdtc_train, tcn_train
 
 
 def _kind(model) -> Optional[str]:
@@ -64,12 +71,19 @@ def _batch_norms(model) -> List[nn.BatchNorm1d]:
     return (mdtc_train if model.backbone.kind == "mdtc" else tcn_train).batch_norms(model)
 
 
-def check_trainable(model, device_dropout: bool) -> None:
-    """Raises NotImplementedError unless ``model.enable_training(device_dropout)`` can train `model`."""
+def check_trainable(model, device_dropout: bool, bptt: bool = False) -> None:
+    """Raises NotImplementedError unless ``model.enable_training(device_dropout, bptt)`` can train `model`."""
     kind = _kind(model)
     if kind == "fsmn":
         return
     label = _label(kind)
+    if kind == "gru":
+        if not bptt:
+            raise NotImplementedError("wekws_b200: training the GRU backbone keeps every step's gates for the backward "
+                                      "through time, (1 + 5 num_layers) * B * T * 128 floats: opt in with "
+                                      "model.enable_training(bptt=True)")
+        gru_train.check_limits(model)
+        return
     if kind in ("tcn", "ds_tcn") and not device_dropout:
         raise NotImplementedError(f"wekws_b200: training the {label} backbone applies Dropout masks made on the device, "
                                   "not torch's Bernoulli draws: opt in with model.enable_training(device_dropout=True)")
@@ -109,7 +123,11 @@ def route(model, x: torch.Tensor, in_cache: torch.Tensor, flags: int) -> bool:
     """Whether a call of `model` in training mode runs ``forward`` (True) or the eval path (False, FSMN without grad).
     Raises the refusals that need no device."""
     kind = _kind(model)
-    if kind == "fsmn":
+    if kind == "gru" and not (model.__dict__.get("_training_enabled", False) and model.__dict__.get("_bptt", False)):
+        raise RuntimeError("wekws_b200.KWSModel is inference-only: call model.eval() first "
+                           "(training-mode BatchNorm/Dropout are not implemented) -- or call "
+                           "model.enable_training(bptt=True) to train this GRU model")
+    if kind in ("fsmn", "gru"):
         train = wants_grad(model)
     else:
         enabled = model.__dict__.get("_training_enabled", False)
@@ -122,7 +140,7 @@ def route(model, x: torch.Tensor, in_cache: torch.Tensor, flags: int) -> bool:
         train = True
     if train and flags != 0:
         raise RuntimeError("wekws_b200: forward_softmax has no training path; call forward() for training")
-    if kind != "fsmn":
+    if kind not in ("fsmn", "gru"):
         label = _label(kind)
         _check_inputs(x, in_cache, label, "is not supported in training mode -- pass no in_cache, or call model.eval()")
         if x.dim() == 3 and x.shape[0] * x.shape[1] <= 1:
@@ -253,55 +271,59 @@ class _BatchStatsTrain(torch.autograd.Function):
         return (None,) * 8 + tuple(grads)
 
 
-def _load(model, dev: torch.device, params) -> C.c_void_p:
+def _load(fam: str, model, dev: torch.device, params) -> C.c_void_p:
     """The model's native handle on `dev` with `params` packed into it (one launch)."""
     h = model._training_handle(dev)
-    _native.call("wekws_fsmn_load_params", h, _pointers(params), len(params), device=dev)
+    _native.call(f"wekws_{fam}_load_params", h, _pointers(params), len(params), device=dev)
     return h
 
 
-class _FsmnTrain(torch.autograd.Function):
-    """(logits, out_cache) of the FSMN training forward; the backward returns one gradient per parameter."""
+class _PackedTrain(torch.autograd.Function):
+    """(logits, out_cache) of the FSMN (`fam` "fsmn") or GRU ("gru") training forward, which runs on the model's
+    native handle with the parameters packed into it; the backward returns one gradient per parameter."""
 
     @staticmethod
-    def forward(ctx, model, x, *params):
+    def forward(ctx, fam, model, x, *params):
         dev = x.device
         B, T = x.shape[0], x.shape[1]
         out = torch.empty(B, T, model.odim, device=dev, dtype=torch.float32)
         if B > 0 and T > 0:
-            h = _load(model, dev, params)
+            h = _load(fam, model, dev, params)
             out_cache = torch.empty(model.cache_shape(B), device=dev, dtype=torch.float32)
-            saved = torch.empty(int(_native.lib().wekws_fsmn_train_saved_floats(h, B, T)), device=dev,
+            saved = torch.empty(int(getattr(_native.lib(), f"wekws_{fam}_train_saved_floats")(h, B, T)), device=dev,
                                 dtype=torch.float32)
-            _native.call("wekws_fsmn_train_forward", h, x, out, out_cache, saved, B, T, device=dev)
+            _native.call(f"wekws_{fam}_train_forward", h, x, out, out_cache, saved, B, T, device=dev)
         else:
             h, saved = None, torch.empty(0, device=dev)
             out_cache = torch.zeros(model.cache_shape(B), device=dev, dtype=torch.float32)
-        ctx.save_for_backward(x, saved, *params)      # the version check: no in-place change before backward
-        ctx.model, ctx.handle = model, h
+        kept = (out,) if fam == "gru" else ()         # the Sigmoid backward reads the logits
+        ctx.save_for_backward(x, saved, *kept, *params)  # the version check: no in-place change before backward
+        ctx.fam, ctx.model, ctx.handle, ctx.nkept = fam, model, h, len(kept)
         ctx.mark_non_differentiable(out_cache)
         return out, out_cache
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g_out, _g_cache):
-        x, saved, *params = ctx.saved_tensors
+        x, saved, *rest = ctx.saved_tensors
+        kept, params = rest[:ctx.nkept], rest[ctx.nkept:]
         grads = [torch.empty_like(p) for p in params]
         B, T = x.shape[0], x.shape[1]
         if B == 0 or T == 0:
             for g in grads:
                 g.zero_()
-            return (None, None) + tuple(grads)
+            return (None, None, None) + tuple(grads)
         dev = x.device
-        model = ctx.model
+        model, fam = ctx.model, ctx.fam
         h = model.__dict__.get("_handle")
         if h is not ctx.handle or model._handle_dev != dev:
-            h = _load(model, dev, params)             # the handle was rebuilt since the forward: same values again
+            h = _load(fam, model, dev, params)        # the handle was rebuilt since the forward: same values again
         g_out = _grad_out(g_out, dev)
-        ws = torch.empty(int(_native.lib().wekws_fsmn_backward_workspace_bytes(h, B, T)), device=dev,
+        ws = torch.empty(int(getattr(_native.lib(), f"wekws_{fam}_backward_workspace_bytes")(h, B, T)), device=dev,
                          dtype=torch.uint8)
-        _native.call("wekws_fsmn_backward", h, x, saved, g_out, B, T, _pointers(grads), len(grads), ws, device=dev)
-        return (None, None) + tuple(grads)
+        _native.call(f"wekws_{fam}_backward", h, x, saved, *kept, g_out, B, T, _pointers(grads), len(grads), ws,
+                     device=dev)
+        return (None, None, None) + tuple(grads)
 
 
 def forward(model, x: torch.Tensor, in_cache: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -309,11 +331,14 @@ def forward(model, x: torch.Tensor, in_cache: torch.Tensor) -> Tuple[torch.Tenso
     CUDA)."""
     dev = x.device
     bb = model.backbone
-    if bb.kind == "fsmn":
-        _check_inputs(x, in_cache, "FSMN", "with grad is not supported -- pass no in_cache, or call under "
+    kind = _kind(model)
+    if kind in ("fsmn", "gru"):
+        label = _label(kind)
+        _check_inputs(x, in_cache, label, "with grad is not supported -- pass no in_cache, or call under "
                       "torch.no_grad()")
-        params = _params(model, dev, fsmn_train.param_names(bb.fsmn_layers), "FSMN")
-        return _FsmnTrain.apply(model, x.contiguous(), *params)
+        names = fsmn_train.param_names(bb.fsmn_layers) if kind == "fsmn" else gru_train.param_names(bb.num_layers)
+        params = _params(model, dev, names, label)
+        return _PackedTrain.apply(kind, model, x.contiguous(), *params)
     label = _label(bb.kind)
     head = _native.HEAD_LINEAR
     if bb.kind == "mdtc" and model.head is not None:
