@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 17  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask; 16: + wekws_mdtc_head_* (MDTC training with the global / last head); 17: + wekws_gru_* (GRU training) */
+#define WEKWS_B200_ABI_VERSION 18  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask; 16: + wekws_mdtc_head_* (MDTC training with the global / last head); 17: + wekws_gru_* (GRU training); 18: + wekws_grad_clip*, wekws_adam_step* (the optimiser step) */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -696,6 +696,45 @@ WEKWS_API int64_t wekws_cmvn_stats_workspace_bytes(int64_t B, int D);
 WEKWS_API int wekws_cmvn_stats_accumulate(const float* d_feats, int64_t B, int64_t max_frames, int D,
                                           const int32_t* d_frames, double* d_acc, int64_t* d_frame_num,
                                           void* d_workspace, void* stream);
+
+/* The training step's optimiser (wekws/utils/executor.py Executor.train: clip_grad_norm_, then optimizer.step() of
+ * torch.optim.Adam).  Tensors travel as host arrays of n device pointers to contiguous float32 data and h_numel[i] >= 1
+ * elements each, as in the training entry points.  Each launch takes a table of up to 1024 (clip) or 512 (Adam)
+ * tensors in its kernel parameters: nothing is uploaded, nothing allocated, nothing synchronised.
+ *
+ * wekws_grad_clip: torch.nn.utils.clip_grad_norm_(norm_type=2) on the n gradients, in place.  Launch 1: CTA c of
+ *   G = min(264, max(1, ceil(E / 2048))) per table (E the total number of elements) writes the double sum of the
+ *   squares of elements [c E_k / G, (c + 1) E_k / G) of its table's concatenated gradients (E_k elements).  Launch 2:
+ *   every CTA adds all partials in one fixed order, total_norm = (float)sqrt(sum), and
+ *     coef = min((1.0f / (total_norm + 1e-6f)) * (float)max_norm, 1.0f)
+ *   each operation rounded to float32, as torch's `max_norm / (total_norm + 1e-6)` (Tensor.__rdiv__: reciprocal, then
+ *   multiply) and clamp(max=1) round it; a NaN coefficient stays NaN.  Every gradient element g becomes g * coef
+ *   (rounded), also when coef == 1; a non-finite norm propagates as in torch (inf: coef 0, NaN where g is inf).
+ *   *d_total_norm gets total_norm.  No atomics: equal inputs give equal bits.  max_norm NaN computes the norm only and
+ *   leaves the gradients untouched (the check of clip_grad_norm_(error_if_nonfinite=True) before it scales).
+ *   d_workspace: wekws_grad_clip_workspace_bytes(n, E) = 8 G ceil(n / 1024) bytes.
+ *   wekws_grad_clip_launches(n) = 2 ceil(n / 1024).
+ * wekws_adam_step: one step of torch 2.11's _multi_tensor_adam with amsgrad, maximize and capturable off and L2
+ *   weight decay, in place on params, exp_avg and exp_avg_sq; the gradients are read only.  The scalars are rounded
+ *   to float32 as torch's foreach kernels take them: w = (float)(1 - beta1), b2 = (float)beta2, c2 = (float)(1 - beta2),
+ *   e = (float)eps, wd = (float)weight_decay, and per tensor i ss = (float)h_step_size[i], bc = (float)h_bc2_sqrt[i],
+ *   where the caller forms, in double, step_size = (lr / (1 - beta1 ** step)) * -1 and bc2_sqrt = (1 - beta2 ** step)
+ *   ** 0.5 with the tensor's own step (torch's own expressions).  Per element, fma() one rounding, every other
+ *   operation rounded to float32 on its own:
+ *     g = weight_decay != 0 ? fma(wd, p, grad) : grad
+ *     m = |w| < 0.5 ? fma(w, g - m, m) : fma(-(g - m), 1 - w, g)        (torch's lerp)
+ *     v = fma(c2, g * g, v * b2)
+ *     p = fma(ss, m / (sqrt(v) / bc + e), p)
+ *   wekws_adam_step_launches(n) = ceil(n / 512).                                                                */
+WEKWS_API int64_t wekws_grad_clip_workspace_bytes(int n, int64_t total_elems);
+WEKWS_API int wekws_grad_clip_launches(int n);
+WEKWS_API int wekws_grad_clip(float* const* h_grads, const int64_t* h_numel, int n, double max_norm,
+                              float* d_total_norm, void* d_workspace, void* stream);
+WEKWS_API int wekws_adam_step_launches(int n);
+WEKWS_API int wekws_adam_step(float* const* h_params, const float* const* h_grads, float* const* h_exp_avg,
+                              float* const* h_exp_avg_sq, const int64_t* h_numel, const double* h_step_size,
+                              const double* h_bc2_sqrt, int n, double beta1, double beta2, double eps,
+                              double weight_decay, void* stream);
 
 #ifdef __cplusplus
 }

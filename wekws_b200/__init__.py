@@ -20,6 +20,8 @@ Public surface mirrors the reference (wenet-e2e/wekws):
                                 Fbank / MFCC, SpecAugment, context expansion, frame skip and padding() on the device
     AugmentSource, reverb, add_noise <- processor.py add_reverb / add_noise with their LMDB sources: room
                                 reverberation and additive noise of the training audio on the device
+    Adam, clip_grad_norm_    <- torch.optim.Adam / torch.nn.utils.clip_grad_norm_ as Executor.train calls them: the
+                                training step's gradient clip and optimiser update on the device
     export_native()          -> weight file for the C++ runtime shim (the role of wekws/bin/export_onnx.py)
     export_onnx()            <- wekws/bin/export_onnx.py: the ONNX file (input, cache -> output, r_cache) for the ORT runtime
 """
@@ -27,6 +29,7 @@ from .augment import AugmentSource, add_noise, reverb
 from .cmvn import load_cmvn, load_kaldi_cmvn
 from .cmvn_stats import CmvnStats, scp_segment
 from .configs import MODEL_NAMES, model_config
+from .optim import Adam, clip_grad_norm_
 from .frontend import Fbank, Mfcc, Resample, fbank, mfcc, resample
 from .kws_model import GlobalCMVN, KWSModel, init_model
 from .ctc import (ctc_keyword_hits, ctc_prefix_beam_search, ctc_state, stream_score_ctc, write_ctc_scores,
@@ -46,5 +49,6 @@ __all__ = ["init_model", "KWSModel", "GlobalCMVN", "Fbank", "fbank", "Mfcc", "mf
            "Pipeline", "ctc_prefix_beam_search", "ctc_keyword_hits", "ctc_state", "write_ctc_scores",
            "KeywordSpotter", "SpotResult", "stream_score_ctc", "write_stream_ctc_scores", "ctc_det_stats",
            "write_ctc_det_stats", "space_mixed_label", "criterion", "Resample", "resample", "CmvnStats", "scp_segment",
-           "TrainFeatures", "spec_aug", "AugmentSource", "reverb", "add_noise"]
+           "TrainFeatures", "spec_aug", "AugmentSource", "reverb", "add_noise", "Adam",
+           "clip_grad_norm_"]
 __version__ = "0.1.0"

@@ -23,7 +23,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 17
+ABI_VERSION = 18
 
 # limits (include/wekws_b200.h #defines)
 CTC_MAX_PREFIX, CTC_MAX_PATH_BEAM, CTC_MAX_SCORE_BEAM = 64, 20, 3
@@ -204,6 +204,12 @@ SIGNATURES = {
     "wekws_resample_output_length": (C.c_int64, [C.c_void_p, C.c_int64]),
     "wekws_resample_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
                                          C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    "wekws_grad_clip_workspace_bytes": (C.c_int64, [C.c_int, C.c_int64]),
+    "wekws_grad_clip_launches": (C.c_int, [C.c_int]),
+    "wekws_grad_clip": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_adam_step_launches": (C.c_int, [C.c_int]),
+    "wekws_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_void_p]),
     "wekws_cmvn_stats_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int]),
     "wekws_cmvn_stats_accumulate": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p]),
