@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define WEKWS_B200_ABI_VERSION 18  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask; 16: + wekws_mdtc_head_* (MDTC training with the global / last head); 17: + wekws_gru_* (GRU training); 18: + wekws_grad_clip*, wekws_adam_step* (the optimiser step) */
+#define WEKWS_B200_ABI_VERSION 19  /* 2: + wekws_fbank_set_mfcc, wekws_fbank_feature_dim, wekws_det_stats; 3: det max_score is double; 4: precision mode 2, wekws_model_uses_tensor_cores_bt; 5: wekws_model_set_head; 6: + wekws_stream_pcm, wekws_stream_context, wekws_ctc_spot, wekws_ctc_spot_state_bytes; 7: + wekws_ctc_stream_score, wekws_ctc_stream_detection; 8: + wekws_criterion_*; 9: + wekws_resample_*, wekws_cmvn_stats_*; 10: + wekws_fbank_forward_dither, wekws_dither_noise, wekws_spec_aug; 11: + wekws_reverb, wekws_add_noise; 12: + wekws_criterion_*_train, wekws_criterion_*_backward; 13: + wekws_fsmn_* (FSMN training); 14: + wekws_mdtc_* (MDTC training); 15: + wekws_tcn_* (TCN / DS-TCN training), wekws_dropout_mask; 16: + wekws_mdtc_head_* (MDTC training with the global / last head); 17: + wekws_gru_* (GRU training); 18: + wekws_grad_clip*, wekws_adam_step* (the optimiser step); 19: one set of training entry points for every model, wekws_train_* and wekws_model_load_params / _train_forward / _backward, in place of the per-model ones */
 
 #if defined(__GNUC__)
 #define WEKWS_API __attribute__((visibility("default")))
@@ -461,210 +461,154 @@ WEKWS_API int wekws_criterion_ctc_backward(const float* d_logits, const int32_t*
                         const float* d_row_max, const float* d_row_sum, const float* d_utt_loss, float* d_alpha,
                         int alpha_is_occupancy, const float* d_upstream, float* d_grad, void* stream);
 
-/* Training the FSMN model (wekws/utils/executor.py Executor.train with an fsmn_ctc.yaml model): the training-mode
- * forward keeps its activations, the backward gives the gradient of every parameter of wekws/model/fsmn.py FSMN.
- * The handle is an FSMN model made by wekws_model_create / _set_tensor / _finalize, with the identity activation
- * (every FSMN config).  Parameters and gradients travel as host arrays of wekws_fsmn_num_params(m) = 8 + 5 L device
- * pointers, in state_dict order (the model's parameters without the CMVN buffers):
- *   backbone.in_linear1.linear.{weight,bias}, backbone.in_linear2.linear.{weight,bias},
- *   per layer l: backbone.fsmn.{l}.0.linear.weight, .1.conv_left.weight, .1.conv_right.weight, .2.linear.{weight,bias},
- *   backbone.out_linear1.linear.{weight,bias}, backbone.out_linear2.linear.{weight,bias}
- * each contiguous float32 in the parameter's own shape (conv_left.weight is (proj, 1, left_order, 1)).
+/* Training on the device (wekws/utils/executor.py Executor.train): a training-mode forward that keeps what its backward
+ * reads, and the backward to every parameter.  Five models train; every entry point below resolves which one from the
+ * handle's backbone and head:
+ *   MDTC with the per-frame linear classifier, MDTC with the global / last head, TCN / DS-TCN with the per-frame linear
+ *   classifier (the BatchNorm models), FSMN, GRU.
+ * A TCN / DS-TCN with a head and a model outside a family's limits below are refused (WEKWS_ERR_INVALID, the message
+ * says why).
  *
- * wekws_fsmn_load_params: the handle's packed weights from those tensors, on the device (1 launch): the optimiser's
- *   updates reach the kernels without a host round trip.  The CMVN buffers keep what _finalize packed.
- * wekws_fsmn_train_forward: wekws_model_forward of B utterances of T frames from empty caches (same launches, same
- *   d_out / d_out_cache bits), also writing d_saved: wekws_fsmn_train_saved_floats(m, B, T) =
- *   B * T * (input_affine_dim + linear_dim + L * (2 proj_dim + linear_dim) + output_affine_dim) floats.
- * wekws_fsmn_backward: from d_feats and d_saved of that forward and d_grad_out = d loss / d out (B, T, odim), writes
- *   every element of every gradient buffer, with all B * T frames as rows (padding included, as torch does).  Weight
- *   and bias gradients are summed in 32 fixed row slices, then the slices in order: no atomics, equal inputs give
- *   equal bits.  d_workspace: wekws_fsmn_backward_workspace_bytes(m, B, T) = 4 * (32 * (number of parameter
- *   elements) + 2 * B * T * max(input_affine_dim, linear_dim, proj_dim, output_affine_dim)) bytes.
- *   wekws_fsmn_backward_launches(m) = 8 + 5 L launches.                                                        */
-WEKWS_API int wekws_fsmn_num_params(const wekws_model* m);
-WEKWS_API int wekws_fsmn_load_params(wekws_model* m, const float* const* h_params, int n, void* stream);
-WEKWS_API int64_t wekws_fsmn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int wekws_fsmn_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
-                                       float* d_saved, int64_t B, int64_t T, void* stream);
-WEKWS_API int64_t wekws_fsmn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int wekws_fsmn_backward_launches(const wekws_model* m);
-WEKWS_API int wekws_fsmn_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_grad_out,
-                                  int64_t B, int64_t T, float* const* h_grads, int n, void* d_workspace, void* stream);
-
-/* Training the GRU model (Executor.train with examples/hi_xiaowen/s0/conf/gru.yaml): the training-mode forward keeps
- * every step's gates, the backward through time gives the gradient of every parameter of wekws/model/kws_model.py
- * with the GRU backbone (preprocessing Linear + ReLU, torch.nn.GRU, linear classifier).  The handle is a GRU model
- * made by wekws_model_create / _set_tensor / _finalize (hidden_dim 128, 1..4 layers, input_dim 1..128, the linear
- * classifier, Sigmoid or Identity).  Parameters and gradients travel as host arrays of wekws_gru_num_params(m) =
- * 4 + 4 L device pointers in named_parameters order, each contiguous float32 in the parameter's own shape:
- *   preprocessing.out.0.{weight,bias}, per layer k: backbone.{weight_ih,weight_hh,bias_ih,bias_hh}_l{k},
- *   classifier.linear.{weight,bias}
+ * Parameters and gradients travel as host arrays of wekws_train_num_params(m) device pointers, each contiguous float32
+ * in the parameter's own shape, in the order each family lists below; a backward writes every element of every
+ * gradient buffer, with all B * T frames as rows (padding included, as torch does).  Weight and bias gradients are
+ * summed over fixed row slices and the slices added in order: no atomics, equal inputs give equal bits.
  *
- * wekws_gru_load_params: the handle's packed FP32 weights from those tensors, on the device (1 launch): the
- *   optimiser's updates reach the kernels without a host round trip.  The CMVN buffers keep what _finalize packed;
- *   the tensor-core weight image is not updated (the training forward does not read it).
- * wekws_gru_train_forward: the FP32 kernel of wekws_model_forward (whatever the precision mode) over B utterances of T
- *   frames from empty caches, one launch, the same d_out / d_out_cache bits, also writing d_saved:
- *   wekws_gru_train_saved_floats(m, B, T) = (1 + 5 L) B T hidden_dim floats, (B T, hidden_dim) row-major blocks with
- *   row b T + t: x0 = ReLU(Linear(CMVN(feats))), then per layer h_t, r, z, n and W_hn h_{t-1} + b_hn.
- * wekws_gru_backward: from d_feats, d_saved and d_out (the logits) of that forward and d_grad_out = d loss / d out
- *   (B, T, odim), writes every element of every gradient buffer, all B T frames as rows (padding included, as torch
- *   does).  Per layer one sequential kernel runs the recurrence backwards in time; the weight gradients are summed in
- *   32 fixed row slices, then the slices in order: no atomics, equal inputs give equal bits.  d_workspace:
- *   wekws_gru_backward_workspace_bytes(m, B, T) = 4 * (32 P + B T (8 hidden_dim + odim)) bytes, P the number of
- *   parameter elements.  wekws_gru_backward_launches(m) = 5 + 4 L launches.
- * The size and launch queries read the config only; they return a negative status (0 for the counts) for another
- * backbone.                                                                                                       */
-WEKWS_API int wekws_gru_num_params(const wekws_model* m);
-WEKWS_API int wekws_gru_load_params(wekws_model* m, const float* const* h_params, int n, void* stream);
-WEKWS_API int64_t wekws_gru_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int wekws_gru_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
-                                      float* d_saved, int64_t B, int64_t T, void* stream);
-WEKWS_API int64_t wekws_gru_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int wekws_gru_backward_launches(const wekws_model* m);
-WEKWS_API int wekws_gru_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_out,
-                                 const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads, int n,
-                                 void* d_workspace, void* stream);
-
-/* Training the MDTC model (wekws/utils/executor.py Executor.train with an mdtc.yaml / mdtc_small.yaml model): the
- * training-mode forward, every BatchNorm normalising with the biased variance of the batch (all B * T frames, padding
- * included) and updating its running statistics, and the backward to every parameter of wekws/model/mdtc.py MDTC.
- * The handle only supplies the config (wekws_model_create is enough): an MDTC model with hidden_dim 32 or 64, the
- * per-frame linear classifier (no wekws_model_set_head), input_dim <= 128, output_dim <= 16, kernel_size <= 8 and at
- * most 25 blocks.  Everything the kernels read travels with the call, so an optimiser step needs no host round trip:
- *   h_params: wekws_mdtc_num_params(m) = 4 + 12 L device pointers (L = 1 + num_stack * stack_size blocks), in
- *     named_parameters order, each contiguous float32 in the parameter's own shape:
+ * The queries read the config only.  wekws_train_num_params and the launch counts return 0, the sizes a negative
+ * status, for a model they do not accept.  wekws_train_saved_floats(m, B, T): the floats of d_saved a forward of B
+ * utterances of T frames writes; wekws_train_backward_workspace_bytes(m, B, T): the bytes of the backward's
+ * d_workspace; wekws_train_backward_launches(m): the backward's kernel launches.
+ *
+ * Two calling conventions; a handle of the other one is refused with a message naming its entry points.
+ *
+ * The BatchNorm models: wekws_train_forward / wekws_train_backward on a handle that only supplies the config
+ * (wekws_model_create, plus wekws_model_set_head for a head).  Everything the kernels read travels with the call, so an
+ * optimiser step needs no host round trip.
+ *   h_params, n: the parameters.  d_cmvn_mean / d_cmvn_istd: global_cmvn.{mean,istd} (idim floats), or both NULL
+ *     without CMVN; cfg.norm_var applies.
+ *   h_running: 2 N device pointers, running_mean and running_var of each of the model's N BatchNorms in the order
+ *     below; h_bn: 2 N host doubles, (momentum, eps) of the same BatchNorms.  Every BatchNorm normalises with the
+ *     biased variance of the batch (all B * T frames, padding included) and updates its running statistics,
+ *     running_var with the unbiased variance.  The kernel writes them: a packed eval model of the same weights must be
+ *     re-made (wekws_model_finalize) to see them.
+ *   Dropout: seed, a 64-bit seed, and h_p, n_p host doubles, one probability in [0, 1] per Dropout module; n_p must be
+ *     the model's Dropout count (MDTC 0, h_p may be NULL; MDTC with a head 1; TCN / DS-TCN L, one per block).  Each
+ *     module applies a mask that is a pure function of the seed: element e is kept iff (word >> 8) >= theta, theta =
+ *     ceil(p 2^24) (in double), word = a component of Philox4x32-10(counter, key = (seed lo, seed hi)) (Random123
+ *     constants, as the dither; the dither's counters have word 3 = 0, so the streams are disjoint); a kept element is
+ *     multiplied by 1.0f / (float)(1 - p), a dropped one is 0 (selected, not multiplied: p = 1 gives exact zeros).  The
+ *     backward recomputes the masks from the same seed and h_p.  wekws_dropout_mask (test hook): d_out (B, T, C) bytes,
+ *     1 where block `layer` keeps the element, for theta.
+ *   wekws_train_forward: B utterances of T frames (B * T >= 2) from empty caches: d_out, d_out_cache (B, hdim,
+ *     padding) as the reference's training-mode new_cache.  save != 0: also writes d_saved; save == 0: d_saved may be
+ *     NULL, same d_out / d_out_cache / running-statistics bits.  d_workspace: wekws_train_workspace_bytes(m, B, T,
+ *     save) bytes; wekws_train_forward_launches(m) launches either way.
+ *   wekws_train_backward: from d_feats, the same h_params / CMVN buffers / seed / h_p and d_saved of a save != 0
+ *     forward and d_grad_out = d loss / d out (shaped as d_out), writes h_grads (same shapes as h_params).  d_out, the
+ *     forward's logits, is read by the TCN / DS-TCN backward only; the others accept NULL.  Batch statistics are
+ *     formed in double over 128 fixed row slices.
+ *
+ * FSMN and GRU: the packed weights of a handle made by wekws_model_create / _set_tensor / _finalize, as
+ * wekws_model_forward runs it.
+ *   wekws_model_load_params: the handle's packed weights from h_params, on the device (1 launch): the optimiser's
+ *     updates reach the kernels without a host round trip.  The CMVN buffers keep what _finalize packed.
+ *   wekws_model_train_forward: wekws_model_forward of B utterances of T frames from empty caches, the same d_out /
+ *     d_out_cache bits, also writing d_saved.
+ *   wekws_model_backward: from d_feats, d_saved (and, GRU only, d_out, the logits) of that forward and d_grad_out =
+ *     d loss / d out (B, T, odim), writes the n = wekws_train_num_params(m) gradient buffers h_grads.
+ *
+ * MDTC (an mdtc.yaml / mdtc_small.yaml model, wekws/model/mdtc.py): hidden_dim 32 or 64, the per-frame linear
+ * classifier (no wekws_model_set_head), input_dim <= 128, output_dim <= 16, kernel_size <= 8, at most 25 blocks.
+ *   h_params: 4 + 12 L (L = 1 + num_stack * stack_size blocks), named_parameters order:
  *     preprocessing.out.0.{weight,bias}; per block (backbone.preprocessor, then backbone.blocks.{s}.res_blocks.{l}):
  *     conv1.conv.{weight,bias}, conv1.bn.{weight,bias}, conv1.pointwise.{weight,bias}, bn1.{weight,bias},
  *     conv2.{weight,bias}, bn2.{weight,bias}; classifier.linear.{weight,bias}.
- *   d_cmvn_mean / d_cmvn_istd: global_cmvn.{mean,istd} (idim floats), or both NULL without CMVN; cfg.norm_var applies.
- *   h_running: 6 L device pointers, running_mean and running_var of conv1.bn, bn1, bn2 of each block in block order;
- *     h_bn: 6 L host doubles, (momentum, eps) of the same BatchNorms.  running_var takes the unbiased variance.  The
- *     kernel writes them: a packed eval model of the same weights must be re-made (wekws_model_finalize) to see them.
+ *   BatchNorms: conv1.bn, bn1, bn2 of each block in block order (N = 3 L).
+ *   d_out (B, T, odim).  Saved: 12 L hdim + B T hdim (4 L + 2) floats (each BatchNorm's mean and invstd, the
+ *   preprocessing output, per block its three pre-BatchNorm tensors and its output, the stack sum).  Forward workspace
+ *   48 * 128 hdim + (save ? 0 : 24 B T hdim) bytes, 2 + 3 L launches.  Every batch statistic and weight-gradient sum is
+ *   formed in double over 128 fixed row slices.  Backward workspace 32 * 128 hdim + 20 B T hdim + 8 * 128 P bytes, P
+ *   the number of weight and bias elements of the preprocessing Linear, the convolutions and the classifier;
+ *   3 + 4 L launches.
  *
- * wekws_mdtc_train_forward: B utterances of T frames (B * T >= 2) from empty caches: d_out (B, T, odim), d_out_cache
- *   (B, hdim, padding) as the reference's training-mode new_cache.  save != 0: also writes d_saved,
- *   wekws_mdtc_train_saved_floats(m, B, T) = 12 L hdim + B T hdim (4 L + 2) floats (each BatchNorm's mean and invstd,
- *   the preprocessing output, per block its three pre-BatchNorm tensors and its output, the stack sum).  save == 0:
- *   d_saved may be NULL, same d_out / d_out_cache / running-statistics bits.  d_workspace:
- *   wekws_mdtc_train_workspace_bytes(m, B, T, save) = 48 * 128 hdim + (save ? 0 : 24 B T hdim) bytes.
- *   wekws_mdtc_train_forward_launches(m) = 2 + 3 L launches either way.
- * wekws_mdtc_backward: from d_feats, the same h_params / CMVN buffers and d_saved of a save != 0 forward and
- *   d_grad_out = d loss / d out (B, T, odim), writes every element of the 4 + 12 L gradient buffers h_grads (same
- *   shapes as h_params), all B * T frames as rows.  Every batch statistic and weight-gradient sum is formed in double
- *   over 128 fixed row slices and the slices added in order: no atomics, equal inputs give equal bits.
- *   d_workspace: wekws_mdtc_backward_workspace_bytes(m, B, T) = 32 * 128 hdim + 20 B T hdim + 8 * 128 P bytes, P the
- *   number of weight and bias elements of the preprocessing Linear, the convolutions and the classifier.
- *   wekws_mdtc_backward_launches(m) = 3 + 4 L launches.
- * The size and launch queries return a negative status (0 for the counts) for a model they do not accept.        */
-WEKWS_API int wekws_mdtc_num_params(const wekws_model* m);
-WEKWS_API int64_t wekws_mdtc_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int64_t wekws_mdtc_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save);
-WEKWS_API int wekws_mdtc_train_forward_launches(const wekws_model* m);
-WEKWS_API int wekws_mdtc_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                       const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
-                                       const double* h_bn, float* d_out, float* d_out_cache, float* d_saved, int save,
-                                       void* d_workspace, int64_t B, int64_t T, void* stream);
-WEKWS_API int64_t wekws_mdtc_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int wekws_mdtc_backward_launches(const wekws_model* m);
-WEKWS_API int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                  const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
-                                  const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads,
-                                  void* d_workspace, void* stream);
-
-/* Training the TCN / DS-TCN model (Executor.train with a tcn.yaml / ds_tcn.yaml / ds_tcn_ctc.yaml model): the
- * training-mode forward of wekws/model/tcn.py with the per-frame linear classifier, every BatchNorm as in MDTC
- * training above, every block's Dropout applying a device mask, and the backward to every parameter.  Supported: the
- * dense (TCN) and depthwise-separable (DS-TCN) backbones, hidden_dim 64 or 256, kernel_size 2..8, 1..8 layers,
- * input_dim <= 128, output_dim <= 4096; the per-frame linear classifier; Sigmoid or Identity activation.
- *   h_params: wekws_tcn_num_params(m) = 4 + P L device pointers (P = 4 dense, 8 ds), named_parameters order:
- *     preprocessing.out.0.{weight,bias}; per block backbone.network.{l}.cnn.: 0.{weight,bias} (the dilated conv),
- *     1.{weight,bias} (BatchNorm), ds only: 3.{weight,bias} (pointwise conv), 4.{weight,bias} (BatchNorm);
- *     classifier.linear.{weight,bias}.
- *   h_running / h_bn: as for MDTC, for the BatchNorms cnn.1 [, cnn.4] of each block in block order (L or 2 L).
- *   Dropout: h_p, L host doubles, block l's probability p_l; seed, a 64-bit seed.  Element (b, t, c) of block l's
- *     ReLU output is kept iff (word >> 8) >= theta_l, theta_l = ceil(p_l 2^24) (in double), word = component c % 4
- *     of Philox4x32-10(counter = (c / 4, t, b, 1 + l), key = (seed lo, seed hi)) (Random123 constants, as the dither;
- *     the dither's counters have word 3 = 0, so the streams are disjoint); a kept element is multiplied by
- *     s_l = 1.0f / (float)(1 - p_l), a dropped one is 0 (selected, not multiplied: p = 1 gives exact zeros).  The
- *     backward recomputes the masks from the same seed and h_p.
- * wekws_tcn_train_forward: B utterances of T frames (B * T >= 2) from empty caches: d_out (B, T, odim), d_out_cache
- *   (B, hdim, padding).  save != 0: also writes d_saved, wekws_tcn_train_saved_floats(m, B, T) = 4 N hdim +
- *   B T hdim (1 + L (P / 4 + 1)) floats, N = L (dense) or 2 L (ds) BatchNorms (each BatchNorm's mean and invstd as
- *   doubles, the preprocessing output, per block its pre-BatchNorm tensors and its output).  d_workspace:
- *   wekws_tcn_train_workspace_bytes(m, B, T, save) = 32 * 128 hdim + (save ? 0 : 16 B T hdim) bytes.
- *   wekws_tcn_train_forward_launches(m) = 2 + L (dense) or 2 + 2 L (ds) launches either way.
- * wekws_tcn_backward: from d_feats, the same h_params / CMVN buffers / seed / h_p, d_saved and d_out of a save != 0
- *   forward and d_grad_out (B, T, odim), writes every element of the gradient buffers h_grads.  Batch statistics are
- *   formed in double over 128 fixed row slices; each weight gradient over Z fixed row ranges (FP32 over 256 rows,
- *   double across them), Z = min(64, max(1, B T / 256), ceil(264 / tiles)) with tiles = ceil(N / 64) ceil((Q + 1) / 64)
- *   for an N x Q weight and its bias; the partials are added in order: no atomics, equal inputs give equal bits.
- *   d_workspace: wekws_tcn_backward_workspace_bytes(m, B, T) = 32 * 128 hdim + 16 B T hdim + 8 (sum of Z N (Q + 1)
- *   over the weights, + 128 hdim (K + 1) per ds block) bytes.  wekws_tcn_backward_launches(m) = 4 + 2 L (dense) or
- *   4 + 3 L (ds) launches.
- * wekws_dropout_mask (test hook): d_out (B, T, C) bytes, 1 where block `layer` keeps the element, for theta.       */
-WEKWS_API int wekws_tcn_num_params(const wekws_model* m);
-WEKWS_API int64_t wekws_tcn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int64_t wekws_tcn_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save);
-WEKWS_API int wekws_tcn_train_forward_launches(const wekws_model* m);
-WEKWS_API int wekws_tcn_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                      const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
-                                      const double* h_bn, uint64_t seed, const double* h_p, float* d_out,
-                                      float* d_out_cache, float* d_saved, int save, void* d_workspace, int64_t B,
-                                      int64_t T, void* stream);
-WEKWS_API int64_t wekws_tcn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int wekws_tcn_backward_launches(const wekws_model* m);
-WEKWS_API int wekws_tcn_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                 const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
-                                 const float* d_out, const float* d_grad_out, uint64_t seed, const double* h_p,
-                                 int64_t B, int64_t T, float* const* h_grads, void* d_workspace, void* stream);
+ * MDTC with the global / last head (examples/speechcommand_v1/s0/conf/mdtc.yaml): the MDTC backbone as above with the
+ * utterance-level head of wekws/model/classifier.py in place of the per-frame linear classifier: GlobalClassifier (the
+ * mean over all T frames, padding included) or LastClassifier (frame T - 1) around Linear(hdim, 64) -> ReLU ->
+ * Dropout(p) -> Linear(64, odim), the Identity activation; within the MDTC limits except output_dim, here 1..4096.
+ *   h_params: 6 + 12 L, the MDTC parameters with classifier.classifier.0.{weight,bias} (64, hdim), (64) and
+ *     classifier.classifier.3.{weight,bias} (odim, 64), (odim) in place of classifier.linear.{weight,bias}.
+ *   BatchNorms: as MDTC.  Dropout (n_p = 1): element (b, j) of the head's ReLU output (B, 64) uses component j % 4 of
+ *     counter (j / 4, 0, b, 256): wekws_dropout_mask(seed, B, 1, 64, 255, theta) gives the mask.  Counter word 3 = 256
+ *     keeps the stream apart from the dither's (0) and the TCN blocks' (1..8).
+ *   d_out (B, odim).  Saved: 12 L hdim + B T hdim (4 L + 2) + B (hdim + 64) floats (MDTC training's, then the pooled
+ *   vectors and the head's pre-ReLU hidden vectors).  Forward workspace 48 * 128 hdim + (save ? 0 : 24 B T hdim) bytes,
+ *   3 + 3 L launches.  The head's weight gradients are sums over the utterances in utterance order, in double, rounded
+ *   once; the backbone's as MDTC.  Backward workspace 32 * 128 hdim + 24 B T hdim + 8 * 128 P + 512 B bytes, P the
+ *   number of weight and bias elements of the preprocessing Linear and the convolutions; 4 + 4 L launches.
+ *
+ * TCN / DS-TCN (a tcn.yaml / ds_tcn.yaml / ds_tcn_ctc.yaml model, wekws/model/tcn.py): the dense (TCN) and
+ * depthwise-separable (DS-TCN) backbones, hidden_dim 64 or 256, kernel_size 2..8, 1..8 layers, input_dim <= 128,
+ * output_dim <= 4096; the per-frame linear classifier; Sigmoid or Identity activation.
+ *   h_params: 4 + P L (P = 4 dense, 8 ds), named_parameters order: preprocessing.out.0.{weight,bias}; per block
+ *     backbone.network.{l}.cnn.: 0.{weight,bias} (the dilated conv), 1.{weight,bias} (BatchNorm), ds only:
+ *     3.{weight,bias} (pointwise conv), 4.{weight,bias} (BatchNorm); classifier.linear.{weight,bias}.
+ *   BatchNorms: cnn.1 [, cnn.4] of each block in block order (N = L or 2 L).  Dropout (n_p = L): element (b, t, c) of
+ *     block l's ReLU output uses p_l and component c % 4 of counter (c / 4, t, b, 1 + l).
+ *   d_out (B, T, odim).  Saved: 4 N hdim + B T hdim (1 + L (P / 4 + 1)) floats (each BatchNorm's mean and invstd as
+ *   doubles, the preprocessing output, per block its pre-BatchNorm tensors and its output).  Forward workspace
+ *   32 * 128 hdim + (save ? 0 : 16 B T hdim) bytes, 2 + L (dense) or 2 + 2 L (ds) launches.  Each weight gradient is
+ *   formed over Z fixed row ranges (FP32 over 256 rows, double across them), Z = min(64, max(1, B T / 256),
+ *   ceil(264 / tiles)) with tiles = ceil(N / 64) ceil((Q + 1) / 64) for an N x Q weight and its bias, the partials
+ *   added in order.  Backward workspace 32 * 128 hdim + 16 B T hdim + 8 (sum of Z N (Q + 1) over the weights,
+ *   + 128 hdim (K + 1) per ds block) bytes; 4 + 2 L (dense) or 4 + 3 L (ds) launches.
+ *
+ * FSMN (an fsmn_ctc.yaml model, wekws/model/fsmn.py FSMN): every FSMN config, with the identity activation.
+ *   h_params: 8 + 5 L, state_dict order (the model's parameters without the CMVN buffers):
+ *     backbone.in_linear1.linear.{weight,bias}, backbone.in_linear2.linear.{weight,bias},
+ *     per layer l: backbone.fsmn.{l}.0.linear.weight, .1.conv_left.weight, .1.conv_right.weight,
+ *     .2.linear.{weight,bias},
+ *     backbone.out_linear1.linear.{weight,bias}, backbone.out_linear2.linear.{weight,bias}
+ *     (conv_left.weight is (proj, 1, left_order, 1)).
+ *   The forward runs wekws_model_forward's launches.  Saved: B * T * (input_affine_dim + linear_dim + L * (2 proj_dim +
+ *   linear_dim) + output_affine_dim) floats.  The weight and bias gradients are summed in 32 fixed row slices.
+ *   Backward workspace 4 * (32 * (number of parameter elements) + 2 * B * T * max(input_affine_dim, linear_dim,
+ *   proj_dim, output_affine_dim)) bytes; 8 + 5 L launches.
+ *
+ * GRU (examples/hi_xiaowen/s0/conf/gru.yaml, wekws/model/kws_model.py with the GRU backbone: preprocessing Linear +
+ * ReLU, torch.nn.GRU, linear classifier): hidden_dim 128, 1..4 layers, input_dim 1..128, the linear classifier, Sigmoid
+ * or Identity.
+ *   h_params: 4 + 4 L, named_parameters order: preprocessing.out.0.{weight,bias}, per layer k:
+ *     backbone.{weight_ih,weight_hh,bias_ih,bias_hh}_l{k}, classifier.linear.{weight,bias}.  wekws_model_load_params
+ *     does not update the tensor-core weight image (the training forward does not read it).
+ *   The forward is the FP32 kernel of wekws_model_forward (whatever the precision mode), one launch.  Saved:
+ *   (1 + 5 L) B T hidden_dim floats, (B T, hidden_dim) row-major blocks with row b T + t:
+ *   x0 = ReLU(Linear(CMVN(feats))), then per layer h_t, r, z, n and W_hn h_{t-1} + b_hn.  Per layer one sequential
+ *   kernel runs the recurrence backwards in time; the weight gradients are summed in 32 fixed row slices.  Backward
+ *   workspace 4 * (32 P + B T (8 hidden_dim + odim)) bytes, P the number of parameter elements; 5 + 4 L launches.   */
+WEKWS_API int wekws_train_num_params(const wekws_model* m);
+WEKWS_API int64_t wekws_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int64_t wekws_train_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
+WEKWS_API int wekws_train_backward_launches(const wekws_model* m);
+WEKWS_API int64_t wekws_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save);
+WEKWS_API int wekws_train_forward_launches(const wekws_model* m);
+WEKWS_API int wekws_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                  const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
+                                  const double* h_bn, uint64_t seed, const double* h_p, int n_p, float* d_out,
+                                  float* d_out_cache, float* d_saved, int save, void* d_workspace, int64_t B, int64_t T,
+                                  void* stream);
+WEKWS_API int wekws_train_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                   const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                   const float* d_out, const float* d_grad_out, uint64_t seed, const double* h_p,
+                                   int n_p, int64_t B, int64_t T, float* const* h_grads, void* d_workspace,
+                                   void* stream);
+WEKWS_API int wekws_model_load_params(wekws_model* m, const float* const* h_params, int n, void* stream);
+WEKWS_API int wekws_model_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
+                                        float* d_saved, int64_t B, int64_t T, void* stream);
+WEKWS_API int wekws_model_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_out,
+                                   const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads, int n,
+                                   void* d_workspace, void* stream);
 WEKWS_API int wekws_dropout_mask(uint64_t seed, int64_t B, int64_t T, int64_t C, int layer, uint32_t theta,
                                  uint8_t* d_out, void* stream);
-
-/* Training the speech-command MDTC model (Executor.train with examples/speechcommand_v1/s0/conf/mdtc.yaml): the MDTC
- * backbone's training forward and backward as in MDTC training above, with the utterance-level head of
- * wekws/model/classifier.py in place of the per-frame linear classifier: GlobalClassifier (the mean over all T frames,
- * padding included) or LastClassifier (frame T - 1) around Linear(hdim, 64) -> ReLU -> Dropout(p) -> Linear(64, odim),
- * the Identity activation.  The handle only supplies the config plus wekws_model_set_head (GLOBAL or LAST): an MDTC
- * model within the limits of MDTC training above except output_dim, here 1..4096, and the Identity activation.  The
- * wekws_mdtc_* entry points above refuse a head model; these refuse a linear-classifier model.
- *   h_params: wekws_mdtc_head_num_params(m) = 6 + 12 L device pointers, named_parameters order: the MDTC parameters
- *     above with classifier.classifier.0.{weight,bias} (64, hdim), (64) and classifier.classifier.3.{weight,bias}
- *     (odim, 64), (odim) in place of classifier.linear.{weight,bias}.  h_running / h_bn / CMVN buffers: as above.
- *   Dropout: p in [0, 1] and a 64-bit seed.  Element (b, j) of the head's ReLU output (B, 64) is kept iff
- *     (word >> 8) >= theta, theta = ceil(p 2^24) (in double), word = component j % 4 of Philox4x32-10(counter =
- *     (j / 4, 0, b, 256), key = (seed lo, seed hi)): wekws_dropout_mask(seed, B, 1, 64, 255, theta) gives the mask.
- *     Counter word 3 = 256 keeps the stream apart from the dither's (0) and the TCN blocks' (1..8).  A kept element is
- *     multiplied by 1.0f / (float)(1 - p), a dropped one is 0 (selected: p = 1 gives exact zeros).  The backward
- *     recomputes the mask from the same seed and p.
- * wekws_mdtc_head_train_forward: B utterances of T frames (B * T >= 2) from empty caches: d_out (B, odim), d_out_cache
- *   (B, hdim, padding).  save != 0: also writes d_saved, wekws_mdtc_head_train_saved_floats(m, B, T) = 12 L hdim +
- *   B T hdim (4 L + 2) + B (hdim + 64) floats (MDTC training's, then the pooled vectors and the head's pre-ReLU
- *   hidden vectors).  d_workspace: wekws_mdtc_head_train_workspace_bytes(m, B, T, save) = 48 * 128 hdim + (save ? 0 :
- *   24 B T hdim) bytes.  wekws_mdtc_head_train_forward_launches(m) = 3 + 3 L launches either way.
- * wekws_mdtc_head_backward: from d_feats, the same h_params / CMVN buffers / seed / p and d_saved of a save != 0
- *   forward and d_grad_out (B, odim), writes every element of the 6 + 12 L gradient buffers h_grads.  The head's weight
- *   gradients are sums over the utterances in utterance order, in double, rounded once; the backbone's as above.
- *   d_workspace: wekws_mdtc_head_backward_workspace_bytes(m, B, T) = 32 * 128 hdim + 24 B T hdim + 8 * 128 P + 512 B
- *   bytes, P the number of weight and bias elements of the preprocessing Linear and the convolutions.
- *   wekws_mdtc_head_backward_launches(m) = 4 + 4 L launches.
- * The size and launch queries return a negative status (0 for the counts) for a model they do not accept.        */
-WEKWS_API int wekws_mdtc_head_num_params(const wekws_model* m);
-WEKWS_API int64_t wekws_mdtc_head_train_saved_floats(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int64_t wekws_mdtc_head_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save);
-WEKWS_API int wekws_mdtc_head_train_forward_launches(const wekws_model* m);
-WEKWS_API int wekws_mdtc_head_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params,
-                                            int n, const float* d_cmvn_mean, const float* d_cmvn_istd,
-                                            float* const* h_running, const double* h_bn, uint64_t seed, double p,
-                                            float* d_out, float* d_out_cache, float* d_saved, int save,
-                                            void* d_workspace, int64_t B, int64_t T, void* stream);
-WEKWS_API int64_t wekws_mdtc_head_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T);
-WEKWS_API int wekws_mdtc_head_backward_launches(const wekws_model* m);
-WEKWS_API int wekws_mdtc_head_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                       const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
-                                       const float* d_grad_out, uint64_t seed, double p, int64_t B, int64_t T,
-                                       float* const* h_grads, void* d_workspace, void* stream);
 
 /* Resampling: torchaudio.transforms.Resample(orig_freq, new_freq) with sinc_interp_hann (the resampling of
  * wekws/dataset/processor.py resample() and tools/compute_cmvn_stats.py:50-53), for B waveforms of their own lengths.

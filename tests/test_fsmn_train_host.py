@@ -95,7 +95,7 @@ def native_model(cfg):
 
 
 @pytest.mark.parametrize("case", list(FSMN_CASES) + ["shipped"])
-def test_saved_floats_and_workspace_formulas(case):
+def test_training_saved_floats_and_workspace_formulas(case):
     cfg = model_config("fsmn", input_dim=400, output_dim=2599) if case == "shipped" else fsmn_config(case)
     model, h = native_model(cfg)
     try:
@@ -104,13 +104,13 @@ def test_saved_floats_and_workspace_formulas(case):
         L, P, D = bb.fsmn_layers, bb.proj_dim, bb.linear_dim
         per_frame = bb.input_affine_dim + D + L * (2 * P + D) + bb.output_affine_dim
         assert fsmn_train.saved_floats_per_frame(bb) == per_frame
-        assert lib.wekws_fsmn_num_params(h) == 8 + 5 * L == len(list(model.parameters()))
-        assert lib.wekws_fsmn_backward_launches(h) == 8 + 5 * L
+        assert lib.wekws_train_num_params(h) == 8 + 5 * L == len(list(model.parameters()))
+        assert lib.wekws_train_backward_launches(h) == 8 + 5 * L
         numel = sum(p.numel() for p in model.parameters())
         width = max(bb.input_affine_dim, D, P, bb.output_affine_dim)
         for B, T in ((1, 1), (13, 5), (256, 200)):
-            assert lib.wekws_fsmn_train_saved_floats(h, B, T) == B * T * per_frame
-            assert lib.wekws_fsmn_backward_workspace_bytes(h, B, T) == 4 * (32 * numel + 2 * B * T * width)
+            assert lib.wekws_train_saved_floats(h, B, T) == B * T * per_frame
+            assert lib.wekws_train_backward_workspace_bytes(h, B, T) == 4 * (32 * numel + 2 * B * T * width)
     finally:
         _native.lib().wekws_model_destroy(h)
 
@@ -122,20 +122,30 @@ def test_shipped_config_sizes():
     assert fsmn_train.saved_floats_per_frame(bb) == 140 + 250 + 4 * (2 * 128 + 250) + 140
 
 
-def test_native_refusals_without_a_device():
+def test_training_entry_point_refusals_without_a_device():
     lib = _native.lib()
     model, h = native_model(fsmn_config("fsmn"))
     try:
         ptrs = (C.c_void_p * 23)()
-        rc = lib.wekws_fsmn_load_params(h, ptrs, 23, None)            # not finalized
+        rc = lib.wekws_model_load_params(h, ptrs, 23, None)           # not finalized
         assert rc == -3 and "finalize" in _native.last_error()
+        # FSMN trains on its packed weights: the entry points that take the parameters with each call refuse it and
+        # name the right ones
+        assert lib.wekws_train_forward(h, None, None, 0, None, None, None, None, 0, None, 0, None, None, None, 1, None,
+                                       2, 3, None) < 0
+        assert "wekws_model_train_forward" in _native.last_error()
+        assert lib.wekws_train_backward(h, None, None, 0, None, None, None, None, None, 0, None, 0, 2, 3, None, None,
+                                        None) < 0
+        assert "wekws_model_backward" in _native.last_error()
+        assert lib.wekws_train_workspace_bytes(h, 2, 3, 1) < 0 and lib.wekws_train_forward_launches(h) == 0
     finally:
         lib.wekws_model_destroy(h)
     _, hm = native_model(model_config("mdtc"))
     try:
-        assert lib.wekws_fsmn_num_params(hm) == 0
-        assert lib.wekws_fsmn_train_saved_floats(hm, 2, 3) < 0 and "FSMN" in _native.last_error()
-        assert lib.wekws_fsmn_load_params(hm, None, 0, None) < 0 and "FSMN backbone only" in _native.last_error()
+        assert lib.wekws_train_num_params(hm) == 4 + 12 * 17                 # the MDTC model's own count
+        assert lib.wekws_model_load_params(hm, None, 0, None) < 0 and "wekws_train_forward" in _native.last_error()
+        assert lib.wekws_model_backward(hm, None, None, None, None, 2, 3, None, 0, None, None) < 0
+        assert "wekws_train_backward" in _native.last_error()
     finally:
         lib.wekws_model_destroy(hm)
 

@@ -82,7 +82,7 @@ def config_handle(model):
 
 
 @pytest.mark.parametrize("layers,idim,odim", [(1, 80, 1), (2, 40, 2), (4, 128, 37)])
-def test_size_and_launch_formulas(layers, idim, odim):
+def test_training_size_and_launch_formulas(layers, idim, odim):
     cfg = model_config("gru", input_dim=idim, output_dim=odim)
     cfg["backbone"]["num_layers"] = layers
     model = init_model(cfg)
@@ -91,21 +91,26 @@ def test_size_and_launch_formulas(layers, idim, odim):
     h = config_handle(model)
     lib = _native.lib()
     try:
-        assert lib.wekws_gru_num_params(h) == 4 + 4 * layers == len(list(model.parameters()))
-        assert lib.wekws_gru_backward_launches(h) == 5 + 4 * layers
+        assert lib.wekws_train_num_params(h) == 4 + 4 * layers == len(list(model.parameters()))
+        assert lib.wekws_train_backward_launches(h) == 5 + 4 * layers
         for B, T in ((0, 5), (1, 1), (3, 7), (256, 200)):
             M = B * T
-            assert lib.wekws_gru_train_saved_floats(h, B, T) == M * gru_train.saved_floats_per_frame(layers) \
+            assert lib.wekws_train_saved_floats(h, B, T) == M * gru_train.saved_floats_per_frame(layers) \
                 == (1 + 5 * layers) * M * H
-            assert lib.wekws_gru_backward_workspace_bytes(h, B, T) == 4 * (32 * P + M * (8 * H + odim))
+            assert lib.wekws_train_backward_workspace_bytes(h, B, T) == 4 * (32 * P + M * (8 * H + odim))
+        # GRU trains on its packed weights: the entry points that take the parameters with each call refuse it and
+        # name the right ones
+        assert lib.wekws_train_backward(h, None, None, 0, None, None, None, None, None, 0, None, 0, 2, 3, None, None,
+                                        None) < 0
+        assert "the GRU model trains on the packed weights" in _native.last_error()
+        assert "wekws_model_backward" in _native.last_error()
+        assert lib.wekws_train_forward_launches(h) == 0 and "wekws_model_train_forward" in _native.last_error()
     finally:
         lib.wekws_model_destroy(h)
-    # the other backbones have no GRU entry points
-    other = init_model(model_config("mdtc"))
-    h = config_handle(other)
+    # an MDTC handle: the same queries give the MDTC model's own numbers
+    h = config_handle(init_model(model_config("mdtc")))
     try:
-        assert lib.wekws_gru_num_params(h) == 0 and lib.wekws_gru_backward_launches(h) == 0
-        assert lib.wekws_gru_train_saved_floats(h, 1, 1) < 0
+        assert lib.wekws_train_num_params(h) == 4 + 12 * 17 and lib.wekws_train_backward_launches(h) == 3 + 4 * 17
     finally:
         lib.wekws_model_destroy(h)
 

@@ -130,7 +130,7 @@ def head_handle(model):
 
 
 @pytest.mark.parametrize("case,odim", [("mdtc_global", 11), ("mdtc_last", 36), ("mdtc_small_last", 4096)])
-def test_size_and_launch_formulas(case, odim):
+def test_training_size_and_launch_formulas(case, odim):
     cfg = head_config(case)
     cfg["output_dim"] = odim
     model = init_model(cfg)
@@ -139,50 +139,56 @@ def test_size_and_launch_formulas(case, odim):
     h = head_handle(model)
     lib = _native.lib()
     try:
-        assert lib.wekws_mdtc_head_num_params(h) == 6 + 12 * L == len(list(model.parameters()))
-        assert lib.wekws_mdtc_head_train_forward_launches(h) == mdtc_train.head_forward_launches(L) == 3 + 3 * L
-        assert lib.wekws_mdtc_head_backward_launches(h) == mdtc_train.head_backward_launches(L) == 4 + 4 * L
+        assert lib.wekws_train_num_params(h) == 6 + 12 * L == len(list(model.parameters()))
+        assert lib.wekws_train_forward_launches(h) == mdtc_train.head_forward_launches(L) == 3 + 3 * L
+        assert lib.wekws_train_backward_launches(h) == mdtc_train.head_backward_launches(L) == 4 + 4 * L
         sliced = Ch * idim + Ch + L * (Ch * K + Ch + 2 * (Ch * Ch + Ch))       # no classifier among the slice sums
         for B, T in ((1, 2), (3, 5), (100, 98), (256, 98)):
             M = B * T
-            assert lib.wekws_mdtc_head_train_saved_floats(h, B, T) == mdtc_train.head_saved_floats(L, Ch, B, T) \
+            assert lib.wekws_train_saved_floats(h, B, T) == mdtc_train.head_saved_floats(L, Ch, B, T) \
                 == 12 * L * Ch + M * Ch * (4 * L + 2) + B * (Ch + 64)
-            assert lib.wekws_mdtc_head_train_workspace_bytes(h, B, T, 1) == 48 * 128 * Ch
-            assert lib.wekws_mdtc_head_train_workspace_bytes(h, B, T, 0) == 48 * 128 * Ch + 24 * M * Ch
-            assert lib.wekws_mdtc_head_backward_workspace_bytes(h, B, T) == \
+            assert lib.wekws_train_workspace_bytes(h, B, T, 1) == 48 * 128 * Ch
+            assert lib.wekws_train_workspace_bytes(h, B, T, 0) == 48 * 128 * Ch + 24 * M * Ch
+            assert lib.wekws_train_backward_workspace_bytes(h, B, T) == \
                 32 * 128 * Ch + 24 * M * Ch + 8 * 128 * sliced + 512 * B
     finally:
         lib.wekws_model_destroy(h)
 
 
-def test_native_refusals_without_a_device():
+def test_training_entry_point_refusals_without_a_device():
     lib = _native.lib()
-    # a linear-classifier model: the head entry points refuse it
+    # the same entry points give a linear-classifier model its own numbers and a head model the head's
     h = head_handle(init_model(model_config("mdtc")))
     try:
-        assert lib.wekws_mdtc_head_num_params(h) == 0 and "global or last head" in _native.last_error()
-        assert lib.wekws_mdtc_head_backward_launches(h) == 0
-        assert lib.wekws_mdtc_head_train_saved_floats(h, 2, 3) < 0
+        assert lib.wekws_train_num_params(h) == 4 + 12 * 17
+        assert lib.wekws_train_backward_launches(h) == mdtc_train.backward_launches(17)
+        assert lib.wekws_train_saved_floats(h, 2, 3) == mdtc_train.saved_floats(17, 64, 2, 3)
     finally:
         lib.wekws_model_destroy(h)
-    # a head model: the per-frame entry points keep refusing it, the head ones take it
     model = init_model(head_config("mdtc_global"))
     h = head_handle(model)
+    p = lambda *ps: (C.c_double * len(ps))(*ps)
     try:
-        assert lib.wekws_mdtc_num_params(h) == 0 and "linear classifier" in _native.last_error()
-        assert lib.wekws_mdtc_head_num_params(h) == 6 + 12 * 17
-        assert lib.wekws_mdtc_head_train_forward(h, None, None, 0, None, None, None, None, 1, 0.5, None, None, None, 1,
-                                                 None, 1, 1, None) < 0
+        assert lib.wekws_train_num_params(h) == 6 + 12 * 17
+        assert lib.wekws_train_backward_launches(h) == mdtc_train.head_backward_launches(17)
+        assert lib.wekws_train_saved_floats(h, 2, 3) == mdtc_train.head_saved_floats(17, 64, 2, 3)
+        assert lib.wekws_train_forward(h, None, None, 0, None, None, None, None, 1, p(0.5), 1, None, None, None, 1,
+                                       None, 1, 1, None) < 0
         assert "B * T >= 2" in _native.last_error()
-        assert lib.wekws_mdtc_head_train_forward(h, None, None, 0, None, None, None, None, 1, 1.5, None, None, None, 1,
-                                                 None, 2, 3, None) < 0
+        assert lib.wekws_train_forward(h, None, None, 0, None, None, None, None, 1, p(1.5), 1, None, None, None, 1,
+                                       None, 2, 3, None) < 0
         assert "outside [0, 1]" in _native.last_error()
-        assert lib.wekws_mdtc_head_backward(h, None, None, 0, None, None, None, None, 1, 0.5, 2, 3, None, None,
-                                            None) < 0
+        assert lib.wekws_train_backward(h, None, None, 0, None, None, None, None, None, 1, p(0.5), 1, 2, 3, None, None,
+                                        None) < 0
         assert "expected 210 parameters" in _native.last_error()
+        # the head has one Dropout: n_p must be 1
+        for ps in ((), (0.5, 0.5)):
+            assert lib.wekws_train_forward(h, None, None, 0, None, None, None, None, 1, p(*ps), len(ps), None, None,
+                                           None, 1, None, 2, 3, None) < 0
+            assert f"n_p = {len(ps)}, but the MDTC (global / last head) model has 1 Dropout" in _native.last_error()
     finally:
         lib.wekws_model_destroy(h)
-    for name, cfg, what in (("tcn", model_config("tcn"), "MDTC model is required"),
+    for name, cfg, what in (("tcn", model_config("tcn"), "TCN model trains with the per-frame linear classifier"),
                             ("odim", dict(head_config("mdtc_global"), output_dim=4097), "output_dim 4097"),
                             ("sigmoid", None, "Identity activation")):
         m = init_model(cfg) if cfg is not None else init_model(head_config("mdtc_global"))
@@ -192,7 +198,7 @@ def test_native_refusals_without_a_device():
             m.activation = torch.nn.Sigmoid()
         h = head_handle(m)
         try:
-            assert lib.wekws_mdtc_head_num_params(h) == 0 and what in _native.last_error(), name
+            assert lib.wekws_train_num_params(h) == 0 and what in _native.last_error(), name
         finally:
             lib.wekws_model_destroy(h)
 

@@ -110,7 +110,7 @@ def config_handle(model):
 
 
 @pytest.mark.parametrize("name", ["mdtc", "mdtc_small"])
-def test_size_and_launch_formulas(name):
+def test_training_size_and_launch_formulas(name):
     model = init_model(model_config(name))
     bb = model.backbone
     L, Ch, K, idim, O = 1 + bb.num_stack * bb.stack_size, model.hdim, bb.kernel_size, model.idim, model.odim
@@ -118,47 +118,53 @@ def test_size_and_launch_formulas(name):
     h = config_handle(model)
     lib = _native.lib()
     try:
-        assert lib.wekws_mdtc_num_params(h) == 4 + 12 * L == len(list(model.parameters()))
-        assert lib.wekws_mdtc_train_forward_launches(h) == mdtc_train.forward_launches(L) == 2 + 3 * L
-        assert lib.wekws_mdtc_backward_launches(h) == mdtc_train.backward_launches(L) == 3 + 4 * L
+        assert lib.wekws_train_num_params(h) == 4 + 12 * L == len(list(model.parameters()))
+        assert lib.wekws_train_forward_launches(h) == mdtc_train.forward_launches(L) == 2 + 3 * L
+        assert lib.wekws_train_backward_launches(h) == mdtc_train.backward_launches(L) == 3 + 4 * L
         sliced = Ch * idim + Ch + L * (Ch * K + Ch + 2 * (Ch * Ch + Ch)) + O * Ch + O
         assert sliced == sum(p.numel() for n, p in model.named_parameters() if ".bn" not in n)
         for B, T in ((1, 2), (3, 5), (100, 200), (100, 1000)):
             M = B * T
-            assert lib.wekws_mdtc_train_saved_floats(h, B, T) == mdtc_train.saved_floats(L, Ch, B, T) \
+            assert lib.wekws_train_saved_floats(h, B, T) == mdtc_train.saved_floats(L, Ch, B, T) \
                 == 12 * L * Ch + M * Ch * (4 * L + 2)
-            assert lib.wekws_mdtc_train_workspace_bytes(h, B, T, 1) == 48 * 128 * Ch
-            assert lib.wekws_mdtc_train_workspace_bytes(h, B, T, 0) == 48 * 128 * Ch + 24 * M * Ch
-            assert lib.wekws_mdtc_backward_workspace_bytes(h, B, T) == 32 * 128 * Ch + 20 * M * Ch + 8 * 128 * sliced
+            assert lib.wekws_train_workspace_bytes(h, B, T, 1) == 48 * 128 * Ch
+            assert lib.wekws_train_workspace_bytes(h, B, T, 0) == 48 * 128 * Ch + 24 * M * Ch
+            assert lib.wekws_train_backward_workspace_bytes(h, B, T) == 32 * 128 * Ch + 20 * M * Ch + 8 * 128 * sliced
     finally:
         lib.wekws_model_destroy(h)
 
 
-def test_native_refusals_without_a_device():
+def test_training_entry_point_refusals_without_a_device():
     lib = _native.lib()
-    for name in ("tcn", "gru"):
-        h = config_handle(init_model(model_config(name)))
-        try:
-            assert lib.wekws_mdtc_num_params(h) == 0 and lib.wekws_mdtc_backward_launches(h) == 0
-            assert lib.wekws_mdtc_train_saved_floats(h, 2, 3) < 0 and "MDTC model is required" in _native.last_error()
-        finally:
-            lib.wekws_model_destroy(h)
-    model = init_model(model_config("mdtc"))
+    model = init_model(model_config("mdtc", activation="identity"))
     h = config_handle(model)
     try:
-        assert lib.wekws_mdtc_train_forward(h, None, None, 0, None, None, None, None, None, None, None, 1, None, 1, 1,
-                                            None) < 0
+        assert lib.wekws_train_forward(h, None, None, 0, None, None, None, None, 0, None, 0, None, None, None, 1, None,
+                                       1, 1, None) < 0
         assert "B * T >= 2" in _native.last_error()
+        # MDTC has no Dropout: n_p must be 0
+        p = (C.c_double * 1)(0.1)
+        assert lib.wekws_train_forward(h, None, None, 0, None, None, None, None, 7, p, 1, None, None, None, 1, None,
+                                       2, 3, None) < 0
+        assert "n_p = 1, but the MDTC model has 0 Dropout probabilities" in _native.last_error()
+        assert lib.wekws_train_backward(h, None, None, 0, None, None, None, None, None, 7, p, 1, 2, 3, None, None,
+                                        None) < 0
+        assert "n_p = 1, but the MDTC model has 0 Dropout probabilities" in _native.last_error()
+        # its parameters travel with each call: the packed-handle entry points refuse it and name the right ones
+        assert lib.wekws_model_load_params(h, None, 0, None) < 0 and "wekws_train_forward" in _native.last_error()
+        assert lib.wekws_model_train_forward(h, None, None, None, None, 2, 3, None) < 0
+        assert "wekws_train_forward" in _native.last_error()
+        # the same entry points take the head model, with the head's numbers
         _native.invoke("wekws_model_set_head", h, _native.HEAD_GLOBAL)
-        assert lib.wekws_mdtc_num_params(h) == 0
-        assert lib.wekws_mdtc_backward_workspace_bytes(h, 2, 3) < 0 and "linear classifier" in _native.last_error()
+        assert lib.wekws_train_num_params(h) == 6 + 12 * 17
+        assert lib.wekws_train_backward_launches(h) == mdtc_train.head_backward_launches(17) == 4 + 4 * 17
     finally:
         lib.wekws_model_destroy(h)
     big = init_model(model_config("mdtc"))
     big.hdim = 128
     h = config_handle(big)
     try:
-        assert lib.wekws_mdtc_num_params(h) == 0 and "hidden_dim 128" in _native.last_error()
+        assert lib.wekws_train_num_params(h) == 0 and "hidden_dim 128" in _native.last_error()
     finally:
         lib.wekws_model_destroy(h)
 

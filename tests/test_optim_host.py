@@ -134,9 +134,9 @@ def test_host_scalars_are_torch_bit_for_bit():
         assert got[0].hex() == ss.hex() and got[1].hex() == bc.hex(), (lr, b1, b2, step, got, ss, bc)
 
 
-def test_abi_version_and_symbols():
+def test_abi_version_and_optimiser_symbols():
     lib = _native.lib()
-    assert lib.wekws_abi_version() == _native.ABI_VERSION == 18
+    assert lib.wekws_abi_version() == _native.ABI_VERSION == 19
     for name in ("wekws_grad_clip_workspace_bytes", "wekws_grad_clip_launches", "wekws_grad_clip",
                  "wekws_adam_step_launches", "wekws_adam_step"):
         assert name in _native.SIGNATURES and getattr(lib, name) is not None

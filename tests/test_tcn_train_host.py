@@ -17,7 +17,7 @@ import torch
 
 from oracle import kws_tcn_train_oracle as KT
 from tests.test_mdtc_train_host import assert_digest, assert_within_rule
-from wekws_b200 import _native, init_model, model_config, synth, tcn_train
+from wekws_b200 import _native, init_model, mdtc_train, model_config, synth, tcn_train
 from wekws_b200.frontend import draw_seed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -106,26 +106,26 @@ def wg_splits(N, Qp, M):
 
 
 @pytest.mark.parametrize("name,kw", CASES)
-def test_size_and_launch_formulas(name, kw):
+def test_training_size_and_launch_formulas(name, kw):
     model = init_model(model_config(name, **kw))
     bb = model.backbone
     L, Ch, K, idim, O, ds = bb.num_layers, model.hdim, bb.kernel_size, model.idim, model.odim, bb.ds
     h = config_handle(model)
     lib = _native.lib()
     try:
-        assert lib.wekws_tcn_num_params(h) == 4 + (8 if ds else 4) * L == len(list(model.parameters()))
-        assert lib.wekws_tcn_train_forward_launches(h) == tcn_train.forward_launches(L, ds) == 2 + (2 if ds else 1) * L
-        assert lib.wekws_tcn_backward_launches(h) == tcn_train.backward_launches(L, ds) == 4 + (3 if ds else 2) * L
+        assert lib.wekws_train_num_params(h) == 4 + (8 if ds else 4) * L == len(list(model.parameters()))
+        assert lib.wekws_train_forward_launches(h) == tcn_train.forward_launches(L, ds) == 2 + (2 if ds else 1) * L
+        assert lib.wekws_train_backward_launches(h) == tcn_train.backward_launches(L, ds) == 4 + (3 if ds else 2) * L
         for B, T in ((1, 2), (3, 5), (256, 200)):
             M = B * T
             nbn = (2 if ds else 1) * L
-            assert lib.wekws_tcn_train_saved_floats(h, B, T) == tcn_train.saved_floats(L, Ch, ds, B, T) \
+            assert lib.wekws_train_saved_floats(h, B, T) == tcn_train.saved_floats(L, Ch, ds, B, T) \
                 == 4 * nbn * Ch + M * Ch * (1 + L * (3 if ds else 2))
-            assert lib.wekws_tcn_train_workspace_bytes(h, B, T, 1) == 32 * 128 * Ch
-            assert lib.wekws_tcn_train_workspace_bytes(h, B, T, 0) == 32 * 128 * Ch + 16 * M * Ch
+            assert lib.wekws_train_workspace_bytes(h, B, T, 1) == 32 * 128 * Ch
+            assert lib.wekws_train_workspace_bytes(h, B, T, 0) == 32 * 128 * Ch + 16 * M * Ch
             jobs = [(Ch, idim + 1), (O, Ch + 1)] + [(Ch, Ch + 1) if ds else (Ch, K * Ch + 1)] * L
             part = sum(wg_splits(n, q, M) * n * q for n, q in jobs) + (128 * Ch * (K + 1) * L if ds else 0)
-            assert lib.wekws_tcn_backward_workspace_bytes(h, B, T) == 32 * 128 * Ch + 16 * M * Ch + 8 * part
+            assert lib.wekws_train_backward_workspace_bytes(h, B, T) == 32 * 128 * Ch + 16 * M * Ch + 8 * part
     finally:
         lib.wekws_model_destroy(h)
 
@@ -166,7 +166,7 @@ def test_opt_in():
         init_model(cfg).enable_training(device_dropout=True)
 
 
-def test_limits_and_refusals_without_a_device():
+def test_training_limits_and_refusals_without_a_device():
     for kw, what in ((dict(output_dim=4097), "output_dim <= 4096"), (dict(input_dim=129), "input_dim <= 128")):
         with pytest.raises(NotImplementedError, match=re.escape(what)):
             init_model(model_config("ds_tcn", **kw)).enable_training(device_dropout=True)
@@ -177,12 +177,28 @@ def test_limits_and_refusals_without_a_device():
     lib = _native.lib()
     h = config_handle(init_model(model_config("tcn", output_dim=4097)))
     try:
-        assert lib.wekws_tcn_num_params(h) == 0 and "output_dim <= 4096" in _native.last_error()
+        assert lib.wekws_train_num_params(h) == 0 and "output_dim <= 4096" in _native.last_error()
+    finally:
+        lib.wekws_model_destroy(h)
+    tcn = init_model(model_config("tcn"))
+    L = tcn.backbone.num_layers
+    h = config_handle(tcn)
+    try:
+        assert lib.wekws_train_backward_launches(h) == tcn_train.backward_launches(L, False)
+        # one Dropout probability per block: n_p must be L
+        for n_p in (0, L - 1, L + 1):
+            ps = (C.c_double * n_p)(*[0.1] * n_p)
+            assert lib.wekws_train_forward(h, None, None, 0, None, None, None, None, 1, ps, n_p, None, None, None, 1,
+                                           None, 2, 3, None) < 0
+            assert f"n_p = {n_p}, but the TCN / DS-TCN model has {L} Dropout" in _native.last_error()
+            assert lib.wekws_train_backward(h, None, None, 0, None, None, None, None, None, 1, ps, n_p, 2, 3, None,
+                                            None, None) < 0
+            assert f"n_p = {n_p}, but the TCN / DS-TCN model has {L} Dropout" in _native.last_error()
     finally:
         lib.wekws_model_destroy(h)
     h = config_handle(init_model(model_config("mdtc")))
     try:
-        assert lib.wekws_tcn_backward_launches(h) == 0 and "TCN or DS-TCN model is required" in _native.last_error()
+        assert lib.wekws_train_backward_launches(h) == mdtc_train.backward_launches(17)
     finally:
         lib.wekws_model_destroy(h)
     model = init_model(model_config("ds_tcn")).enable_training(device_dropout=True).train()

@@ -23,7 +23,7 @@ ACT_IDENTITY, ACT_SIGMOID = 0, 1
 PCM_S16, PCM_F32 = 0, 1
 HEAD_LINEAR, HEAD_GLOBAL, HEAD_LAST = 0, 1, 2
 FWD_SOFTMAX = 1
-ABI_VERSION = 18
+ABI_VERSION = 19
 
 # limits (include/wekws_b200.h #defines)
 CTC_MAX_PREFIX, CTC_MAX_PATH_BEAM, CTC_MAX_SCORE_BEAM = 64, 20, 3
@@ -140,60 +140,23 @@ SIGNATURES = {
     "wekws_criterion_ctc_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
                                                C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wekws_fsmn_num_params": (C.c_int, [C.c_void_p]),
-    "wekws_fsmn_load_params": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
-    "wekws_fsmn_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_fsmn_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
-                                           C.c_int64, C.c_void_p]),
-    "wekws_fsmn_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_fsmn_backward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_fsmn_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
-                                      C.c_int, C.c_void_p, C.c_void_p]),
-    "wekws_gru_num_params": (C.c_int, [C.c_void_p]),
-    "wekws_gru_load_params": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
-    "wekws_gru_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_gru_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
-                                          C.c_int64, C.c_void_p]),
-    "wekws_gru_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_gru_backward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_gru_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
-                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "wekws_mdtc_num_params": (C.c_int, [C.c_void_p]),
-    "wekws_mdtc_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_mdtc_train_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64, C.c_int]),
-    "wekws_mdtc_train_forward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_mdtc_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                           C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
-    "wekws_mdtc_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_mdtc_backward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_mdtc_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                      C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wekws_mdtc_head_num_params": (C.c_int, [C.c_void_p]),
-    "wekws_mdtc_head_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_mdtc_head_train_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64, C.c_int]),
-    "wekws_mdtc_head_train_forward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_mdtc_head_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                                C.c_void_p, C.c_void_p, C.c_uint64, C.c_double, C.c_void_p,
-                                                C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64,
-                                                C.c_void_p]),
-    "wekws_mdtc_head_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_mdtc_head_backward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_mdtc_head_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_void_p, C.c_uint64, C.c_double, C.c_int64, C.c_int64,
-                                           C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wekws_tcn_num_params": (C.c_int, [C.c_void_p]),
-    "wekws_tcn_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_tcn_train_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64, C.c_int]),
-    "wekws_tcn_train_forward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_tcn_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                          C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                          C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
-    "wekws_tcn_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
-    "wekws_tcn_backward_launches": (C.c_int, [C.c_void_p]),
-    "wekws_tcn_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                     C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
-                                     C.c_void_p, C.c_void_p]),
+    "wekws_train_num_params": (C.c_int, [C.c_void_p]),
+    "wekws_train_saved_floats": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
+    "wekws_train_backward_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64]),
+    "wekws_train_backward_launches": (C.c_int, [C.c_void_p]),
+    "wekws_train_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int64, C.c_int]),
+    "wekws_train_forward_launches": (C.c_int, [C.c_void_p]),
+    "wekws_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_uint64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    "wekws_train_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int, C.c_int64, C.c_int64,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_model_load_params": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "wekws_model_train_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                            C.c_int64, C.c_void_p]),
+    "wekws_model_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                       C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wekws_dropout_mask": (C.c_int, [C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_uint32, C.c_void_p,
                                      C.c_void_p]),
     "wekws_pipeline_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64,

@@ -855,237 +855,36 @@ extern "C" int wekws_model_forward(wekws_model* m, const float* d_feats, const f
   return WEKWS_OK;
 }
 
-// ------------------------------------------------------------------------------- FSMN training
+// ------------------------------------------------------------------------------- training
 namespace {
 
-// the layer widths of an FSMN model's config (the fields the saved-activation and workspace sizes depend on)
-FsmnArgs fsmn_dims(const wekws_model_config& c) {
-  FsmnArgs a{};
-  a.idim = c.idim; a.aff_in = c.fsmn_input_affine_dim; a.lin = c.fsmn_linear_dim; a.proj = c.fsmn_proj_dim;
-  a.aff_out = c.fsmn_output_affine_dim; a.odim = c.odim; a.L = c.num_layers;
-  a.lorder = c.fsmn_left_order; a.rorder = c.fsmn_right_order;
-  return a;
-}
+// The models that train on the device.  The BatchNorm models (MDTC, MDTC with a head, TCN / DS-TCN) take their
+// parameters with every call on a config-only handle; FSMN and GRU train on the packed weights of a finalized handle.
+enum class TrainFamily { Mdtc, MdtcHead, Tcn, Fsmn, Gru };
 
-int fsmn_train_check(const wekws_model* m, const char* what) {
-  WEKWS_REQUIRE(m, "%s: null handle", what);
-  WEKWS_REQUIRE(m->cfg.backbone == WEKWS_BACKBONE_FSMN, "%s: training is implemented for the FSMN backbone only", what);
-  if (!m->finalized) { set_error("%s called before wekws_model_finalize", what); return WEKWS_ERR_STATE; }
-  WEKWS_REQUIRE(m->cfg.activation == WEKWS_ACT_IDENTITY, "%s: the FSMN model trains with the identity activation", what);
-  int dev = 0;
-  WEKWS_CUDA_OK(cudaGetDevice(&dev));
-  WEKWS_REQUIRE(dev == m->device, "model was finalized on device %d but current device is %d", m->device, dev);
-  return WEKWS_OK;
-}
-
-}  // namespace
-
-extern "C" int wekws_fsmn_num_params(const wekws_model* m) {
-  if (!m || m->cfg.backbone != WEKWS_BACKBONE_FSMN) return 0;
-  return 8 + 5 * m->cfg.num_layers;
-}
-
-extern "C" int wekws_fsmn_load_params(wekws_model* m, const float* const* h_params, int n, void* stream) {
-  int rc = fsmn_train_check(m, "wekws_fsmn_load_params");
-  if (rc) return rc;
-  const FsmnArgs& a = m->fsmn;
-  WEKWS_REQUIRE(h_params && n == 8 + 5 * a.L, "wekws_fsmn_load_params: expected the %d parameters of a %d-layer FSMN, got %d",
-                8 + 5 * a.L, a.L, n);
-  FsmnPackArgs p{};
-  p.packed = m->d_vec;
-  p.n = n;
-  int k = 0;                                   // the parameters in state_dict order, each into its place in the pack
-  auto put = [&](int rows, int cols, long long dst, int ld) {
-    FsmnParamCopy& c = p.p[k];
-    c.src = h_params[k]; c.dst = dst; c.rows = rows; c.cols = cols; c.ld = ld;
-    ++k;
-  };
-  const int D = a.lin, P = a.proj;
-  put(a.aff_in, a.idim, a.o_w_in1, a.np_aff_in); put(a.aff_in, 1, a.o_b_in1, 1);
-  put(D, a.aff_in, a.o_w_in2, a.np_lin); put(D, 1, a.o_b_in2, 1);
-  for (int l = 0; l < a.L; ++l) {
-    const long long base = a.o_layers + (long long)l * a.layer_stride;
-    put(P, D, base + a.lo_wp, a.np_proj);
-    put(P, a.lorder, base + a.lo_taps, P);
-    put(P, a.rorder, base + a.lo_taps + (long long)a.lorder * P, P);
-    put(D, P, base + a.lo_wa, a.np_lin); put(D, 1, base + a.lo_ba, 1);
+const char* train_label(TrainFamily f) {
+  switch (f) {
+    case TrainFamily::Mdtc: return "MDTC";
+    case TrainFamily::MdtcHead: return "MDTC (global / last head)";
+    case TrainFamily::Tcn: return "TCN / DS-TCN";
+    case TrainFamily::Fsmn: return "FSMN";
+    default: return "GRU";
   }
-  put(a.aff_out, D, a.o_w_out1, a.np_aff_out); put(a.aff_out, 1, a.o_b_out1, 1);
-  put(a.odim, a.aff_out, a.o_w_out2, a.np_odim); put(a.odim, 1, a.o_b_out2, 1);
-  for (int i = 0; i < p.n; ++i)
-    WEKWS_REQUIRE(p.p[i].src != nullptr, "wekws_fsmn_load_params: parameter %d is null", i);
-  return fsmn_pack_launch(p, (cudaStream_t)stream);
 }
 
-extern "C" int64_t wekws_fsmn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
-  WEKWS_REQUIRE(m && m->cfg.backbone == WEKWS_BACKBONE_FSMN && B >= 0 && T >= 0,
-                "wekws_fsmn_train_saved_floats: an FSMN model and B, T >= 0 are required");
-  return B * T * fsmn_saved_per_frame(fsmn_dims(m->cfg));
-}
-
-extern "C" int64_t wekws_fsmn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
-  WEKWS_REQUIRE(m && m->cfg.backbone == WEKWS_BACKBONE_FSMN && B >= 0 && T >= 0,
-                "wekws_fsmn_backward_workspace_bytes: an FSMN model and B, T >= 0 are required");
-  return (int64_t)sizeof(float) * fsmn_backward_workspace_floats(fsmn_dims(m->cfg), B * T);
-}
-
-extern "C" int wekws_fsmn_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
-                                        float* d_saved, int64_t B, int64_t T, void* stream) {
-  int rc = fsmn_train_check(m, "wekws_fsmn_train_forward");
-  if (rc) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_fsmn_train_forward: bad B/T");
-  WEKWS_REQUIRE(d_feats && d_out && d_out_cache && d_saved, "wekws_fsmn_train_forward: null tensor");
-  cudaStream_t st = (cudaStream_t)stream;
-  // the time chunks of wekws_model_forward, each launch also storing its frames' activations
-  const int maxT = fsmn_tile_rows();
-  const int nchunk = (int)((T + maxT - 1) / maxT);
-  const int Tc = (int)((T + nchunk - 1) / nchunk);
-  for (int64_t t0 = 0; t0 < T; t0 += Tc) {
-    FsmnArgs a = m->fsmn;
-    a.feats = d_feats + t0 * m->cfg.idim;
-    a.out = d_out + t0 * m->cfg.odim;
-    a.in_cache = t0 == 0 ? nullptr : d_out_cache;
-    a.out_cache = d_out_cache;
-    a.B = (int)B;
-    a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
-    a.feat_bstride = T * m->cfg.idim;
-    a.out_bstride = T * m->cfg.odim;
-    a.saved = d_saved; a.save_T = (int)T; a.save_t0 = (int)t0;
-    if ((rc = fsmn_train_launch(a, st))) return rc;
-  }
-  return WEKWS_OK;
-}
-
-extern "C" int wekws_fsmn_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_grad_out,
-                                   int64_t B, int64_t T, float* const* h_grads, int n, void* d_workspace, void* stream) {
-  int rc = fsmn_train_check(m, "wekws_fsmn_backward");
-  if (rc) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_fsmn_backward: bad B/T");
-  WEKWS_REQUIRE(d_feats && d_saved && d_grad_out && d_workspace && h_grads, "wekws_fsmn_backward: null argument");
-  WEKWS_REQUIRE(n == 8 + 5 * m->fsmn.L, "wekws_fsmn_backward: expected %d gradient buffers, got %d", 8 + 5 * m->fsmn.L, n);
-  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_grads[i] != nullptr, "wekws_fsmn_backward: gradient buffer %d is null", i);
-  return fsmn_backward_launch(m->fsmn, d_feats, d_saved, d_grad_out, (int)B, (int)T, h_grads, (float*)d_workspace,
-                              (cudaStream_t)stream);
-}
-
-extern "C" int wekws_fsmn_backward_launches(const wekws_model* m) {
-  return m && m->cfg.backbone == WEKWS_BACKBONE_FSMN ? fsmn_backward_launches(m->cfg.num_layers) : 0;
-}
-
-// ------------------------------------------------------------------------------- GRU training
-namespace {
-
-bool is_gru(const wekws_model* m) { return m && m->cfg.backbone == WEKWS_BACKBONE_GRU; }
-
-// the dimensions of a GRU model's config (the fields the saved-activation and workspace sizes depend on)
-GruArgs gru_dims(const wekws_model_config& c) {
-  GruArgs a{};
-  a.L = c.num_layers; a.H = c.hdim; a.idim = c.idim; a.odim = c.odim;
-  return a;
-}
-
-int gru_train_check(const wekws_model* m, const char* what) {
-  WEKWS_REQUIRE(m, "%s: null handle", what);
-  WEKWS_REQUIRE(is_gru(m), "%s: a GRU model is required", what);
-  if (!m->finalized) { set_error("%s called before wekws_model_finalize", what); return WEKWS_ERR_STATE; }
-  int dev = 0;
-  WEKWS_CUDA_OK(cudaGetDevice(&dev));
-  WEKWS_REQUIRE(dev == m->device, "model was finalized on device %d but current device is %d", m->device, dev);
-  return WEKWS_OK;
-}
-
-}  // namespace
-
-extern "C" int wekws_gru_num_params(const wekws_model* m) {
-  return is_gru(m) ? gru_num_params(m->cfg.num_layers) : 0;
-}
-
-extern "C" int wekws_gru_load_params(wekws_model* m, const float* const* h_params, int n, void* stream) {
-  int rc = gru_train_check(m, "wekws_gru_load_params");
-  if (rc) return rc;
-  const GruArgs& a = m->gru;
-  const int H = a.H, G = 3 * H;
-  WEKWS_REQUIRE(h_params && n == gru_num_params(a.L), "wekws_gru_load_params: expected the %d parameters of a "
-                "%d-layer GRU model, got %d", gru_num_params(a.L), a.L, n);
-  FsmnPackArgs p{};
-  p.packed = m->d_vec;
-  p.n = n;
-  int k = 0;                                   // each parameter [rows][cols] into its place in pack_gru's layout
-  auto put = [&](int rows, int cols, long long dst, int ld) {
-    FsmnParamCopy& c = p.p[k];
-    c.src = h_params[k]; c.dst = dst; c.rows = rows; c.cols = cols; c.ld = ld;
-    ++k;
-  };
-  put(H, a.idim, a.v_wp, H); put(H, 1, a.v_bp, 1);
-  for (int l = 0; l < a.L; ++l) {
-    const long long base = a.v_layers + (long long)l * a.v_layer_stride;
-    put(G, H, base, 2 * G); put(G, H, base + G, 2 * G);
-    put(G, 1, base + 2LL * H * G, 1); put(G, 1, base + 2LL * H * G + G, 1);
-  }
-  put(a.odim, H, a.v_wc, a.odim); put(a.odim, 1, a.v_bc, 1);
-  for (int i = 0; i < p.n; ++i)
-    WEKWS_REQUIRE(p.p[i].src != nullptr, "wekws_gru_load_params: parameter %d is null", i);
-  return fsmn_pack_launch(p, (cudaStream_t)stream);
-}
-
-extern "C" int64_t wekws_gru_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
-  WEKWS_REQUIRE(is_gru(m) && B >= 0 && T >= 0, "wekws_gru_train_saved_floats: a GRU model and B, T >= 0 are required");
-  return B * T * gru_saved_per_frame(m->cfg.num_layers, m->cfg.hdim);
-}
-
-extern "C" int64_t wekws_gru_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
-  WEKWS_REQUIRE(is_gru(m) && B >= 0 && T >= 0,
-                "wekws_gru_backward_workspace_bytes: a GRU model and B, T >= 0 are required");
-  return (int64_t)sizeof(float) * gru_backward_workspace_floats(gru_dims(m->cfg), B * T);
-}
-
-extern "C" int wekws_gru_backward_launches(const wekws_model* m) {
-  return is_gru(m) ? gru_backward_launches(m->cfg.num_layers) : 0;
-}
-
-extern "C" int wekws_gru_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
-                                       float* d_saved, int64_t B, int64_t T, void* stream) {
-  int rc = gru_train_check(m, "wekws_gru_train_forward");
-  if (rc) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_gru_train_forward: bad B/T");
-  WEKWS_REQUIRE(d_feats && d_out && d_out_cache && d_saved, "wekws_gru_train_forward: null tensor");
-  GruArgs a = m->gru;                          // the FP32 kernel whatever the precision mode
-  a.feats = d_feats; a.in_cache = nullptr; a.out = d_out; a.out_cache = d_out_cache;
-  a.B = (int)B; a.T = (int)T; a.saved = d_saved;
-  return gru_launch(a, (cudaStream_t)stream, true);
-}
-
-extern "C" int wekws_gru_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_out,
-                                  const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads, int n,
-                                  void* d_workspace, void* stream) {
-  int rc = gru_train_check(m, "wekws_gru_backward");
-  if (rc) return rc;
-  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "wekws_gru_backward: bad B/T");
-  WEKWS_REQUIRE(d_feats && d_saved && d_out && d_grad_out && d_workspace && h_grads,
-                "wekws_gru_backward: null argument");
-  const int np = gru_num_params(m->gru.L);
-  WEKWS_REQUIRE(n == np, "wekws_gru_backward: expected %d gradient buffers, got %d", np, n);
-  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_grads[i] != nullptr, "wekws_gru_backward: gradient buffer %d is null", i);
-  return gru_backward_launch(m->gru, d_feats, d_saved, d_out, d_grad_out, (int)B, (int)T, h_grads,
-                             (float*)d_workspace, (cudaStream_t)stream);
-}
-
-// ------------------------------------------------------------------------------- MDTC training
-namespace {
+// A trainable model resolved from its handle: its family, the dimensions its kernels take, its parameter count
+struct TrainModel {
+  TrainFamily fam;
+  MdtcTrainDims mdtc;                  // Mdtc, MdtcHead (odim 0: the backbone alone)
+  TcnTrainDims tcn;                    // Tcn
+  int n_params;                        // parameter and gradient pointers per call
+};
 
 // the dimensions of an MDTC model with the per-frame linear classifier (head == false) or with the global / last head
 // (head == true: odim 0, the backbone alone), as the training kernels take them
 int mdtc_dims(const wekws_model* m, const char* what, bool head, MdtcTrainDims* d) {
-  WEKWS_REQUIRE(m, "%s: null handle", what);
   const wekws_model_config& c = m->cfg;
-  WEKWS_REQUIRE(c.backbone == WEKWS_BACKBONE_MDTC, "%s: an MDTC model is required", what);
-  if (!head) {
-    WEKWS_REQUIRE(m->head == WEKWS_HEAD_LINEAR, "%s: the MDTC model trains with the per-frame linear classifier", what);
-  } else {
-    WEKWS_REQUIRE(m->head != WEKWS_HEAD_LINEAR, "%s: a model with the global or last head is required (the per-frame "
-                  "linear classifier trains through wekws_mdtc_train_forward)", what);
-    WEKWS_REQUIRE(c.activation == WEKWS_ACT_IDENTITY, "%s: the head trains with the Identity activation", what);
-  }
+  if (head) WEKWS_REQUIRE(c.activation == WEKWS_ACT_IDENTITY, "%s: the head trains with the Identity activation", what);
   WEKWS_REQUIRE(c.hdim == 32 || c.hdim == 64, "%s: hidden_dim %d unsupported in training (32 or 64)", what, c.hdim);
   WEKWS_REQUIRE(c.kernel_size >= 2 && c.kernel_size <= MDTC_TRAIN_MAX_K, "%s: kernel_size %d unsupported (2..%d)", what,
                 c.kernel_size, MDTC_TRAIN_MAX_K);
@@ -1113,22 +912,131 @@ int mdtc_dims(const wekws_model* m, const char* what, bool head, MdtcTrainDims* 
   return WEKWS_OK;
 }
 
-int mdtc_train_dims(const wekws_model* m, const char* what, MdtcTrainDims* d) { return mdtc_dims(m, what, false, d); }
-
-// the head of one call: theta = ceil(p 2^24) in double, scale = 1 / (float)(1 - p), torch's scale
-int mdtc_head(const wekws_model* m, uint64_t seed, double p, const char* what, MdtcHead* h) {
-  WEKWS_REQUIRE(p >= 0.0 && p <= 1.0, "%s: dropout probability %g is outside [0, 1]", what, p);
-  memset(h, 0, sizeof(*h));
-  h->last = m->head == WEKWS_HEAD_LAST ? 1 : 0;
-  h->odim = m->cfg.odim;
-  h->seed = seed;
-  h->theta = (uint32_t)ceil(p * 16777216.0);
-  h->scale = 1.0f / (float)(1.0 - p);
+// the dimensions of a TCN / DS-TCN model with the per-frame linear classifier, as the training kernels take them
+int tcn_train_dims(const wekws_model* m, const char* what, TcnTrainDims* d) {
+  const wekws_model_config& c = m->cfg;
+  WEKWS_REQUIRE((c.hdim == 64 || c.hdim == 256) && c.kernel_size >= 2 && c.kernel_size <= TCN_TRAIN_MAX_K &&
+                    c.num_layers >= 1 && c.num_layers <= TCN_TRAIN_MAX_LAYERS && c.idim >= 1 &&
+                    c.idim <= TCN_TRAIN_MAX_IDIM && c.odim >= 1 && c.odim <= TCN_TRAIN_MAX_ODIM,
+                "%s: TCN training supports hidden_dim 64 or 256, kernel_size 2..%d, 1..%d layers, input_dim <= %d and "
+                "output_dim <= %d; got hidden %d, kernel %d, %d layers, input %d, output %d", what, TCN_TRAIN_MAX_K,
+                TCN_TRAIN_MAX_LAYERS, TCN_TRAIN_MAX_IDIM, TCN_TRAIN_MAX_ODIM, c.hdim, c.kernel_size, c.num_layers,
+                c.idim, c.odim);
+  memset(d, 0, sizeof(*d));
+  d->C = c.hdim; d->idim = c.idim; d->odim = c.odim; d->K = c.kernel_size; d->L = c.num_layers;
+  d->ds = c.backbone == WEKWS_BACKBONE_DSTCN ? 1 : 0;
+  d->act = c.activation == WEKWS_ACT_SIGMOID ? 1 : 0;
+  d->norm_var = c.norm_var;
+  d->pad_total = (c.kernel_size - 1) * ((1 << c.num_layers) - 1);
   return WEKWS_OK;
 }
 
-// The arguments of a batch-statistics training forward (MDTC, TCN / DS-TCN) of a model of width C and output width
-// odim with n_expected parameters and nbn BatchNorms.
+// the layer widths of an FSMN model's config (the fields the saved-activation and workspace sizes depend on)
+FsmnArgs fsmn_dims(const wekws_model_config& c) {
+  FsmnArgs a{};
+  a.idim = c.idim; a.aff_in = c.fsmn_input_affine_dim; a.lin = c.fsmn_linear_dim; a.proj = c.fsmn_proj_dim;
+  a.aff_out = c.fsmn_output_affine_dim; a.odim = c.odim; a.L = c.num_layers;
+  a.lorder = c.fsmn_left_order; a.rorder = c.fsmn_right_order;
+  return a;
+}
+
+// the dimensions of a GRU model's config (the fields the saved-activation and workspace sizes depend on)
+GruArgs gru_dims(const wekws_model_config& c) {
+  GruArgs a{};
+  a.L = c.num_layers; a.H = c.hdim; a.idim = c.idim; a.odim = c.odim;
+  return a;
+}
+
+// The family of a trainable model and what its calls need from the config; a TCN / DS-TCN with a head is refused.
+int train_model(const wekws_model* m, const char* what, TrainModel* t) {
+  WEKWS_REQUIRE(m, "%s: null handle", what);
+  const int L = m->cfg.num_layers;
+  int rc = WEKWS_OK;
+  switch (m->cfg.backbone) {
+    case WEKWS_BACKBONE_MDTC:
+      t->fam = m->head == WEKWS_HEAD_LINEAR ? TrainFamily::Mdtc : TrainFamily::MdtcHead;
+      if ((rc = mdtc_dims(m, what, t->fam == TrainFamily::MdtcHead, &t->mdtc))) return rc;
+      t->n_params =
+          t->fam == TrainFamily::Mdtc ? mdtc_train_num_params(t->mdtc.L) : mdtc_head_train_num_params(t->mdtc.L);
+      return WEKWS_OK;
+    case WEKWS_BACKBONE_TCN:
+    case WEKWS_BACKBONE_DSTCN:
+      WEKWS_REQUIRE(m->head == WEKWS_HEAD_LINEAR, "%s: the TCN model trains with the per-frame linear classifier",
+                    what);
+      t->fam = TrainFamily::Tcn;
+      if ((rc = tcn_train_dims(m, what, &t->tcn))) return rc;
+      t->n_params = tcn_train_num_params(t->tcn);
+      return WEKWS_OK;
+    case WEKWS_BACKBONE_FSMN:
+      t->fam = TrainFamily::Fsmn;
+      t->n_params = 8 + 5 * L;
+      return WEKWS_OK;
+    case WEKWS_BACKBONE_GRU:
+      t->fam = TrainFamily::Gru;
+      t->n_params = gru_num_params(L);
+      return WEKWS_OK;
+  }
+  set_error("%s: training is not implemented for backbone %d", what, m->cfg.backbone);
+  return WEKWS_ERR_INVALID;
+}
+
+bool batch_stats(TrainFamily f) { return f != TrainFamily::Fsmn && f != TrainFamily::Gru; }
+
+// A model for wekws_train_forward / _backward and their queries: the BatchNorm models only.
+int batch_stats_model(const wekws_model* m, const char* what, TrainModel* t) {
+  int rc = train_model(m, what, t);
+  if (rc) return rc;
+  WEKWS_REQUIRE(batch_stats(t->fam), "%s: the %s model trains on the packed weights of its finalized handle, through "
+                "wekws_model_load_params / wekws_model_train_forward / wekws_model_backward", what,
+                train_label(t->fam));
+  return WEKWS_OK;
+}
+
+// A model for wekws_model_load_params / _train_forward / _backward: FSMN or GRU, finalized on the current device.
+int packed_model(const wekws_model* m, const char* what, TrainModel* t) {
+  int rc = train_model(m, what, t);
+  if (rc) return rc;
+  WEKWS_REQUIRE(!batch_stats(t->fam), "%s: the %s model takes its parameters with each call, through "
+                "wekws_train_forward / wekws_train_backward", what, train_label(t->fam));
+  if (!m->finalized) { set_error("%s called before wekws_model_finalize", what); return WEKWS_ERR_STATE; }
+  WEKWS_REQUIRE(t->fam != TrainFamily::Fsmn || m->cfg.activation == WEKWS_ACT_IDENTITY,
+                "%s: the FSMN model trains with the identity activation", what);
+  int dev = 0;
+  WEKWS_CUDA_OK(cudaGetDevice(&dev));
+  WEKWS_REQUIRE(dev == m->device, "model was finalized on device %d but current device is %d", m->device, dev);
+  return WEKWS_OK;
+}
+
+// The model of a wekws_train_forward / _backward call and its Dropout: n_p probabilities (MDTC 0, MDTC with a head 1,
+// TCN / DS-TCN one per block), each as theta = ceil(p 2^24) in double and scale = 1 / (float)(1 - p), torch's scale.
+int batch_stats_call(const wekws_model* m, const char* what, uint64_t seed, const double* h_p, int n_p, TrainModel* t,
+                     MdtcHead* head, TcnDropout* drop) {
+  int rc = batch_stats_model(m, what, t);
+  if (rc) return rc;
+  const int n_drop = t->fam == TrainFamily::Mdtc ? 0 : t->fam == TrainFamily::MdtcHead ? 1 : t->tcn.L;
+  WEKWS_REQUIRE(n_p == n_drop, "%s: n_p = %d, but the %s model has %d Dropout probabilities", what, n_p,
+                train_label(t->fam), n_drop);
+  WEKWS_REQUIRE(n_p == 0 || h_p, "%s: null dropout probabilities", what);
+  memset(head, 0, sizeof(*head));
+  memset(drop, 0, sizeof(*drop));
+  head->last = m->head == WEKWS_HEAD_LAST ? 1 : 0;
+  head->odim = m->cfg.odim;
+  head->seed = drop->seed = seed;
+  uint32_t* theta = t->fam == TrainFamily::MdtcHead ? &head->theta : drop->theta;
+  float* scale = t->fam == TrainFamily::MdtcHead ? &head->scale : drop->scale;
+  for (int l = 0; l < n_p; ++l) {
+    WEKWS_REQUIRE(h_p[l] >= 0.0 && h_p[l] <= 1.0, "%s: dropout probability %g (number %d) is outside [0, 1]", what,
+                  h_p[l], l);
+    theta[l] = (uint32_t)ceil(h_p[l] * 16777216.0);
+    scale[l] = 1.0f / (float)(1.0 - h_p[l]);
+  }
+  return WEKWS_OK;
+}
+
+int num_batch_norms(const TrainModel& t) { return t.fam == TrainFamily::Tcn ? tcn_train_num_bns(t.tcn) : 3 * t.mdtc.L; }
+
+// The arguments of a batch-statistics training forward of a model of width C and output width odim with nbn
+// BatchNorms.
 int batch_stats_forward_check(const char* what, int64_t B, int64_t T, int C, int odim, int n, int n_expected, int nbn,
                               const float* d_feats, const float* const* h_params, const float* d_cmvn_mean,
                               const float* d_cmvn_istd, float* const* h_running, const double* h_bn,
@@ -1163,269 +1071,233 @@ int batch_stats_backward_check(const char* what, int64_t B, int64_t T, int C, in
 
 }  // namespace
 
-extern "C" int wekws_mdtc_num_params(const wekws_model* m) {
-  MdtcTrainDims d;
-  return mdtc_train_dims(m, "wekws_mdtc_num_params", &d) ? 0 : mdtc_train_num_params(d.L);
+extern "C" int wekws_train_num_params(const wekws_model* m) {
+  TrainModel t;
+  return train_model(m, "wekws_train_num_params", &t) ? 0 : t.n_params;
 }
 
-extern "C" int64_t wekws_mdtc_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
-  MdtcTrainDims d;
-  int rc = mdtc_train_dims(m, "wekws_mdtc_train_saved_floats", &d);
+extern "C" int64_t wekws_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
+  const char* what = "wekws_train_saved_floats";
+  TrainModel t;
+  int rc = train_model(m, what, &t);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_train_saved_floats: B, T >= 0 are required");
-  return mdtc_train_saved_floats(d, B * T);
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "%s: B, T >= 0 are required", what);
+  switch (t.fam) {
+    case TrainFamily::Mdtc: return mdtc_train_saved_floats(t.mdtc, B * T);
+    case TrainFamily::MdtcHead: return mdtc_head_train_saved_floats(t.mdtc, B, T);
+    case TrainFamily::Tcn: return tcn_train_saved_floats(t.tcn, B * T);
+    case TrainFamily::Fsmn: return B * T * fsmn_saved_per_frame(fsmn_dims(m->cfg));
+    default: return B * T * gru_saved_per_frame(m->cfg.num_layers, m->cfg.hdim);
+  }
 }
 
-extern "C" int64_t wekws_mdtc_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save) {
-  MdtcTrainDims d;
-  int rc = mdtc_train_dims(m, "wekws_mdtc_train_workspace_bytes", &d);
+extern "C" int64_t wekws_train_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
+  const char* what = "wekws_train_backward_workspace_bytes";
+  TrainModel t;
+  int rc = train_model(m, what, &t);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_train_workspace_bytes: B, T >= 0 are required");
-  return mdtc_train_workspace_bytes(d, B * T, save != 0);
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "%s: B, T >= 0 are required", what);
+  switch (t.fam) {
+    case TrainFamily::Mdtc: return mdtc_backward_workspace_bytes(t.mdtc, B * T);
+    case TrainFamily::MdtcHead: return mdtc_head_backward_workspace_bytes(t.mdtc, B, T);
+    case TrainFamily::Tcn: return tcn_backward_workspace_bytes(t.tcn, B * T);
+    case TrainFamily::Fsmn: return (int64_t)sizeof(float) * fsmn_backward_workspace_floats(fsmn_dims(m->cfg), B * T);
+    default: return (int64_t)sizeof(float) * gru_backward_workspace_floats(gru_dims(m->cfg), B * T);
+  }
 }
 
-extern "C" int64_t wekws_mdtc_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
-  MdtcTrainDims d;
-  int rc = mdtc_train_dims(m, "wekws_mdtc_backward_workspace_bytes", &d);
+extern "C" int wekws_train_backward_launches(const wekws_model* m) {
+  TrainModel t;
+  if (train_model(m, "wekws_train_backward_launches", &t)) return 0;
+  switch (t.fam) {
+    case TrainFamily::Mdtc: return mdtc_train_backward_launches(t.mdtc.L);
+    case TrainFamily::MdtcHead: return mdtc_head_backward_launches(t.mdtc.L);
+    case TrainFamily::Tcn: return tcn_train_backward_launches(t.tcn);
+    case TrainFamily::Fsmn: return fsmn_backward_launches(m->cfg.num_layers);
+    default: return gru_backward_launches(m->cfg.num_layers);
+  }
+}
+
+extern "C" int64_t wekws_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save) {
+  const char* what = "wekws_train_workspace_bytes";
+  TrainModel t;
+  int rc = batch_stats_model(m, what, &t);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_backward_workspace_bytes: B, T >= 0 are required");
-  return mdtc_backward_workspace_bytes(d, B * T);
+  WEKWS_REQUIRE(B >= 0 && T >= 0, "%s: B, T >= 0 are required", what);
+  switch (t.fam) {
+    case TrainFamily::Mdtc: return mdtc_train_workspace_bytes(t.mdtc, B * T, save != 0);
+    case TrainFamily::MdtcHead: return mdtc_head_train_workspace_bytes(t.mdtc, B, T, save != 0);
+    default: return tcn_train_workspace_bytes(t.tcn, B * T, save != 0);
+  }
 }
 
-extern "C" int wekws_mdtc_train_forward_launches(const wekws_model* m) {
-  MdtcTrainDims d;
-  return mdtc_train_dims(m, "wekws_mdtc_train_forward_launches", &d) ? 0 : mdtc_train_forward_launches(d.L);
+extern "C" int wekws_train_forward_launches(const wekws_model* m) {
+  TrainModel t;
+  if (batch_stats_model(m, "wekws_train_forward_launches", &t)) return 0;
+  switch (t.fam) {
+    case TrainFamily::Mdtc: return mdtc_train_forward_launches(t.mdtc.L);
+    case TrainFamily::MdtcHead: return mdtc_head_train_forward_launches(t.mdtc.L);
+    default: return tcn_train_forward_launches(t.tcn);
+  }
 }
 
-extern "C" int wekws_mdtc_backward_launches(const wekws_model* m) {
-  MdtcTrainDims d;
-  return mdtc_train_dims(m, "wekws_mdtc_backward_launches", &d) ? 0 : mdtc_train_backward_launches(d.L);
-}
-
-extern "C" int wekws_mdtc_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                        const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
-                                        const double* h_bn, float* d_out, float* d_out_cache, float* d_saved, int save,
-                                        void* d_workspace, int64_t B, int64_t T, void* stream) {
-  MdtcTrainDims d;
-  const char* what = "wekws_mdtc_train_forward";
-  int rc = mdtc_train_dims(m, what, &d);
+extern "C" int wekws_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                   const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
+                                   const double* h_bn, uint64_t seed, const double* h_p, int n_p, float* d_out,
+                                   float* d_out_cache, float* d_saved, int save, void* d_workspace, int64_t B,
+                                   int64_t T, void* stream) {
+  const char* what = "wekws_train_forward";
+  TrainModel t;
+  MdtcHead head;
+  TcnDropout drop;
+  int rc = batch_stats_call(m, what, seed, h_p, n_p, &t, &head, &drop);
   if (rc) return rc;
-  if ((rc = batch_stats_forward_check(what, B, T, d.C, d.odim, n, mdtc_train_num_params(d.L), 3 * d.L, d_feats,
+  if ((rc = batch_stats_forward_check(what, B, T, m->cfg.hdim, m->cfg.odim, n, t.n_params, num_batch_norms(t), d_feats,
                                       h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache, d_saved,
                                       save, d_workspace)))
     return rc;
-  return mdtc_train_forward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache,
-                                   save ? d_saved : nullptr, d_workspace, (int)B, (int)T, (cudaStream_t)stream);
+  float* saved = save ? d_saved : nullptr;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (t.fam) {
+    case TrainFamily::Mdtc:
+      return mdtc_train_forward_launch(t.mdtc, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out,
+                                       d_out_cache, saved, d_workspace, (int)B, (int)T, st);
+    case TrainFamily::MdtcHead:
+      return mdtc_head_train_forward_launch(t.mdtc, head, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn,
+                                            d_out, d_out_cache, saved, d_workspace, (int)B, (int)T, st);
+    default:
+      return tcn_train_forward_launch(t.tcn, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out,
+                                      d_out_cache, saved, d_workspace, (int)B, (int)T, st);
+  }
 }
 
-extern "C" int wekws_mdtc_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                   const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
-                                   const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads,
-                                   void* d_workspace, void* stream) {
-  MdtcTrainDims d;
-  const char* what = "wekws_mdtc_backward";
-  int rc = mdtc_train_dims(m, what, &d);
+extern "C" int wekws_train_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
+                                    const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
+                                    const float* d_out, const float* d_grad_out, uint64_t seed, const double* h_p,
+                                    int n_p, int64_t B, int64_t T, float* const* h_grads, void* d_workspace,
+                                    void* stream) {
+  const char* what = "wekws_train_backward";
+  TrainModel t;
+  MdtcHead head;
+  TcnDropout drop;
+  int rc = batch_stats_call(m, what, seed, h_p, n_p, &t, &head, &drop);
   if (rc) return rc;
-  if ((rc = batch_stats_backward_check(what, B, T, d.C, d.odim, n, mdtc_train_num_params(d.L), h_params, h_grads,
-                                       d_feats && d_saved && d_grad_out && d_workspace)))
+  const bool reads_out = t.fam == TrainFamily::Tcn;      // only the TCN backward reads the logits
+  if ((rc = batch_stats_backward_check(what, B, T, m->cfg.hdim, m->cfg.odim, n, t.n_params, h_params, h_grads,
+                                       d_feats && d_saved && (d_out || !reads_out) && d_grad_out && d_workspace)))
     return rc;
-  return mdtc_backward_launch(d, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B, (int)T,
-                              h_grads, d_workspace, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (t.fam) {
+    case TrainFamily::Mdtc:
+      return mdtc_backward_launch(t.mdtc, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B,
+                                  (int)T, h_grads, d_workspace, st);
+    case TrainFamily::MdtcHead:
+      return mdtc_head_backward_launch(t.mdtc, head, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out,
+                                       (int)B, (int)T, h_grads, d_workspace, st);
+    default:
+      return tcn_backward_launch(t.tcn, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_out, d_grad_out,
+                                 (int)B, (int)T, h_grads, d_workspace, st);
+  }
 }
 
-// ------------------------------------------------------------------------------- MDTC training, global / last head
-extern "C" int wekws_mdtc_head_num_params(const wekws_model* m) {
-  MdtcTrainDims d;
-  return mdtc_dims(m, "wekws_mdtc_head_num_params", true, &d) ? 0 : mdtc_head_train_num_params(d.L);
-}
-
-extern "C" int64_t wekws_mdtc_head_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
-  MdtcTrainDims d;
-  int rc = mdtc_dims(m, "wekws_mdtc_head_train_saved_floats", true, &d);
+extern "C" int wekws_model_load_params(wekws_model* m, const float* const* h_params, int n, void* stream) {
+  const char* what = "wekws_model_load_params";
+  TrainModel t;
+  int rc = packed_model(m, what, &t);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_head_train_saved_floats: B, T >= 0 are required");
-  return mdtc_head_train_saved_floats(d, B, T);
+  WEKWS_REQUIRE(h_params && n == t.n_params, "%s: expected the %d parameters of a %d-layer %s model, got %d", what,
+                t.n_params, m->cfg.num_layers, train_label(t.fam), n);
+  FsmnPackArgs p{};
+  p.packed = m->d_vec;
+  p.n = n;
+  int k = 0;                                   // the parameters in order, each [rows][cols] into its place in the pack
+  auto put = [&](int rows, int cols, long long dst, int ld) {
+    FsmnParamCopy& c = p.p[k];
+    c.src = h_params[k]; c.dst = dst; c.rows = rows; c.cols = cols; c.ld = ld;
+    ++k;
+  };
+  if (t.fam == TrainFamily::Fsmn) {            // state_dict order into pack_fsmn's layout
+    const FsmnArgs& a = m->fsmn;
+    const int D = a.lin, P = a.proj;
+    put(a.aff_in, a.idim, a.o_w_in1, a.np_aff_in); put(a.aff_in, 1, a.o_b_in1, 1);
+    put(D, a.aff_in, a.o_w_in2, a.np_lin); put(D, 1, a.o_b_in2, 1);
+    for (int l = 0; l < a.L; ++l) {
+      const long long base = a.o_layers + (long long)l * a.layer_stride;
+      put(P, D, base + a.lo_wp, a.np_proj);
+      put(P, a.lorder, base + a.lo_taps, P);
+      put(P, a.rorder, base + a.lo_taps + (long long)a.lorder * P, P);
+      put(D, P, base + a.lo_wa, a.np_lin); put(D, 1, base + a.lo_ba, 1);
+    }
+    put(a.aff_out, D, a.o_w_out1, a.np_aff_out); put(a.aff_out, 1, a.o_b_out1, 1);
+    put(a.odim, a.aff_out, a.o_w_out2, a.np_odim); put(a.odim, 1, a.o_b_out2, 1);
+  } else {                                     // named_parameters order into pack_gru's layout
+    const GruArgs& a = m->gru;
+    const int H = a.H, G = 3 * H;
+    put(H, a.idim, a.v_wp, H); put(H, 1, a.v_bp, 1);
+    for (int l = 0; l < a.L; ++l) {
+      const long long base = a.v_layers + (long long)l * a.v_layer_stride;
+      put(G, H, base, 2 * G); put(G, H, base + G, 2 * G);
+      put(G, 1, base + 2LL * H * G, 1); put(G, 1, base + 2LL * H * G + G, 1);
+    }
+    put(a.odim, H, a.v_wc, a.odim); put(a.odim, 1, a.v_bc, 1);
+  }
+  for (int i = 0; i < p.n; ++i) WEKWS_REQUIRE(p.p[i].src != nullptr, "%s: parameter %d is null", what, i);
+  return fsmn_pack_launch(p, (cudaStream_t)stream);
 }
 
-extern "C" int64_t wekws_mdtc_head_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save) {
-  MdtcTrainDims d;
-  int rc = mdtc_dims(m, "wekws_mdtc_head_train_workspace_bytes", true, &d);
+extern "C" int wekws_model_train_forward(wekws_model* m, const float* d_feats, float* d_out, float* d_out_cache,
+                                         float* d_saved, int64_t B, int64_t T, void* stream) {
+  const char* what = "wekws_model_train_forward";
+  TrainModel t;
+  int rc = packed_model(m, what, &t);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_head_train_workspace_bytes: B, T >= 0 are required");
-  return mdtc_head_train_workspace_bytes(d, B, T, save != 0);
-}
-
-extern "C" int64_t wekws_mdtc_head_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
-  MdtcTrainDims d;
-  int rc = mdtc_dims(m, "wekws_mdtc_head_backward_workspace_bytes", true, &d);
-  if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_mdtc_head_backward_workspace_bytes: B, T >= 0 are required");
-  return mdtc_head_backward_workspace_bytes(d, B, T);
-}
-
-extern "C" int wekws_mdtc_head_train_forward_launches(const wekws_model* m) {
-  MdtcTrainDims d;
-  return mdtc_dims(m, "wekws_mdtc_head_train_forward_launches", true, &d) ? 0 : mdtc_head_train_forward_launches(d.L);
-}
-
-extern "C" int wekws_mdtc_head_backward_launches(const wekws_model* m) {
-  MdtcTrainDims d;
-  return mdtc_dims(m, "wekws_mdtc_head_backward_launches", true, &d) ? 0 : mdtc_head_backward_launches(d.L);
-}
-
-extern "C" int wekws_mdtc_head_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params,
-                                             int n, const float* d_cmvn_mean, const float* d_cmvn_istd,
-                                             float* const* h_running, const double* h_bn, uint64_t seed, double p,
-                                             float* d_out, float* d_out_cache, float* d_saved, int save,
-                                             void* d_workspace, int64_t B, int64_t T, void* stream) {
-  MdtcTrainDims d;
-  MdtcHead h;
-  const char* what = "wekws_mdtc_head_train_forward";
-  int rc = mdtc_dims(m, what, true, &d);
-  if (rc) return rc;
-  if ((rc = mdtc_head(m, seed, p, what, &h))) return rc;
-  if ((rc = batch_stats_forward_check(what, B, T, d.C, h.odim, n, mdtc_head_train_num_params(d.L), 3 * d.L, d_feats,
-                                      h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache, d_saved,
-                                      save, d_workspace)))
-    return rc;
-  return mdtc_head_train_forward_launch(d, h, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out,
-                                        d_out_cache, save ? d_saved : nullptr, d_workspace, (int)B, (int)T,
-                                        (cudaStream_t)stream);
-}
-
-extern "C" int wekws_mdtc_head_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                        const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
-                                        const float* d_grad_out, uint64_t seed, double p, int64_t B, int64_t T,
-                                        float* const* h_grads, void* d_workspace, void* stream) {
-  MdtcTrainDims d;
-  MdtcHead h;
-  const char* what = "wekws_mdtc_head_backward";
-  int rc = mdtc_dims(m, what, true, &d);
-  if (rc) return rc;
-  if ((rc = mdtc_head(m, seed, p, what, &h))) return rc;
-  if ((rc = batch_stats_backward_check(what, B, T, d.C, h.odim, n, mdtc_head_train_num_params(d.L), h_params, h_grads,
-                                       d_feats && d_saved && d_grad_out && d_workspace)))
-    return rc;
-  return mdtc_head_backward_launch(d, h, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_grad_out, (int)B,
-                                   (int)T, h_grads, d_workspace, (cudaStream_t)stream);
-}
-
-// ------------------------------------------------------------------------------- TCN / DS-TCN training
-namespace {
-
-// the dimensions of a TCN / DS-TCN model with the per-frame linear classifier, as the training kernels take them
-int tcn_train_dims(const wekws_model* m, const char* what, TcnTrainDims* d) {
-  WEKWS_REQUIRE(m, "%s: null handle", what);
-  const wekws_model_config& c = m->cfg;
-  WEKWS_REQUIRE(c.backbone == WEKWS_BACKBONE_TCN || c.backbone == WEKWS_BACKBONE_DSTCN,
-                "%s: a TCN or DS-TCN model is required", what);
-  WEKWS_REQUIRE(m->head == WEKWS_HEAD_LINEAR, "%s: the TCN model trains with the per-frame linear classifier", what);
-  WEKWS_REQUIRE((c.hdim == 64 || c.hdim == 256) && c.kernel_size >= 2 && c.kernel_size <= TCN_TRAIN_MAX_K &&
-                    c.num_layers >= 1 && c.num_layers <= TCN_TRAIN_MAX_LAYERS && c.idim >= 1 &&
-                    c.idim <= TCN_TRAIN_MAX_IDIM && c.odim >= 1 && c.odim <= TCN_TRAIN_MAX_ODIM,
-                "%s: TCN training supports hidden_dim 64 or 256, kernel_size 2..%d, 1..%d layers, input_dim <= %d and "
-                "output_dim <= %d; got hidden %d, kernel %d, %d layers, input %d, output %d", what, TCN_TRAIN_MAX_K,
-                TCN_TRAIN_MAX_LAYERS, TCN_TRAIN_MAX_IDIM, TCN_TRAIN_MAX_ODIM, c.hdim, c.kernel_size, c.num_layers,
-                c.idim, c.odim);
-  memset(d, 0, sizeof(*d));
-  d->C = c.hdim; d->idim = c.idim; d->odim = c.odim; d->K = c.kernel_size; d->L = c.num_layers;
-  d->ds = c.backbone == WEKWS_BACKBONE_DSTCN ? 1 : 0;
-  d->act = c.activation == WEKWS_ACT_SIGMOID ? 1 : 0;
-  d->norm_var = c.norm_var;
-  d->pad_total = (c.kernel_size - 1) * ((1 << c.num_layers) - 1);
-  return WEKWS_OK;
-}
-
-// theta = ceil(p 2^24) in double, scale = 1 / (float)(1 - p), torch's scale
-int tcn_dropout(const TcnTrainDims& d, uint64_t seed, const double* h_p, const char* what, TcnDropout* o) {
-  WEKWS_REQUIRE(h_p, "%s: null dropout probabilities", what);
-  memset(o, 0, sizeof(*o));
-  o->seed = seed;
-  for (int l = 0; l < d.L; ++l) {
-    WEKWS_REQUIRE(h_p[l] >= 0.0 && h_p[l] <= 1.0, "%s: dropout probability %g of block %d is outside [0, 1]", what,
-                  h_p[l], l);
-    o->theta[l] = (uint32_t)ceil(h_p[l] * 16777216.0);
-    o->scale[l] = 1.0f / (float)(1.0 - h_p[l]);
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "%s: bad B/T", what);
+  WEKWS_REQUIRE(d_feats && d_out && d_out_cache && d_saved, "%s: null tensor", what);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (t.fam == TrainFamily::Gru) {
+    GruArgs a = m->gru;                        // the FP32 kernel whatever the precision mode
+    a.feats = d_feats; a.in_cache = nullptr; a.out = d_out; a.out_cache = d_out_cache;
+    a.B = (int)B; a.T = (int)T; a.saved = d_saved;
+    return gru_launch(a, st, true);
+  }
+  // FSMN: the time chunks of wekws_model_forward, each launch also storing its frames' activations
+  const int maxT = fsmn_tile_rows();
+  const int nchunk = (int)((T + maxT - 1) / maxT);
+  const int Tc = (int)((T + nchunk - 1) / nchunk);
+  for (int64_t t0 = 0; t0 < T; t0 += Tc) {
+    FsmnArgs a = m->fsmn;
+    a.feats = d_feats + t0 * m->cfg.idim;
+    a.out = d_out + t0 * m->cfg.odim;
+    a.in_cache = t0 == 0 ? nullptr : d_out_cache;
+    a.out_cache = d_out_cache;
+    a.B = (int)B;
+    a.T = (int)(T - t0 < Tc ? T - t0 : Tc);
+    a.feat_bstride = T * m->cfg.idim;
+    a.out_bstride = T * m->cfg.odim;
+    a.saved = d_saved; a.save_T = (int)T; a.save_t0 = (int)t0;
+    if ((rc = fsmn_train_launch(a, st))) return rc;
   }
   return WEKWS_OK;
 }
 
-}  // namespace
-
-extern "C" int wekws_tcn_num_params(const wekws_model* m) {
-  TcnTrainDims d;
-  return tcn_train_dims(m, "wekws_tcn_num_params", &d) ? 0 : tcn_train_num_params(d);
-}
-
-extern "C" int64_t wekws_tcn_train_saved_floats(const wekws_model* m, int64_t B, int64_t T) {
-  TcnTrainDims d;
-  int rc = tcn_train_dims(m, "wekws_tcn_train_saved_floats", &d);
+extern "C" int wekws_model_backward(wekws_model* m, const float* d_feats, const float* d_saved, const float* d_out,
+                                    const float* d_grad_out, int64_t B, int64_t T, float* const* h_grads, int n,
+                                    void* d_workspace, void* stream) {
+  const char* what = "wekws_model_backward";
+  TrainModel t;
+  int rc = packed_model(m, what, &t);
   if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_tcn_train_saved_floats: B, T >= 0 are required");
-  return tcn_train_saved_floats(d, B * T);
-}
-
-extern "C" int64_t wekws_tcn_train_workspace_bytes(const wekws_model* m, int64_t B, int64_t T, int save) {
-  TcnTrainDims d;
-  int rc = tcn_train_dims(m, "wekws_tcn_train_workspace_bytes", &d);
-  if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_tcn_train_workspace_bytes: B, T >= 0 are required");
-  return tcn_train_workspace_bytes(d, B * T, save != 0);
-}
-
-extern "C" int64_t wekws_tcn_backward_workspace_bytes(const wekws_model* m, int64_t B, int64_t T) {
-  TcnTrainDims d;
-  int rc = tcn_train_dims(m, "wekws_tcn_backward_workspace_bytes", &d);
-  if (rc) return rc;
-  WEKWS_REQUIRE(B >= 0 && T >= 0, "wekws_tcn_backward_workspace_bytes: B, T >= 0 are required");
-  return tcn_backward_workspace_bytes(d, B * T);
-}
-
-extern "C" int wekws_tcn_train_forward_launches(const wekws_model* m) {
-  TcnTrainDims d;
-  return tcn_train_dims(m, "wekws_tcn_train_forward_launches", &d) ? 0 : tcn_train_forward_launches(d);
-}
-
-extern "C" int wekws_tcn_backward_launches(const wekws_model* m) {
-  TcnTrainDims d;
-  return tcn_train_dims(m, "wekws_tcn_backward_launches", &d) ? 0 : tcn_train_backward_launches(d);
-}
-
-extern "C" int wekws_tcn_train_forward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                       const float* d_cmvn_mean, const float* d_cmvn_istd, float* const* h_running,
-                                       const double* h_bn, uint64_t seed, const double* h_p, float* d_out,
-                                       float* d_out_cache, float* d_saved, int save, void* d_workspace, int64_t B,
-                                       int64_t T, void* stream) {
-  TcnTrainDims d;
-  TcnDropout drop;
-  const char* what = "wekws_tcn_train_forward";
-  int rc = tcn_train_dims(m, what, &d);
-  if (rc) return rc;
-  if ((rc = tcn_dropout(d, seed, h_p, what, &drop))) return rc;
-  if ((rc = batch_stats_forward_check(what, B, T, d.C, d.odim, n, tcn_train_num_params(d), tcn_train_num_bns(d),
-                                      d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out, d_out_cache,
-                                      d_saved, save, d_workspace)))
-    return rc;
-  return tcn_train_forward_launch(d, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, h_running, h_bn, d_out,
-                                  d_out_cache, save ? d_saved : nullptr, d_workspace, (int)B, (int)T,
-                                  (cudaStream_t)stream);
-}
-
-extern "C" int wekws_tcn_backward(const wekws_model* m, const float* d_feats, const float* const* h_params, int n,
-                                  const float* d_cmvn_mean, const float* d_cmvn_istd, const float* d_saved,
-                                  const float* d_out, const float* d_grad_out, uint64_t seed, const double* h_p,
-                                  int64_t B, int64_t T, float* const* h_grads, void* d_workspace, void* stream) {
-  TcnTrainDims d;
-  TcnDropout drop;
-  const char* what = "wekws_tcn_backward";
-  int rc = tcn_train_dims(m, what, &d);
-  if (rc) return rc;
-  if ((rc = tcn_dropout(d, seed, h_p, what, &drop))) return rc;
-  if ((rc = batch_stats_backward_check(what, B, T, d.C, d.odim, n, tcn_train_num_params(d), h_params, h_grads,
-                                       d_feats && d_saved && d_out && d_grad_out && d_workspace)))
-    return rc;
-  return tcn_backward_launch(d, drop, d_feats, h_params, d_cmvn_mean, d_cmvn_istd, d_saved, d_out, d_grad_out, (int)B,
-                             (int)T, h_grads, d_workspace, (cudaStream_t)stream);
+  const bool gru = t.fam == TrainFamily::Gru;              // only the GRU backward reads the logits
+  WEKWS_REQUIRE(B >= 1 && T >= 1 && B < (1 << 30) && T < (1 << 30), "%s: bad B/T", what);
+  WEKWS_REQUIRE(d_feats && d_saved && (d_out || !gru) && d_grad_out && d_workspace && h_grads, "%s: null argument",
+                what);
+  WEKWS_REQUIRE(n == t.n_params, "%s: expected %d gradient buffers, got %d", what, t.n_params, n);
+  for (int i = 0; i < n; ++i) WEKWS_REQUIRE(h_grads[i] != nullptr, "%s: gradient buffer %d is null", what, i);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (gru)
+    return gru_backward_launch(m->gru, d_feats, d_saved, d_out, d_grad_out, (int)B, (int)T, h_grads,
+                               (float*)d_workspace, st);
+  return fsmn_backward_launch(m->fsmn, d_feats, d_saved, d_grad_out, (int)B, (int)T, h_grads, (float*)d_workspace, st);
 }
 
 extern "C" int wekws_dropout_mask(uint64_t seed, int64_t B, int64_t T, int64_t C, int layer, uint32_t theta,

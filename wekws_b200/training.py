@@ -35,11 +35,10 @@ Which models train, and how they opt in:
 
 Dropout (TCN / DS-TCN blocks, the MDTC heads): no device generator reproduces torch's Bernoulli stream, so every
 ``nn.Dropout`` applies a mask that is a documented pure function of a 64-bit seed (include/wekws_b200.h,
-``wekws_tcn_train_forward``, ``wekws_mdtc_head_train_forward``).  The seed is one draw from torch's default CPU
-generator per training forward (``frontend.draw_seed``), so ``torch.manual_seed`` makes a run reproducible; when every
-``p`` is 0 nothing is drawn.  ``p`` is read from the model's own ``nn.Dropout`` modules at call time.  The backward
-recomputes the masks from the seed; they are never stored.  ``device_dropout=True`` is the caller's acceptance of these
-masks in place of torch's.
+``wekws_train_forward``).  The seed is one draw from torch's default CPU generator per training forward
+(``frontend.draw_seed``), so ``torch.manual_seed`` makes a run reproducible; when every ``p`` is 0 nothing is drawn.
+``p`` is read from the model's own ``nn.Dropout`` modules at call time.  The backward recomputes the masks from the
+seed; they are never stored.  ``device_dropout=True`` is the caller's acceptance of these masks in place of torch's.
 
 Refused: GRU training without ``bptt=True``, a GRU with inter-layer Dropout or outside the kernels' limits, and the
 heads behind TCN / DS-TCN (at ``enable_training``); per call, ``forward_softmax``, a non-empty streaming cache,
@@ -219,9 +218,9 @@ class _Config:
         _native.lib().wekws_model_destroy(self.h)
 
 
-def _run_forward(fam, net, x, params, cmvn, running, hyper, drop, cache_shape, save: bool):
-    """(logits, out_cache, saved activations -- empty without `save`) of the ``wekws_{fam}_train_forward`` call:
-    logits (B, T, odim), or (B, odim) with a head."""
+def _run_forward(net, x, params, cmvn, running, hyper, drop, cache_shape, save: bool):
+    """(logits, out_cache, saved activations -- empty without `save`) of the ``wekws_train_forward`` call: logits
+    (B, T, odim), or (B, odim) with a head."""
     dev = x.device
     B, T = x.shape[0], x.shape[1]
     lib = _native.lib()
@@ -230,27 +229,25 @@ def _run_forward(fam, net, x, params, cmvn, running, hyper, drop, cache_shape, s
                       dtype=torch.float32)
     out_cache = torch.empty(cache_shape, device=dev, dtype=torch.float32)
     with _Config(net) as h:
-        saved = torch.empty(int(getattr(lib, f"wekws_{fam}_train_saved_floats")(h, B, T)) if save else 0, device=dev,
-                            dtype=torch.float32)
-        ws = torch.empty(int(getattr(lib, f"wekws_{fam}_train_workspace_bytes")(h, B, T, int(save))), device=dev,
-                         dtype=torch.uint8)
-        _native.call(f"wekws_{fam}_train_forward", h, x, _pointers(params), len(params), cmvn[0], cmvn[1],
+        saved = torch.empty(int(lib.wekws_train_saved_floats(h, B, T)) if save else 0, device=dev, dtype=torch.float32)
+        ws = torch.empty(int(lib.wekws_train_workspace_bytes(h, B, T, int(save))), device=dev, dtype=torch.uint8)
+        _native.call("wekws_train_forward", h, x, _pointers(params), len(params), cmvn[0], cmvn[1],
                      _pointers(running), hyper, *drop, out, out_cache, saved if save else None, int(save), ws, B, T,
                      device=dev)
     return out, out_cache, saved
 
 
 class _BatchStatsTrain(torch.autograd.Function):
-    """(logits, out_cache) of an MDTC (`fam` "mdtc"), MDTC with a head ("mdtc_head") or TCN / DS-TCN ("tcn")
-    training forward of the native model `net` (config, head id), whose Dropout arguments `drop` are (seed, per-block
-    p), (seed, p) or, for MDTC, empty; the backward returns one gradient per parameter."""
+    """(logits, out_cache) of an MDTC, MDTC with a head or TCN / DS-TCN training forward of the native model `net`
+    (config, head id), whose Dropout arguments `drop` are (seed, probabilities, their count); the backward returns one
+    gradient per parameter."""
 
     @staticmethod
-    def forward(ctx, fam, net, x, cmvn, running, hyper, drop, cache_shape, *params):
-        out, out_cache, saved = _run_forward(fam, net, x, params, cmvn, running, hyper, drop, cache_shape, True)
-        kept = (out,) if fam == "tcn" else ()         # only the TCN backward reads the logits
+    def forward(ctx, net, x, cmvn, running, hyper, drop, cache_shape, *params):
+        out, out_cache, saved = _run_forward(net, x, params, cmvn, running, hyper, drop, cache_shape, True)
+        kept = (out,) if net[0].backbone != _native.BACKBONE_MDTC else ()   # only the TCN backward reads the logits
         ctx.save_for_backward(x, saved, *kept, *params)  # the version check: no in-place change before backward
-        ctx.fam, ctx.net, ctx.cmvn, ctx.drop, ctx.nkept = fam, net, cmvn, drop, len(kept)
+        ctx.net, ctx.cmvn, ctx.drop, ctx.nkept = net, cmvn, drop, len(kept)
         ctx.mark_non_differentiable(out_cache)
         return out, out_cache
 
@@ -264,41 +261,40 @@ class _BatchStatsTrain(torch.autograd.Function):
         g_out = _grad_out(g_out, dev)
         grads = [torch.empty_like(p) for p in params]
         with _Config(ctx.net) as h:
-            ws = torch.empty(int(getattr(_native.lib(), f"wekws_{ctx.fam}_backward_workspace_bytes")(h, B, T)),
-                             device=dev, dtype=torch.uint8)
-            _native.call(f"wekws_{ctx.fam}_backward", h, x, _pointers(params), len(params), ctx.cmvn[0], ctx.cmvn[1],
-                         saved, *kept, g_out, *ctx.drop, B, T, _pointers(grads), ws, device=dev)
-        return (None,) * 8 + tuple(grads)
+            ws = torch.empty(int(_native.lib().wekws_train_backward_workspace_bytes(h, B, T)), device=dev,
+                             dtype=torch.uint8)
+            _native.call("wekws_train_backward", h, x, _pointers(params), len(params), ctx.cmvn[0], ctx.cmvn[1],
+                         saved, kept[0] if kept else None, g_out, *ctx.drop, B, T, _pointers(grads), ws, device=dev)
+        return (None,) * 7 + tuple(grads)
 
 
-def _load(fam: str, model, dev: torch.device, params) -> C.c_void_p:
+def _load(model, dev: torch.device, params) -> C.c_void_p:
     """The model's native handle on `dev` with `params` packed into it (one launch)."""
     h = model._training_handle(dev)
-    _native.call(f"wekws_{fam}_load_params", h, _pointers(params), len(params), device=dev)
+    _native.call("wekws_model_load_params", h, _pointers(params), len(params), device=dev)
     return h
 
 
 class _PackedTrain(torch.autograd.Function):
-    """(logits, out_cache) of the FSMN (`fam` "fsmn") or GRU ("gru") training forward, which runs on the model's
-    native handle with the parameters packed into it; the backward returns one gradient per parameter."""
+    """(logits, out_cache) of the FSMN or GRU training forward, which runs on the model's native handle with the
+    parameters packed into it; the backward returns one gradient per parameter."""
 
     @staticmethod
-    def forward(ctx, fam, model, x, *params):
+    def forward(ctx, model, x, *params):
         dev = x.device
         B, T = x.shape[0], x.shape[1]
         out = torch.empty(B, T, model.odim, device=dev, dtype=torch.float32)
         if B > 0 and T > 0:
-            h = _load(fam, model, dev, params)
+            h = _load(model, dev, params)
             out_cache = torch.empty(model.cache_shape(B), device=dev, dtype=torch.float32)
-            saved = torch.empty(int(getattr(_native.lib(), f"wekws_{fam}_train_saved_floats")(h, B, T)), device=dev,
-                                dtype=torch.float32)
-            _native.call(f"wekws_{fam}_train_forward", h, x, out, out_cache, saved, B, T, device=dev)
+            saved = torch.empty(int(_native.lib().wekws_train_saved_floats(h, B, T)), device=dev, dtype=torch.float32)
+            _native.call("wekws_model_train_forward", h, x, out, out_cache, saved, B, T, device=dev)
         else:
             h, saved = None, torch.empty(0, device=dev)
             out_cache = torch.zeros(model.cache_shape(B), device=dev, dtype=torch.float32)
-        kept = (out,) if fam == "gru" else ()         # the Sigmoid backward reads the logits
+        kept = (out,) if _kind(model) == "gru" else ()   # the Sigmoid backward reads the logits
         ctx.save_for_backward(x, saved, *kept, *params)  # the version check: no in-place change before backward
-        ctx.fam, ctx.model, ctx.handle, ctx.nkept = fam, model, h, len(kept)
+        ctx.model, ctx.handle, ctx.nkept = model, h, len(kept)
         ctx.mark_non_differentiable(out_cache)
         return out, out_cache
 
@@ -312,18 +308,18 @@ class _PackedTrain(torch.autograd.Function):
         if B == 0 or T == 0:
             for g in grads:
                 g.zero_()
-            return (None, None, None) + tuple(grads)
+            return (None, None) + tuple(grads)
         dev = x.device
-        model, fam = ctx.model, ctx.fam
+        model = ctx.model
         h = model.__dict__.get("_handle")
         if h is not ctx.handle or model._handle_dev != dev:
-            h = _load(fam, model, dev, params)        # the handle was rebuilt since the forward: same values again
+            h = _load(model, dev, params)             # the handle was rebuilt since the forward: same values again
         g_out = _grad_out(g_out, dev)
-        ws = torch.empty(int(getattr(_native.lib(), f"wekws_{fam}_backward_workspace_bytes")(h, B, T)), device=dev,
+        ws = torch.empty(int(_native.lib().wekws_train_backward_workspace_bytes(h, B, T)), device=dev,
                          dtype=torch.uint8)
-        _native.call(f"wekws_{fam}_backward", h, x, saved, *kept, g_out, B, T, _pointers(grads), len(grads), ws,
-                     device=dev)
-        return (None, None, None) + tuple(grads)
+        _native.call("wekws_model_backward", h, x, saved, kept[0] if kept else None, g_out, B, T, _pointers(grads),
+                     len(grads), ws, device=dev)
+        return (None, None) + tuple(grads)
 
 
 def forward(model, x: torch.Tensor, in_cache: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -338,32 +334,32 @@ def forward(model, x: torch.Tensor, in_cache: torch.Tensor) -> Tuple[torch.Tenso
                       "torch.no_grad()")
         names = fsmn_train.param_names(bb.fsmn_layers) if kind == "fsmn" else gru_train.param_names(bb.num_layers)
         params = _params(model, dev, names, label)
-        return _PackedTrain.apply(kind, model, x.contiguous(), *params)
+        return _PackedTrain.apply(model, x.contiguous(), *params)
     label = _label(bb.kind)
     head = _native.HEAD_LINEAR
     if bb.kind == "mdtc" and model.head is not None:
-        fam, names = "mdtc_head", mdtc_train.head_param_names(bb.num_stack, bb.stack_size)
+        names = mdtc_train.head_param_names(bb.num_stack, bb.stack_size)
         head = {"global": _native.HEAD_GLOBAL, "last": _native.HEAD_LAST}[model.head]
     elif bb.kind == "mdtc":
-        fam, names = "mdtc", mdtc_train.param_names(bb.num_stack, bb.stack_size)
+        names = mdtc_train.param_names(bb.num_stack, bb.stack_size)
     else:
-        fam, names = "tcn", tcn_train.param_names(bb.num_layers, bb.ds)
+        names = tcn_train.param_names(bb.num_layers, bb.ds)
     params = _params(model, dev, names, label)
     cmvn, running, hyper, counters = _buffers(model, dev, _batch_norms(model), label)
     net = (model._native_config(), head)
     x = x.contiguous()
-    drop = ()
-    if fam == "tcn":
+    seed, ps = 0, []                             # Dropout: none in MDTC, one in a head, one per TCN block
+    if bb.kind != "mdtc":
         seed, ps = tcn_train.draw_dropout(model)
-        drop = (seed, (C.c_double * len(ps))(*ps))
-    elif fam == "mdtc_head":
+    elif head != _native.HEAD_LINEAR:
         seed, p = mdtc_train.draw_head_dropout(model)
-        drop = (seed, C.c_double(p))
+        ps = [p]
+    drop = (seed, (C.c_double * len(ps))(*ps), len(ps))
     B = x.shape[0]
     if wants_grad(model):
-        out, out_cache = _BatchStatsTrain.apply(fam, net, x, cmvn, running, hyper, drop, model.cache_shape(B), *params)
+        out, out_cache = _BatchStatsTrain.apply(net, x, cmvn, running, hyper, drop, model.cache_shape(B), *params)
     else:
-        out, out_cache, _ = _run_forward(fam, net, x, params, cmvn, running, hyper, drop, model.cache_shape(B), False)
+        out, out_cache, _ = _run_forward(net, x, params, cmvn, running, hyper, drop, model.cache_shape(B), False)
     torch._foreach_add_(counters, 1)
     model.invalidate()           # the running statistics changed without a version-counter bump: repack for eval
     return out, out_cache
