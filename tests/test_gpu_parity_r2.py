@@ -271,6 +271,30 @@ def test_fsmn_shipped_size_matches_oracle(B, T):
     assert torch.equal(y0, yz)
 
 
+def test_fsmn_at_exactly_48_kb_of_dynamic_shared_memory():
+    """Widths 20 / 20 / 20 / 20 with memory width 12 give row strides 24 + 24 + 16 = 64 floats, so both FSMN kernels ask
+    for exactly 48 KB of dynamic shared memory on top of their static shared memory: more than a kernel may take
+    without the opt-in.  Inference against the oracle; the training-mode forward (its own kernel) equals it bit for
+    bit."""
+    cfg = model_config("fsmn", input_dim=20, output_dim=5, activation="identity")
+    cfg["backbone"].update(input_affine_dim=20, linear_dim=20, proj_dim=12, output_affine_dim=20, num_layers=2)
+    torch.manual_seed(777)
+    m = synth.randomize_(init_model(cfg), seed=777).eval()
+    sd = {k: v.clone() for k, v in m.state_dict().items()}
+    m = m.to(DEV)
+    x = synth.features(9, 30, 20, seed=12)
+    cache = torch.randn(9, 12, 11, 2, generator=torch.Generator().manual_seed(9))
+    y, c = m(x.to(DEV), cache.to(DEV))
+    y_ref, c_ref = O.kws_forward(sd, cfg, x, cache)
+    assert y.shape == (9, 30, 5) and c.shape == (9, 12, 11, 2)
+    assert float((y.cpu() - y_ref).abs().max()) <= TOL_POST * max(1.0, float(y_ref.abs().max()))
+    assert float((c.cpu() - c_ref).abs().max()) <= TOL_POST * max(1.0, float(c_ref.abs().max()))
+    y_eval, c_eval = m(x.to(DEV))
+    y_train, c_train = m.train()(x.to(DEV))
+    assert torch.equal(y_train.detach().view(torch.int32), y_eval.view(torch.int32))
+    assert torch.equal(c_train.view(torch.int32), c_eval.view(torch.int32))
+
+
 def test_context_expansion_and_frame_skip_bit_exact():
     """Device transform == reference processor (golden) and oracle, bit for bit; ragged batch with zero padding."""
     from tests.conftest import golden

@@ -357,3 +357,17 @@ def test_patch_reference_rebinds_the_reference_factory():
                  "import wekws.model.mdtc  # the rest of the reference package stays importable\n" % ROOT)
     r = subprocess.run([sys.executable, "-c", code_real], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr
+
+
+def test_dynamic_shared_memory_opt_in_has_one_home():
+    """The dynamic shared-memory limit is a per-device attribute of a kernel function that every caller in the process
+    shares, so only opt_in_smem (model_host.cu) may set it: raised only, under one lock.  No other source sets the
+    attribute or names it."""
+    csrc = os.path.join(ROOT, "wekws_b200", "csrc")
+    code = {f: re.sub(r"//[^\n]*|/\*.*?\*/", "", open(os.path.join(csrc, f)).read(), flags=re.S)
+            for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh", ".h"))}
+    for name in ("cudaFuncSetAttribute", "cudaFuncAttributeMaxDynamicSharedMemorySize"):
+        assert {f: c.count(name) for f, c in code.items() if name in c} == {"model_host.cu": 1}, name
+    helper = re.search(r"^int opt_in_smem\(const void\* kernel, size_t bytes\) \{$.*?^\}$", code["model_host.cu"],
+                       flags=re.S | re.M)
+    assert helper and "cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize" in helper.group(0)

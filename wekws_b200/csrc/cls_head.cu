@@ -60,9 +60,7 @@ __global__ void __launch_bounds__(NT_HEAD) cls_head_kernel(const ClsHeadArgs a) 
 int cls_head_launch(const ClsHeadArgs& a, cudaStream_t st) {
   WEKWS_REQUIRE(a.B >= 1 && a.H >= 1 && a.odim >= 1, "cls_head_launch: bad shape");
   const size_t smem = (size_t)(a.H + kHeadWidth + a.odim) * sizeof(float);
-  if (smem > 48 * 1024) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(cls_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  }
+  if (const int rc = opt_in_smem((const void*)cls_head_kernel, smem)) return rc;
   cls_head_kernel<<<(unsigned)a.B, NT_HEAD, smem, st>>>(a);
   return check_launch("cls_head_kernel");
 }

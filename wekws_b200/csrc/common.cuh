@@ -44,6 +44,9 @@ inline int check_launch(const char* what) {
 }
 
 int device_sm_count();
+// Lets `kernel` launch on the current device with `bytes` of dynamic shared memory: raises its limit when needed,
+// never lowers it.  Thread-safe.
+int opt_in_smem(const void* kernel, size_t bytes);
 
 // ---- device helpers ----
 #ifdef __CUDACC__

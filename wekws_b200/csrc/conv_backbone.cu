@@ -427,8 +427,7 @@ __global__ void __launch_bounds__(NT, 1) conv_backbone_kernel(const ConvArgs a) 
 
 template <int C>
 int launch_c(const ConvArgs& a, int grid, size_t smem, cudaStream_t st) {
-  WEKWS_CUDA_OK(cudaFuncSetAttribute(conv_backbone_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem));
+  if (const int rc = opt_in_smem((const void*)conv_backbone_kernel<C>, smem)) return rc;
   conv_backbone_kernel<C><<<grid, NT, smem, st>>>(a);
   return check_launch("conv_backbone_kernel");
 }

@@ -547,17 +547,6 @@ __global__ void __launch_bounds__(32) ctc_stream_score_kernel(const StreamScoreA
   }
 }
 
-// the dynamic shared-memory opt-in of a kernel, once per device and size
-int opt_in_smem(const void* kern, size_t smem, size_t* attr_bytes /* [64] */) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_bytes[dev] < smem) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_bytes[dev] = smem;
-  }
-  return WEKWS_OK;
-}
-
 }  // namespace
 
 size_t ctc_state_bytes() { return sizeof(Work); }
@@ -567,9 +556,7 @@ template <bool kFromLogits>
 int prefix_beam_launch(const CtcArgs& a, cudaStream_t st) {
   const size_t smem = sizeof(Work) + (size_t)((a.V + 31) / 32) * 4;
   WEKWS_REQUIRE(smem <= 227 * 1024, "ctc decode: vocabulary %d too large for the shared-memory token bitmap", a.V);
-  static size_t attr_bytes[64] = {0};                  // per device: the largest dynamic size opted into so far
-  const int rc = opt_in_smem((const void*)ctc_prefix_beam_kernel<kFromLogits>, smem, attr_bytes);
-  if (rc != WEKWS_OK) return rc;
+  if (const int rc = opt_in_smem((const void*)ctc_prefix_beam_kernel<kFromLogits>, smem)) return rc;
   ctc_prefix_beam_kernel<kFromLogits><<<(unsigned)a.B, 32, smem, st>>>(a);
   return check_launch("ctc_prefix_beam_kernel");
 }
@@ -581,9 +568,7 @@ int ctc_launch(const CtcArgs& a, cudaStream_t st) {
 int ctc_spot_launch(const SpotArgs& a, cudaStream_t st) {
   const size_t smem = sizeof(Work) + (size_t)((a.V + 31) / 32) * 4;
   WEKWS_REQUIRE(smem <= 227 * 1024, "ctc spot: vocabulary %d too large for the shared-memory token bitmap", a.V);
-  static size_t attr_bytes[64] = {0};
-  const int rc = opt_in_smem((const void*)ctc_spot_kernel, smem, attr_bytes);
-  if (rc != WEKWS_OK) return rc;
+  if (const int rc = opt_in_smem((const void*)ctc_spot_kernel, smem)) return rc;
   ctc_spot_kernel<<<(unsigned)a.B, 32, smem, st>>>(a);
   return check_launch("ctc_spot_kernel");
 }
@@ -591,9 +576,7 @@ int ctc_spot_launch(const SpotArgs& a, cudaStream_t st) {
 int ctc_stream_score_launch(const StreamScoreArgs& a, cudaStream_t st) {
   const size_t smem = sizeof(Work) + (size_t)((a.V + 31) / 32) * 4;
   WEKWS_REQUIRE(smem <= 227 * 1024, "ctc stream score: vocabulary %d too large for the shared-memory token bitmap", a.V);
-  static size_t attr_bytes[64] = {0};
-  const int rc = opt_in_smem((const void*)ctc_stream_score_kernel, smem, attr_bytes);
-  if (rc != WEKWS_OK) return rc;
+  if (const int rc = opt_in_smem((const void*)ctc_stream_score_kernel, smem)) return rc;
   ctc_stream_score_kernel<<<(unsigned)a.B, 32, smem, st>>>(a);
   return check_launch("ctc_stream_score_kernel");
 }

@@ -530,7 +530,7 @@ static int fbank_launch(wekws_fbank* fb, const void* d_pcm, int pcm_dtype, int64
   WEKWS_CUDA_OK(cudaGetDevice(&dev));
   WEKWS_REQUIRE(dev == fb->device, "fbank handle was created on device %d but the current device is %d", fb->device, dev);
   WEKWS_REQUIRE(dev >= 0 && dev < 64, "fbank: device index %d out of range", dev);
-  static int occ_dev[64][8] = {};        // the shared-memory attribute and the occupancy are per device
+  static int occ_dev[64][8] = {};        // the occupancy is per device
   int* occ = occ_dev[dev];
   const int ti = (pcm_dtype == WEKWS_PCM_S16 ? 0 : 1) + (mf ? 2 : 0) + (dz ? 4 : 0);
   static const void* const kernels[8] = {
@@ -540,7 +540,7 @@ static int fbank_launch(wekws_fbank* fb, const void* d_pcm, int pcm_dtype, int64
       (const void*)fbank_kernel<int16_t, true, true>,   (const void*)fbank_kernel<float, true, true>};
   const void* kern = kernels[ti];
   if (occ[ti] == 0) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (const int rc = opt_in_smem(kern, smem)) return rc;
     WEKWS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[ti], kern, FB_NT, smem));
     if (occ[ti] < 1) occ[ti] = 1;
   }

@@ -256,14 +256,8 @@ int launch(FsmnArgs a, cudaStream_t st) {
   a.n_tiles = (a.B + a.S - 1) / a.S;
   const size_t smem = fsmn_smem_bytes(a);
   WEKWS_REQUIRE(smem <= 226 * 1024, "fsmn: layer widths need %zu bytes of shared memory (max 226 KB + static)", smem);
-  static size_t attr_bytes[64] = {0};                  // per device: the largest dynamic size opted into so far
   auto kernel = SAVE ? fsmn_train_kernel : fsmn_kernel;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && attr_bytes[dev] < smem) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_bytes[dev] = smem;
-  }
+  if (const int rc = opt_in_smem((const void*)kernel, smem)) return rc;
   const int sms = device_sm_count();
   const int grid = a.n_tiles < sms ? a.n_tiles : sms;
   kernel<<<grid, FN_T, smem, st>>>(a);

@@ -209,7 +209,7 @@ int launch_s(const GruArgs& a, cudaStream_t st) {
   const int idimP = (a.idim + 3) & ~3;
   const size_t smem = (size_t)(2 * CHUNK_FLOATS + S * GH + a.L * S * GH + 2 * S * GG + S * idimP) * sizeof(float);
   const int sms = device_sm_count();
-  WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_kernel<S, SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (const int rc = opt_in_smem((const void*)gru_kernel<S, SAVE>, smem)) return rc;
   const int grid = b.n_tiles < sms ? b.n_tiles : sms;
   gru_kernel<S, SAVE><<<grid, GG, smem, st>>>(b);
   return check_launch(SAVE ? "gru_kernel<save>" : "gru_kernel");

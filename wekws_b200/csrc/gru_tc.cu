@@ -412,13 +412,7 @@ int gru_tc_launch(GruTcArgs a, cudaStream_t st) {
   const int sms0 = device_sm_count();
   a.ms = a.B > 32 * sms0 ? 64 : a.B > 16 * sms0 ? 32 : 16;
   a.n_tiles = (a.B + a.ms - 1) / a.ms;
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    attr_set[dev] = true;
-  }
+  if (const int rc = opt_in_smem((const void*)gru_tc_kernel, SMEM_BYTES)) return rc;
   const int sms = device_sm_count();
   const int grid = a.n_tiles < sms ? a.n_tiles : sms;
   gru_tc_kernel<<<grid, NT, SMEM_BYTES, st>>>(a);

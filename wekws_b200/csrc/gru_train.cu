@@ -151,7 +151,7 @@ template <int S>
 int bptt_s(BpttArgs a, cudaStream_t st) {
   a.n_tiles = (a.B + S - 1) / S;
   const size_t smem = (size_t)(GG * WLD + S * (GG + 3 * GH + GH)) * sizeof(float);
-  WEKWS_CUDA_OK(cudaFuncSetAttribute(gru_bptt_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (const int rc = opt_in_smem((const void*)gru_bptt_kernel<S>, smem)) return rc;
   const int sms = device_sm_count();
   gru_bptt_kernel<S><<<a.n_tiles < sms ? a.n_tiles : sms, GG, smem, st>>>(a);
   return check_launch("gru_bptt_kernel");

@@ -146,13 +146,7 @@ int linear_tc_launch(LinearTcArgs a, cudaStream_t st) {
                 (long long)a.rows, a.N, a.K);
   WEKWS_REQUIRE(((uintptr_t)a.x & 15) == 0 && (a.x_stride & 3) == 0, "linear_tc_launch: input rows must be 16-byte aligned");
   a.n_mtiles = (int)((a.rows + 127) / 128);
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    attr_set[dev] = true;
-  }
+  if (const int rc = opt_in_smem((const void*)linear_tc_kernel, SMEM_BYTES)) return rc;
   const int sms = device_sm_count();
   const int grid = a.n_mtiles < sms ? a.n_mtiles : sms;
   linear_tc_kernel<<<grid, NT, SMEM_BYTES, st>>>(a);

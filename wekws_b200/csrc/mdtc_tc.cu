@@ -734,23 +734,11 @@ int mdtc_tc_launch(TcArgs a, int padmax, cudaStream_t st, bool head) {
   }
   const int sms = device_sm_count();
   const int grid = a.B < sms ? a.B : sms;
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL_HEAD));
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(mdtc_tc_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL_HEAD));
-    attr_set[dev] = true;
-  }
-  if (head) {
-    if (a.ktaps == 5) mdtc_tc_kernel<5, true><<<grid, NT_TC, SMEM_TOTAL_HEAD, st>>>(a);
-    else mdtc_tc_kernel<0, true><<<grid, NT_TC, SMEM_TOTAL_HEAD, st>>>(a);
-    return check_launch("mdtc_tc_kernel");
-  }
-  if (a.ktaps == 5) mdtc_tc_kernel<5, false><<<grid, NT_TC, SMEM_TOTAL, st>>>(a);
-  else mdtc_tc_kernel<0, false><<<grid, NT_TC, SMEM_TOTAL, st>>>(a);
+  auto* kernel = head ? (a.ktaps == 5 ? mdtc_tc_kernel<5, true> : mdtc_tc_kernel<0, true>)
+                      : (a.ktaps == 5 ? mdtc_tc_kernel<5, false> : mdtc_tc_kernel<0, false>);
+  const int smem = head ? SMEM_TOTAL_HEAD : SMEM_TOTAL;
+  if (const int rc = opt_in_smem((const void*)kernel, smem)) return rc;
+  kernel<<<grid, NT_TC, smem, st>>>(a);
   return check_launch("mdtc_tc_kernel");
 }
 

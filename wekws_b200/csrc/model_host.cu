@@ -56,6 +56,29 @@ int device_sm_count() {
   return cached[dev];
 }
 
+// cudaFuncAttributeMaxDynamicSharedMemorySize belongs to the kernel function on a device, not to a caller: every
+// caller in the process shares it.  So it is only ever raised, per device and kernel instance, to the largest size any
+// launch has needed; a later, smaller launch never lowers it under a concurrent larger one.  The starting limit is
+// read from the kernel, not assumed: without an opt-in, static and dynamic shared memory share 48 KB.
+int opt_in_smem(const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> limit;   // (device, kernel) -> its dynamic shared-memory limit
+  int dev = 0;
+  WEKWS_CUDA_OK(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = limit.find({dev, kernel});
+  if (it == limit.end()) {
+    cudaFuncAttributes fa;
+    WEKWS_CUDA_OK(cudaFuncGetAttributes(&fa, kernel));
+    it = limit.emplace(std::make_pair(dev, kernel), (size_t)fa.maxDynamicSharedSizeBytes).first;
+  }
+  if (it->second < bytes) {
+    WEKWS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    it->second = bytes;
+  }
+  return WEKWS_OK;
+}
+
 namespace {
 
 __global__ void softmax_rows_kernel(float* x, long long rows, int n) {

@@ -16,7 +16,6 @@
 // are replaced by zeros, never read as data; outputs past a row's length are written as zeros.
 #include <stdint.h>
 
-#include <mutex>
 #include <new>
 #include <vector>
 
@@ -131,21 +130,6 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(const ResampleArgs
   }
 }
 
-// cudaFuncAttributeMaxDynamicSharedMemorySize belongs to the kernel function, not to a handle: every handle on a
-// device shares it.  So it is only ever raised, per device and kernel instance, to the largest size any handle has
-// needed; a handle created later with a smaller table never lowers it under an existing one.
-int raise_smem_limit(int dev, int ti, const void* kern, size_t smem) {
-  static std::mutex mu;
-  static size_t opted[64][2] = {};
-  WEKWS_REQUIRE(dev >= 0 && dev < 64, "resample: device index %d out of range", dev);
-  std::lock_guard<std::mutex> lock(mu);
-  if (opted[dev][ti] < smem) {
-    WEKWS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    opted[dev][ti] = smem;
-  }
-  return WEKWS_OK;
-}
-
 long long gcd_ll(long long a, long long b) {
   while (b) { const long long t = a % b; a = b; b = t; }
   return a;
@@ -219,7 +203,7 @@ extern "C" int wekws_resample_create(int orig_freq, int new_freq, const float* h
   }
   const void* kern[2] = {(const void*)resample_kernel<int16_t>, (const void*)resample_kernel<float>};
   for (int i = 0; i < 2; ++i) {
-    const int rc = raise_smem_limit(h->device, i, kern[i], h->smem);     // forward checks the device matches
+    const int rc = opt_in_smem(kern[i], h->smem);     // h->device is current; forward checks it still is
     if (rc != WEKWS_OK) {
       wekws_resample_destroy(h);
       return rc;

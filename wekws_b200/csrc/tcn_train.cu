@@ -774,16 +774,7 @@ long long partial_doubles(const std::vector<Job>& js) {
 
 template <auto kernel, class Arg>
 int launch_dyn(dim3 grid, size_t smem, const Arg& a, cudaStream_t st, const char* name) {
-  // the opt-in above 48 KB of dynamic shared memory, once per instantiation and device (smem is fixed by C)
-  static bool opted[64] = {false};
-  if (smem > 48 * 1024) {
-    int dev = 0;
-    WEKWS_CUDA_OK(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !opted[dev]) {
-      WEKWS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      if (dev >= 0 && dev < 64) opted[dev] = true;
-    }
-  }
+  if (const int rc = opt_in_smem((const void*)kernel, smem)) return rc;
   kernel<<<grid, NT, smem, st>>>(a);
   return check_launch(name);
 }
