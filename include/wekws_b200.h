@@ -35,6 +35,10 @@
  *                          (beam-search step, execute_detection, resets), for many streams per call.
  *   wekws_ctc_stream_score the per-utterance frame loop of wekws/bin/stream_score_ctc.py:221-377 (streaming
  *                          decode with its own detection rule over whole utterances of a test set).
+ *   wekws_det_stats        the threshold sweep of wekws/bin/compute_det.py:76-105 over whole utterances.
+ *   wekws_threshold_spot / the alarm rule of that sweep online, for the max-pooling (Sigmoid) models: the
+ *   _state_bytes           per-stream records that let many live streams fire exactly as compute_det.py counts,
+ *                          chunk by chunk (added within ABI 19: no existing entry point changed).
  */
 #ifndef WEKWS_B200_H_
 #define WEKWS_B200_H_
@@ -250,6 +254,30 @@ WEKWS_API int wekws_model_forward(wekws_model* m, const float* d_feats, const fl
 WEKWS_API int wekws_det_stats(const float* d_post, const int32_t* d_lens, int64_t B, int64_t T, int K,
                     const double* d_thresholds, int nthr, int window_shift, double* d_max_score,
                     int32_t* d_triggers, void* stream);
+
+/* Online threshold detector of max-pooling keyword models: the trigger rule of wekws_det_stats (compute_det.py:91-97)
+ * applied to live streams chunk by chunk.  Per stream b and keyword k a record in d_state holds two int64: `seen`, the
+ * model frames consumed since reset, and `next`, the first frame index that may fire (a zero record is a stream after
+ * reset).  Stream b's frames of this call are rows d_rows[b] .. d_rows[b] + d_frames[b] - 1 of d_probs (row width K,
+ * the model's Sigmoid outputs); frame i of the call is t = seen + i.  It fires when t >= next and
+ * rint((double)p * 1e6) / 1e6 >= d_thresholds[k] (the text-rounded comparison of wekws_det_stats), which records the
+ * event (t, k, p) and sets next = t + window_shift; afterwards seen += d_frames[b].  Over the concatenation of a
+ * stream's chunks this is the compute_det.py scan for any chunking, so a stream's firings at threshold x number
+ * exactly wekws_det_stats' triggers at x.
+ *   d_counts (B, K): firings of this call (every one, also for streams with d_frames[b] <= 0, which count 0 and whose
+ *   records are not touched).  d_events (B, K, max_events): the first max_events firings of (b, k) in frame order.  A
+ *   pair fires at most once per window_shift frames, so max_events = ceil(max_b d_frames[b] / window_shift) holds
+ *   every firing.  d_events may be NULL when max_events is 0; every other pointer is required (B > 0).  One launch,
+ *   one thread per (b, k), no atomics.                                                                             */
+typedef struct {
+  int64_t frame;           /* t: model frames since the stream's reset                 */
+  int32_t keyword;         /* k                                                        */
+  float score;             /* the posterior p as the model wrote it                    */
+} wekws_threshold_event;
+WEKWS_API int64_t wekws_threshold_spot_state_bytes(void);   /* bytes of one (stream, keyword) record */
+WEKWS_API int wekws_threshold_spot(const float* d_probs, int K, const int32_t* d_rows, const int32_t* d_frames,
+                                   int64_t B, const double* d_thresholds, int window_shift, void* d_state,
+                                   int max_events, int32_t* d_counts, wekws_threshold_event* d_events, void* stream);
 
 /* CTC prefix beam search + keyword look-up on the device (SURVEY 8f-2, CTC models), bit-exact with the reference's pure
  * Python: wekws/model/loss.py:206-312 ctc_prefix_beam_search as called by wekws/bin/score_ctc.py:198-200 (whole

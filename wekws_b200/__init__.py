@@ -12,6 +12,8 @@ Public surface mirrors the reference (wenet-e2e/wekws):
     det_stats, det_curve     <- wekws/bin/compute_det.py threshold sweep (on the device, bit-exact)
     ctc_prefix_beam_search, ctc_keyword_hits, write_ctc_scores <- wekws/model/loss.py:206-312 + score_ctc.py:198-226
     KeywordSpotter           <- wekws/bin/stream_kws_ctc.py KeyWordSpotter: online CTC keyword spotting, B streams per call
+    ThresholdSpotter, ThresholdDecoder <- wekws/bin/compute_det.py's alarm rule online: keyword spotting with the
+                                max-pooling (Sigmoid) models, B streams per call, firing where the DET curve counts
     stream_score_ctc, write_stream_ctc_scores <- wekws/bin/stream_score_ctc.py: streaming decode of a CTC test set
     ctc_det_stats, write_ctc_det_stats <- wekws/bin/compute_det_ctc.py: DET statistics of a CTC score file
     criterion                <- wekws/model/loss.py criterion(): held-out loss / accuracy (max_pooling, ce, ctc)
@@ -41,13 +43,14 @@ from .overlay import patch_reference
 from .pipeline import Pipeline
 from .postproc import (context_expansion, ctc_det_stats, det_curve, det_stats, det_thresholds, space_mixed_label,
                        write_ctc_det_stats)
-from .spotter import KeywordSpotter, SpotResult
+from .spotter import KeywordSpotter, SpotResult, ThresholdDecoder, ThresholdResult, ThresholdSpotter
 from .train_features import TrainFeatures, spec_aug
 
 __all__ = ["init_model", "KWSModel", "GlobalCMVN", "Fbank", "fbank", "Mfcc", "mfcc", "load_cmvn", "load_kaldi_cmvn",
            "model_config", "MODEL_NAMES", "patch_reference", "export_native", "export_onnx", "det_stats", "det_curve", "det_thresholds", "context_expansion",
            "Pipeline", "ctc_prefix_beam_search", "ctc_keyword_hits", "ctc_state", "write_ctc_scores",
-           "KeywordSpotter", "SpotResult", "stream_score_ctc", "write_stream_ctc_scores", "ctc_det_stats",
+           "KeywordSpotter", "SpotResult", "ThresholdSpotter", "ThresholdDecoder", "ThresholdResult",
+           "stream_score_ctc", "write_stream_ctc_scores", "ctc_det_stats",
            "write_ctc_det_stats", "space_mixed_label", "criterion", "Resample", "resample", "CmvnStats", "scp_segment",
            "TrainFeatures", "spec_aug", "AugmentSource", "reverb", "add_noise", "Adam",
            "clip_grad_norm_"]

@@ -35,6 +35,8 @@ SPOT_RESULT_DTYPE = [("score", "<f8"), ("state", "<i4"), ("keyword", "<i4"), ("s
 SPOT_RESULT_BYTES = 32
 STREAM_DETECTION_DTYPE = [("score", "<f8"), ("keyword", "<i4"), ("start", "<i4"), ("end", "<i4"), ("frame", "<i4")]
 STREAM_DETECTION_BYTES = 24
+THRESHOLD_EVENT_DTYPE = [("frame", "<i8"), ("keyword", "<i4"), ("score", "<f4")]      # wekws_threshold_event
+THRESHOLD_EVENT_BYTES = 16
 
 
 class FbankConfig(C.Structure):
@@ -91,6 +93,9 @@ SIGNATURES = {
                                       C.c_int64, C.c_int64, C.c_uint32, C.c_void_p]),
     "wekws_det_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                   C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wekws_threshold_spot_state_bytes": (C.c_int64, []),
+    "wekws_threshold_spot": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int,
+                                       C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wekws_ctc_state_bytes": (C.c_int64, []),
     "wekws_ctc_prefix_beam_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int,
                                                C.c_int, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p,

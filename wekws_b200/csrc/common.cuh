@@ -70,6 +70,11 @@ __device__ __forceinline__ void cp_async_wait_pending(int pending) {
 }
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// The double Python parses back from '{:.6f}'.format(x) (the score file of wekws/bin/score.py:128-137): x * 1e6 is
+// exact in double for a float x in [0, 1] (24 x 20 significant bits), so rint of it is the 6-decimal text value.
+// The DET sweep and the online threshold detector compare scores through this one definition.
+__device__ __forceinline__ double text_round6(float x) { return rint((double)x * 1e6) / 1e6; }
+
 // Softmax normaliser of the row p[0..n) across one warp: every lane gets m = max p and s = sum expf(p[i] - m), and
 // the row's softmax is expf(p[i] - m) / s.  The model's softmax and the CTC criterion (log-softmax, and the
 // posteriors its accuracy decodes) share this code, so their probabilities are bit-identical.

@@ -14,8 +14,6 @@
 namespace wekws {
 namespace {
 
-__device__ __forceinline__ double text_round6(float x) { return rint((double)x * 1e6) / 1e6; }
-
 // one thread per (stream b, keyword k, threshold i); a warp covers consecutive thresholds of one (b, k), so the
 // posteriors it scans are broadcast loads
 __global__ void det_stats_kernel(const float* __restrict__ post, const int32_t* __restrict__ lens, long long B,
@@ -63,6 +61,77 @@ extern "C" int wekws_det_stats(const float* d_post, const int32_t* d_lens, int64
   det_stats_kernel<<<(unsigned)((total + nt - 1) / nt), nt, 0, (cudaStream_t)stream>>>(
       d_post, d_lens, B, T, K, d_thresholds, nthr, window_shift, d_max_score, d_triggers);
   return check_launch("det_stats_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// The same rule online: compute_det.py:91-97 over the concatenation of a stream's chunks, resumed each call from a
+// two-integer record per (stream, keyword).  After a firing at frame t the scan skips to t + window_shift, which may
+// lie in a later chunk, so the record keeps that frame as `next`.
+namespace wekws {
+namespace {
+
+struct ThresholdState {
+  long long seen;   // model frames consumed since reset
+  long long next;   // first frame index that may fire
+};
+
+// one thread per (stream b, keyword k); the thread owns that pair's record and its event slots, so there are no atomics
+__global__ void threshold_spot_kernel(const float* __restrict__ probs, int K, const int32_t* __restrict__ rows,
+                                      const int32_t* __restrict__ frames, long long B, const double* __restrict__ thr,
+                                      int window_shift, ThresholdState* __restrict__ state, int max_events,
+                                      int32_t* __restrict__ counts, wekws_threshold_event* __restrict__ events) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * K) return;
+  const long long b = idx / K;
+  const int k = (int)(idx - b * K);
+  const int n = frames[b];
+  int count = 0;
+  if (n > 0) {
+    ThresholdState s = state[idx];
+    const float* p = probs + (long long)rows[b] * K + k;
+    const double th = thr[k];
+    long long i = s.next > s.seen ? s.next - s.seen : 0;
+    while (i < n) {
+      const float x = p[i * K];
+      if (text_round6(x) >= th) {
+        const long long t = s.seen + i;
+        if (count < max_events) events[idx * max_events + count] = wekws_threshold_event{t, k, x};
+        ++count;
+        s.next = t + window_shift;
+        i += window_shift;
+      } else {
+        ++i;
+      }
+    }
+    s.seen += n;
+    state[idx] = s;
+  }
+  counts[idx] = count;
+}
+
+}  // namespace
+}  // namespace wekws
+
+static_assert(sizeof(wekws_threshold_event) == 16, "wekws_threshold_event layout is part of the C ABI");
+
+extern "C" int64_t wekws_threshold_spot_state_bytes(void) { return (int64_t)sizeof(ThresholdState); }
+
+extern "C" int wekws_threshold_spot(const float* d_probs, int K, const int32_t* d_rows, const int32_t* d_frames,
+                                    int64_t B, const double* d_thresholds, int window_shift, void* d_state,
+                                    int max_events, int32_t* d_counts, wekws_threshold_event* d_events, void* stream) {
+  WEKWS_REQUIRE(B >= 0 && B < (1ll << 31) && K >= 1 && K <= 65535, "wekws_threshold_spot: bad sizes");
+  WEKWS_REQUIRE(window_shift >= 1, "wekws_threshold_spot: window_shift must be >= 1 (got %d)", window_shift);
+  WEKWS_REQUIRE(max_events >= 0, "wekws_threshold_spot: max_events must be >= 0");
+  if (B == 0) return WEKWS_OK;
+  WEKWS_REQUIRE(d_probs && d_rows && d_frames && d_thresholds && d_state && d_counts &&
+                    (d_events || max_events == 0),
+                "wekws_threshold_spot: null argument");
+  const long long total = (long long)B * K;
+  const int nt = 128;
+  threshold_spot_kernel<<<(unsigned)((total + nt - 1) / nt), nt, 0, (cudaStream_t)stream>>>(
+      d_probs, K, d_rows, d_frames, B, d_thresholds, window_shift, (ThresholdState*)d_state, max_events, d_counts,
+      d_events);
+  return check_launch("threshold_spot_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------------
