@@ -590,7 +590,9 @@ WEKWS_API int wekws_criterion_ctc_backward(const float* d_logits, const int32_t*
  *   added in order.  Backward workspace 32 * 128 hdim + 16 B T hdim + 8 (sum of Z N (Q + 1) over the weights,
  *   + 128 hdim (K + 1) per ds block) bytes; 4 + 2 L (dense) or 4 + 3 L (ds) launches.
  *
- * FSMN (an fsmn_ctc.yaml model, wekws/model/fsmn.py FSMN): every FSMN config, with the identity activation.
+ * FSMN (an fsmn_ctc.yaml model, wekws/model/fsmn.py FSMN): every FSMN config with at most 32 memory taps
+ * (left_order + right_order; the backward keeps one register per tap), with the identity activation.  The three entry
+ * points refuse a model with more taps before any launch; wekws_model_forward runs it.
  *   h_params: 8 + 5 L, state_dict order (the model's parameters without the CMVN buffers):
  *     backbone.in_linear1.linear.{weight,bias}, backbone.in_linear2.linear.{weight,bias},
  *     per layer l: backbone.fsmn.{l}.0.linear.weight, .1.conv_left.weight, .1.conv_right.weight,

@@ -1,6 +1,6 @@
 """Every backbone kernel across the model configurations it accepts, not only the shipped recipe shapes.
 
-ROWS below lists about thirty configurations.  Each sits on a kernel variant no recipe reaches (one A atom, 17 MDTC
+ROWS below lists about fifty configurations.  Each sits on a kernel variant no recipe reaches (one A atom, 17 MDTC
 blocks, generic DS-TCN cache pitch, one-layer GRU, ...) or one step past an eligibility edge, and names the kernel a
 large-batch call with T >= 8 takes:
 
@@ -8,6 +8,7 @@ large-batch call with T >= 8 takes:
     DsTcn+linear_tc       the DS-TCN kernel with the classifier as its own tensor-core GEMM (output_dim > 4)
     Gru                   the tensor-core GRU (batch thresholds under "auto", always under "tensor")
     fp32                  the FP32 kernels only (conv_backbone.cu, gru.cu)
+    Fsmn                  the fused FP32 FSMN kernel (fsmn.cu), the only one that model has
 
 Without a GPU: the kernel choice (a tensor-core model packs a weight image), the packed FP32 weights against the oracle,
 and the oracle against the reference (live when its sources are present, else tests/golden/config_sweep.npz, made by
@@ -29,10 +30,15 @@ from tests.conftest import golden, have_reference, reference_init_model
 from wekws_b200 import init_model, synth
 from wekws_b200.configs import model_config
 
-# (id, recipe, overrides, kernel).  Overrides: model_config arguments (input_dim, output_dim, activation, cmvn),
-# backbone fields (num_stack, stack_size, kernel_size, num_layers), hidden_dim, head ("global" / "last").  Hidden 64 for
-# MDTC and TCN, 256 for DS-TCN, 128 for GRU unless given; output_dim 1 unless given.  The rows output logits (activation
-# identity) unless they ask for the sigmoid: a saturated sigmoid would hide differences the gates must see.
+# (id, recipe, overrides, kernel).  Overrides: model_config arguments (input_dim, output_dim, activation, cmvn,
+# norm_var), backbone fields (num_stack, stack_size, kernel_size, num_layers and FSMN_FIELDS), hidden_dim, head
+# ("global" / "last").  Hidden 64 for MDTC and TCN, 256 for DS-TCN, 128 for GRU unless given; output_dim 1 unless given.
+# The rows output logits (activation identity) unless they ask for the sigmoid: a saturated sigmoid would hide
+# differences the gates must see.
+FSMN_FIELDS = ("input_affine_dim", "linear_dim", "proj_dim", "output_affine_dim", "left_order", "right_order",
+               "left_stride", "right_stride")
+FSMN_SMALL = dict(input_dim=40, output_dim=7, input_affine_dim=24, linear_dim=36, proj_dim=16, output_affine_dim=20,
+                  num_layers=3, left_order=10, right_order=2)
 ROWS = [
     # MDTC tensor-core kernel: kernel 5, stack_size <= 4, <= 17 blocks, input_dim % 8 == 0 and <= 96, output_dim <= 8
     ("mdtc_1x1_i40_o3", "mdtc", dict(num_stack=1, stack_size=1, input_dim=40, output_dim=3, activation="sigmoid"),
@@ -78,13 +84,29 @@ ROWS = [
     ("gru_3l", "gru", dict(num_layers=3), "fp32"),
     ("gru_4l", "gru", dict(num_layers=4), "fp32"),
     ("gru_i97", "gru", dict(input_dim=97), "fp32"),
+    # FSMN kernel (fsmn.cu, FP32 only): widths input_affine / linear / proj / output_affine 24 / 36 / 16 / 20, 3 layers,
+    # orders 10 / 2, input 40, output 7 unless given (FSMN_SMALL); cache (B, proj, left_order - 1 + right_order, layers)
+    ("fsmn_l1_r1", "fsmn", dict(FSMN_SMALL, left_order=1, right_order=1, num_layers=1), "Fsmn"),     # cache of 1
+    ("fsmn_l1_r5", "fsmn", dict(FSMN_SMALL, left_order=1, right_order=5), "Fsmn"),                  # right taps only
+    ("fsmn_l20_r12", "fsmn", dict(FSMN_SMALL, left_order=20, right_order=12), "Fsmn"),  # 32 taps: the backward's limit
+    ("fsmn_l60_r20", "fsmn", dict(FSMN_SMALL, left_order=60, right_order=20), "Fsmn"),  # cache of 79 > a 64-row tile
+    ("fsmn_odd_cmvn", "fsmn", dict(FSMN_SMALL, input_dim=13, input_affine_dim=7, linear_dim=33, proj_dim=5,
+                                   output_affine_dim=9, output_dim=1, cmvn=True, norm_var=False), "Fsmn"),  # K tails 1, 3
+    ("fsmn_wide", "fsmn", dict(FSMN_SMALL, input_dim=80, input_affine_dim=129, linear_dim=257, proj_dim=129,
+                               output_affine_dim=129, output_dim=129), "Fsmn"),              # two 128-column passes
+    ("fsmn_16l", "fsmn", dict(FSMN_SMALL, num_layers=16), "Fsmn"),                          # the pack's layer limit
+    ("fsmn_sigmoid_o2", "fsmn", dict(FSMN_SMALL, output_dim=2, activation="sigmoid"), "Fsmn"),
+    ("fsmn_strided", "fsmn", dict(FSMN_SMALL, left_order=4, right_order=1, left_stride=2, right_stride=3),
+     "Fsmn"),                                                                  # cache 4, FSMN.padding 9
+    ("fsmn_shipped", "fsmn", dict(input_dim=400, output_dim=2599), "Fsmn"),                 # fsmn_ctc.yaml
 ]
 ROW_IDS = [r[0] for r in ROWS]
 _ROW = {r[0]: r for r in ROWS}
 TENSOR_CORE = ("Mdtc", "Tcn", "DsTcn", "DsTcn+linear_tc", "Gru")
 
 # the rows the reference golden covers (oracle/make_sweep_golden.py) and its inputs
-GOLDEN_ROWS = ["tcn_k3x5_i40_o8", "tcn_k8x7", "dstcn_5l_o5", "mdtc_1x1_i40_o3", "gru_1l_i40", "gru_3l"]
+GOLDEN_ROWS = ["tcn_k3x5_i40_o8", "tcn_k8x7", "dstcn_5l_o5", "mdtc_1x1_i40_o3", "gru_1l_i40", "gru_3l", "fsmn_l1_r5",
+               "fsmn_l20_r12"]
 GOLDEN_B, GOLDEN_T = 2, (98, 9)      # a 1 s clip from a random cache, then 9 frames with the cache carried
 
 # A DS-TCN with 6 layers packs, but the FP32 conv kernel every conv model keeps cannot hold one frame of it
@@ -110,11 +132,15 @@ def row_config(row_id):
 def _config(name, ov):
     ov = dict(ov)
     ov.setdefault("activation", "identity")
-    bb_keys = {k: ov.pop(k) for k in ("num_stack", "stack_size", "kernel_size", "num_layers") if k in ov}
+    bb_keys = {k: ov.pop(k) for k in ("num_stack", "stack_size", "kernel_size", "num_layers") + FSMN_FIELDS if k in ov}
     hidden, head = ov.pop("hidden_dim", None), ov.pop("head", None)
     cmvn_file = synth.write_cmvn_json(ov.get("input_dim", 80)) if ov.pop("cmvn", False) else None
     cfg = model_config(name, cmvn_file=cmvn_file, **ov)
     cfg["backbone"].update(bb_keys)
+    if name == "fsmn" and ov["activation"] == "sigmoid":
+        # the config grammar gives an FSMN model (classifier 'identity') the Identity activation only: build_config
+        # sets the Sigmoid module, and the oracle reads the missing key as the Sigmoid
+        del cfg["activation"]
     if hidden is not None:
         cfg["hidden_dim"] = hidden
         if name.startswith("mdtc"):
@@ -139,6 +165,8 @@ def build_config(name, ov, factory, seed=777):
             model = factory(cfg)
     finally:
         cleanup()
+    if cfg["backbone"]["type"] == "fsmn" and "activation" not in cfg:
+        model.activation = torch.nn.Sigmoid()
     synth.randomize_(model, seed=seed)
     model.eval()
     return cfg, model
@@ -148,6 +176,8 @@ def cache_shape(cfg, B):
     bb = cfg["backbone"]
     if bb["type"] == "gru":
         return (bb["num_layers"], B, cfg["hidden_dim"])
+    if bb["type"] == "fsmn":              # the blocks run with strides 1 whatever the config says: no FSMN.padding
+        return (B, bb["proj_dim"], bb["left_order"] - 1 + bb["right_order"], bb["num_layers"])
     return (B, cfg["hidden_dim"], O.backbone_padding(cfg))
 
 
@@ -187,7 +217,7 @@ def test_kernel_choice_is_pinned_by_the_pack(row, native):
     assert has_image == (expected(row) in TENSOR_CORE), (row, expected(row))
 
 
-@pytest.mark.parametrize("row", [r for r in ROW_IDS if "head" not in _ROW[r][2]])
+@pytest.mark.parametrize("row", [r for r in ROW_IDS if "head" not in _ROW[r][2] and kind(r) != "fsmn"])
 def test_fold_and_pack_reproduce_the_oracle(row, native):
     """The packed FP32 weight stream (BN folded, every kernel's source), evaluated with plain torch ops, against the
     oracle with a random cache."""
@@ -289,6 +319,8 @@ _BOLD_T = [1, 7, 8, 40, 56, 57, 98, 120, 121, 125, 128, 250]   # around the 56- 
 def _times(row):
     if row in ("tcn_k8x7", "tcn_k4x8"):
         return _BOLD_T
+    if expected(row) == "Fsmn":        # 64-row tiles: 1 .. 64 streams per tile, then 2 and 3 host chunks (33 + 32, 3 x 43)
+        return [1, 7, 8, 21, 33, 40, 63, 64, 65, 129]
     extra = {"Mdtc": [129, 257], "Tcn": [129, 257], "DsTcn": [121], "DsTcn+linear_tc": [121], "Gru": [129],
              "fp32": [300]}[expected(row)]
     return [1, 7, 8, 40] + extra
@@ -436,7 +468,7 @@ def test_gpu_misaligned_inputs_fall_back_to_fp32(row, sweep_models):
 @pytest.mark.gpu
 @pytest.mark.parametrize("T", [40, 200])
 @pytest.mark.parametrize("row", ["mdtc_1x1_i40_o3", "tcn_k3x5_i40_o8", "dstcn_3l_i40_o4", "dstcn_5l_o5",
-                                 "dstcn_1l", "gru_1l_i40"])
+                                 "dstcn_1l", "gru_1l_i40", "fsmn_l60_r20"])
 def test_gpu_in_place_cache_through_the_c_abi(row, T, sweep_models, native):
     """wekws_model_forward with d_in_cache == d_out_cache (what the native runtime shim does) for 300 streams equals
     the call with separate buffers bit for bit."""

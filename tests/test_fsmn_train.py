@@ -7,7 +7,9 @@ import torch
 from oracle import kws_criterion_grad_oracle as KG
 from oracle import kws_criterion_oracle as K
 from oracle import kws_fsmn_train_oracle as KF
+from oracle import kws_head_oracle as HO
 from tests.cases import fsmn_config
+from tests.test_config_sweep import FSMN_SMALL, build_config, build_row, inputs
 from tests.test_fsmn_train_host import (GOLDEN, NAMES, assert_within_rule, golden_feats, golden_grads, golden_model,
                                         golden_up)
 from wekws_b200 import _native, criterion, init_model, model_config
@@ -193,3 +195,37 @@ def test_refusals():
         other = init_model(model_config(name)).to(DEV).train()
         with pytest.raises(RuntimeError, match="inference-only"):
             other(torch.randn(1, 8, 80, device=DEV))
+
+
+def test_33_taps_are_refused_before_any_launch_and_still_run_in_eval():
+    """An FSMN with 21 + 12 memory taps, one more than the backward's memory kernel holds: a training-mode forward with
+    grad raises, naming the taps, before its parameter pack or forward launches; the eval forward runs it."""
+    cfg, model = build_config("fsmn", dict(FSMN_SMALL, left_order=21, right_order=12), init_model)
+    sd64 = {k: v.double() for k, v in model.state_dict().items()}
+    model = model.to(DEV)
+    x, cache = inputs(cfg, 5, 40, seed=33)
+    y, c = model(x.to(DEV), cache.to(DEV))
+    y_ref, c_ref = HO.kws_forward(sd64, cfg, x.double(), cache.double())
+    assert float((y.cpu().double() - y_ref).abs().max()) <= 2e-5 * max(1.0, float(y_ref.abs().max()))
+    assert float((c.cpu().double() - c_ref).abs().max()) <= 2e-5 * max(1.0, float(c_ref.abs().max()))
+    torch.cuda.synchronize()
+    n0 = _native.launch_count()
+    with pytest.raises(RuntimeError, match=r"at most 32 memory taps \(left_order \+ right_order\), this one has 21 \+ 12"):
+        model.train()(x.to(DEV))
+    torch.cuda.synchronize()
+    assert _native.launch_count() == n0
+
+
+def test_32_taps_gradients_against_oracle():
+    """The backward's memory kernel with every tap register in use (20 + 12 taps): one training step's gradients
+    against the float64 oracle, under the rule the golden cases are held to."""
+    cfg, model = build_row("fsmn_l20_r12", init_model)
+    sd = {k: v.clone() for k, v in model.state_dict().items()}
+    gen = torch.Generator().manual_seed(32)
+    feats = torch.randn(8, 100, cfg["input_dim"], generator=gen)
+    up = torch.randn(8, 100, cfg["output_dim"], generator=gen)
+    _, g32 = KF.fsmn_grads(sd, cfg, feats, up, torch.float32)
+    _, g64 = KF.fsmn_grads(sd, cfg, feats, up, torch.float64)
+    _, _, grads = train_step(model.to(DEV), feats.to(DEV), up.to(DEV))
+    err32 = [float((a.double() - b).abs().max()) for a, b in zip(g32, g64)]
+    assert_within_rule(grads, g64, err32, "fsmn_l20_r12")

@@ -150,6 +150,37 @@ def test_training_entry_point_refusals_without_a_device():
         lib.wekws_model_destroy(hm)
 
 
+def taps_config(left_order, right_order):
+    cfg = fsmn_config("fsmn")
+    cfg["backbone"].update(left_order=left_order, right_order=right_order)
+    return cfg
+
+
+def test_more_taps_than_the_backward_holds_are_refused_by_every_training_entry_point():
+    """The backward's memory kernel keeps one register per tap (32).  A 33-tap model is refused by the parameter
+    pack, the training forward and the backward alike, naming the taps, before they look at anything else; a 32-tap
+    model passes that check (and stops at the next: this handle is not finalized)."""
+    lib = _native.lib()
+    for lo, ro in ((21, 12), (1, 32), (60, 20)):
+        _, h = native_model(taps_config(lo, ro))
+        try:
+            n = lib.wekws_train_num_params(h)
+            assert lib.wekws_model_load_params(h, (C.c_void_p * n)(), n, None) < 0
+            assert f"at most 32 memory taps (left_order + right_order), this one has {lo} + {ro}" in _native.last_error()
+            assert lib.wekws_model_train_forward(h, None, None, None, None, 2, 3, None) < 0
+            assert "wekws_model_train_forward: the FSMN model trains with at most 32" in _native.last_error()
+            assert lib.wekws_model_backward(h, None, None, None, None, 2, 3, None, n, None, None) < 0
+            assert "wekws_model_backward: the FSMN model trains with at most 32" in _native.last_error()
+        finally:
+            lib.wekws_model_destroy(h)
+    _, h = native_model(taps_config(20, 12))
+    try:
+        assert lib.wekws_model_load_params(h, (C.c_void_p * 23)(), 23, None) == -3
+        assert "finalize" in _native.last_error()
+    finally:
+        lib.wekws_model_destroy(h)
+
+
 @pytest.mark.parametrize("name", ["mdtc", "tcn", "ds_tcn", "gru"])
 def test_other_backbones_keep_refusing_training(name):
     model = init_model(model_config(name)).train()

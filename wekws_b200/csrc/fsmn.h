@@ -50,6 +50,7 @@ int fsmn_train_launch(FsmnArgs a, cudaStream_t st);    // fsmn_launch that also 
 
 // fsmn_grad.cu -------------------------------------------------------------------------------------------------------
 constexpr int FSMN_MAX_LAYERS = 16;
+constexpr int FSMN_MAX_TAPS = 32;                          // lorder + rorder: one register per tap in the memory kernel
 constexpr int FSMN_MAX_PARAMS = 8 + 5 * FSMN_MAX_LAYERS;   // parameters of an FSMN of L layers: 8 + 5 L
 constexpr int FSMN_GRAD_SLICES = 32;                       // row slices of every weight-gradient reduction
 

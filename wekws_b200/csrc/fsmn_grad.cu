@@ -36,7 +36,7 @@ __global__ void fsmn_pack_kernel(const FsmnPackArgs a) {
 // CTA = 32 channels x 8 row groups over one of the FSMN_GRAD_SLICES row slices; each row group sums its contiguous
 // share of the slice in row order, the eight are added in group order: the tap partials of the slice, in the
 // parameters' [proj][order] layout.
-constexpr int MB_C = 32, MB_R = 8, MAX_TAPS = 32;
+constexpr int MB_C = 32, MB_R = 8;
 
 struct MemArgs {
   const float* G; const float* p; const float* taps;   // taps: the pack's [lo + ro][P]
@@ -45,16 +45,16 @@ struct MemArgs {
 };
 
 __global__ void __launch_bounds__(MB_C * MB_R) fsmn_grad_memory_kernel(const MemArgs a) {
-  __shared__ float red[MB_R][MB_C][MAX_TAPS + 1];
+  __shared__ float red[MB_R][MB_C][FSMN_MAX_TAPS + 1];
   const int cl = threadIdx.x & (MB_C - 1), rg = threadIdx.x / MB_C;
   const int c = blockIdx.x * MB_C + cl;
   const int lo = a.lo, ro = a.ro, pad = lo - 1 + ro, ntap = lo + ro, T = a.T, P = a.P;
   const int s_begin = blockIdx.y * a.rslice, s_end = min(a.M, s_begin + a.rslice);
   const int per = (a.rslice + MB_R - 1) / MB_R;
   const int r_begin = s_begin + rg * per, r_end = min(s_end, r_begin + per);
-  float acc[MAX_TAPS];
+  float acc[FSMN_MAX_TAPS];
 #pragma unroll
-  for (int i = 0; i < MAX_TAPS; ++i) acc[i] = 0.f;
+  for (int i = 0; i < FSMN_MAX_TAPS; ++i) acc[i] = 0.f;
   if (c < P) {
     for (int r = r_begin; r < r_end; ++r) {
       const int t = r % T, base = r - t;
@@ -66,12 +66,12 @@ __global__ void __launch_bounds__(MB_C * MB_R) fsmn_grad_memory_kernel(const Mem
       a.dp[(long long)r * P + c] = d;
       const float g = G(t);
 #pragma unroll
-      for (int i = 0; i < MAX_TAPS; ++i)
+      for (int i = 0; i < FSMN_MAX_TAPS; ++i)
         if (i < ntap) acc[i] = fmaf(g, pv(t + i - pad), acc[i]);   // cat[t + i], left taps then right
     }
   }
 #pragma unroll
-  for (int i = 0; i < MAX_TAPS; ++i)
+  for (int i = 0; i < FSMN_MAX_TAPS; ++i)
     if (i < ntap) red[rg][cl][i] = acc[i];
   __syncthreads();
   // thread (cl, rg) adds the eight groups' sums of taps rg, rg + 8, ... in group order
@@ -142,7 +142,7 @@ long long fsmn_backward_workspace_floats(const FsmnArgs& a, long long M) {
 int fsmn_backward_launch(const FsmnArgs& a, const float* feats, const float* saved, const float* grad_out, int B, int T,
                          float* const* grads, float* ws, cudaStream_t st) {
   const long long M = (long long)B * T;
-  WEKWS_REQUIRE(a.L >= 1 && a.L <= FSMN_MAX_LAYERS && a.lorder + a.rorder <= MAX_TAPS,
+  WEKWS_REQUIRE(a.L >= 1 && a.L <= FSMN_MAX_LAYERS && a.lorder + a.rorder <= FSMN_MAX_TAPS,
                 "fsmn backward: %d layers, %d + %d taps unsupported", a.L, a.lorder, a.rorder);
   WEKWS_REQUIRE(M >= 1 && M < (1LL << 31) / max_width(a), "fsmn backward: %lld frames unsupported", M);
   const int nparam = 8 + 5 * a.L;

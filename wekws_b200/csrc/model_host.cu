@@ -1015,12 +1015,17 @@ int batch_stats_model(const wekws_model* m, const char* what, TrainModel* t) {
   return WEKWS_OK;
 }
 
-// A model for wekws_model_load_params / _train_forward / _backward: FSMN or GRU, finalized on the current device.
+// A model for wekws_model_load_params / _train_forward / _backward: FSMN (at most FSMN_MAX_TAPS memory taps) or GRU,
+// finalized on the current device.
 int packed_model(const wekws_model* m, const char* what, TrainModel* t) {
   int rc = train_model(m, what, t);
   if (rc) return rc;
   WEKWS_REQUIRE(!batch_stats(t->fam), "%s: the %s model takes its parameters with each call, through "
                 "wekws_train_forward / wekws_train_backward", what, train_label(t->fam));
+  // the backward's memory kernel keeps one register per tap; inference takes any order
+  WEKWS_REQUIRE(t->fam != TrainFamily::Fsmn || m->cfg.fsmn_left_order + m->cfg.fsmn_right_order <= FSMN_MAX_TAPS,
+                "%s: the FSMN model trains with at most %d memory taps (left_order + right_order), this one has "
+                "%d + %d taps", what, FSMN_MAX_TAPS, m->cfg.fsmn_left_order, m->cfg.fsmn_right_order);
   if (!m->finalized) { set_error("%s called before wekws_model_finalize", what); return WEKWS_ERR_STATE; }
   WEKWS_REQUIRE(t->fam != TrainFamily::Fsmn || m->cfg.activation == WEKWS_ACT_IDENTITY,
                 "%s: the FSMN model trains with the identity activation", what);
