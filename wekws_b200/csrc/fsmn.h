@@ -55,7 +55,9 @@ constexpr int FSMN_MAX_PARAMS = 8 + 5 * FSMN_MAX_LAYERS;   // parameters of an F
 constexpr int FSMN_GRAD_SLICES = 32;                       // row slices of every weight-gradient reduction
 
 // One parameter tensor of the state_dict: src viewed as [rows][cols] lands transposed at packed[dst + c * ld + r]
-// (a Linear weight [N][K] -> W^T [K][Npad]; a bias: cols 1; a tap bank [proj][order] -> [order][proj]).
+// (a Linear weight [N][K] -> W^T [K][Npad]; a bias: cols 1; a tap bank [proj][order] -> [order][proj]).  The host
+// pack of the FSMN and GRU models (model_host.cu place) writes every parameter by this rule and keeps each one's
+// dst, rows, cols and ld, so the device pack of wekws_model_load_params reuses the host's layout.
 struct FsmnParamCopy {
   const float* src;
   long long dst;

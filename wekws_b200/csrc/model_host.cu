@@ -97,6 +97,14 @@ struct Folded {           // BN as per-channel scale/shift
 
 enum class TcKernel { None, Mdtc, Tcn, DsTcn, Gru };   // the tensor-core kernel a model has, if any
 
+// Where one state_dict tensor sits in h_vec: `name` viewed as [rows][cols] lands transposed at h_vec[dst + c * ld + r],
+// the meaning of FsmnParamCopy (fsmn.h) without its source pointer.
+struct PackedParam {
+  std::string name;
+  long long dst;
+  int rows, cols, ld;
+};
+
 }  // namespace
 }  // namespace wekws
 
@@ -140,6 +148,9 @@ struct wekws_model {
   int v_w0 = 0, v_b0 = 0, v_w1 = 0, v_b1 = 0;   // the head's MLP in h_vec (pack_head)
   float* d_pool = nullptr;                  // (B, hdim) pooled backbone output between the two kernels; grows monotonically
   size_t pool_cap = 0;
+  // FSMN and GRU: every trainable parameter's place in h_vec, in wekws_train_num_params order (FSMN: state_dict,
+  // GRU: named_parameters), which wekws_model_load_params packs on the device; empty for the other backbones
+  std::vector<PackedParam> params;
 };
 
 namespace {
@@ -178,6 +189,28 @@ int fold_bn(const wekws_model* m, const std::string& p, int C, Folded* f) {
 
 size_t pad4(size_t n) { return (n + 3) & ~(size_t)3; }
 
+// Appends a zero-filled block of n floats to h_vec; returns where it starts.
+int new_block(wekws_model* m, size_t n) {
+  const size_t off = m->h_vec.size();
+  m->h_vec.resize(off + n, 0.f);
+  return (int)off;
+}
+
+// Copies the state_dict tensor `name`, viewed as [rows][cols], to h_vec[dst + c * ld + r] inside a block the caller
+// has made, and appends its entry to `table` (nullptr: the model does not train on its pack).  This is what
+// fsmn_pack_kernel does with the same entry on the device.
+int place(wekws_model* m, std::vector<PackedParam>* table, const std::string& name, int rows, int cols, long long dst,
+          int ld) {
+  GET(src, name, (size_t)rows * cols);
+  for (int r = 0; r < rows; ++r)
+    for (int c = 0; c < cols; ++c) m->h_vec[dst + (long long)c * ld + r] = src[(size_t)r * cols + c];
+  if (table) table->push_back({name, dst, rows, cols, ld});
+  return WEKWS_OK;
+}
+
+#define PLACE(table, name, rows, cols, dst, ld)                                              \
+  do { int _rc = place(m, (table), (name), (rows), (cols), (dst), (ld)); if (_rc) return _rc; } while (0)
+
 // Appends W^T (K x C, from W[o][c] * s[o] with arbitrary source strides) as row chunks.
 void push_gemm(wekws_model* m, int K, int C, const float* W, size_t o_stride, size_t c_stride, const double* s) {
   const int KC = conv_chunk_rows(C);
@@ -212,40 +245,27 @@ int pack_common_front(wekws_model* m, int* v_mean, int* v_istd) {
   return WEKWS_OK;
 }
 
-int pack_classifier(wekws_model* m, int H, int* v_wc, int* v_bc) {
+// the per-frame classifier: W_c^T [H][odim], b_c
+int pack_classifier(wekws_model* m, std::vector<PackedParam>* table, int H, int* v_wc, int* v_bc) {
   const int odim = m->cfg.odim;
-  GET(wc, "classifier.linear.weight", (size_t)odim * H);
-  GET(bc, "classifier.linear.bias", (size_t)odim);
-  *v_wc = (int)m->h_vec.size();
-  m->h_vec.resize(m->h_vec.size() + pad4((size_t)H * odim), 0.f);
-  for (int c = 0; c < H; ++c)
-    for (int j = 0; j < odim; ++j) m->h_vec[*v_wc + c * odim + j] = wc[j * H + c];
-  *v_bc = (int)m->h_vec.size();
-  m->h_vec.resize(m->h_vec.size() + pad4(odim), 0.f);
-  for (int j = 0; j < odim; ++j) m->h_vec[*v_bc + j] = bc[j];
+  *v_wc = new_block(m, pad4((size_t)H * odim));
+  *v_bc = new_block(m, pad4(odim));
+  PLACE(table, "classifier.linear.weight", odim, H, *v_wc, odim);
+  PLACE(table, "classifier.linear.bias", odim, 1, *v_bc, 1);
   return WEKWS_OK;
 }
 
 // Utterance-level head (classifier.py:19-40 around kws_model.py:180-182): W0^T [H][64], b0, W1^T [64][odim], b1
 int pack_head(wekws_model* m, int H) {
   const int odim = m->cfg.odim, W = kHeadWidth;
-  GET(w0, "classifier.classifier.0.weight", (size_t)W * H);
-  GET(b0, "classifier.classifier.0.bias", (size_t)W);
-  GET(w1, "classifier.classifier.3.weight", (size_t)odim * W);
-  GET(b1, "classifier.classifier.3.bias", (size_t)odim);
-  m->v_w0 = (int)m->h_vec.size();
-  m->h_vec.resize(m->h_vec.size() + pad4((size_t)H * W), 0.f);
-  for (int c = 0; c < H; ++c)
-    for (int j = 0; j < W; ++j) m->h_vec[m->v_w0 + c * W + j] = w0[j * H + c];
-  m->v_b0 = (int)m->h_vec.size();
-  m->h_vec.insert(m->h_vec.end(), b0, b0 + W);
-  m->v_w1 = (int)m->h_vec.size();
-  m->h_vec.resize(m->h_vec.size() + pad4((size_t)W * odim), 0.f);
-  for (int k = 0; k < W; ++k)
-    for (int j = 0; j < odim; ++j) m->h_vec[m->v_w1 + k * odim + j] = w1[j * W + k];
-  m->v_b1 = (int)m->h_vec.size();
-  m->h_vec.resize(m->h_vec.size() + pad4(odim), 0.f);
-  for (int j = 0; j < odim; ++j) m->h_vec[m->v_b1 + j] = b1[j];
+  m->v_w0 = new_block(m, pad4((size_t)H * W));
+  m->v_b0 = new_block(m, W);
+  m->v_w1 = new_block(m, pad4((size_t)W * odim));
+  m->v_b1 = new_block(m, pad4(odim));
+  PLACE(nullptr, "classifier.classifier.0.weight", W, H, m->v_w0, W);
+  PLACE(nullptr, "classifier.classifier.0.bias", W, 1, m->v_b0, 1);
+  PLACE(nullptr, "classifier.classifier.3.weight", odim, W, m->v_w1, odim);
+  PLACE(nullptr, "classifier.classifier.3.bias", odim, 1, m->v_b1, 1);
   return WEKWS_OK;
 }
 
@@ -438,7 +458,7 @@ int pack_conv(wekws_model* m) {
   }
   if (m->head != WEKWS_HEAD_LINEAR) {
     if ((rc = pack_head(m, C))) return rc;
-  } else if ((rc = pack_classifier(m, C, &a.v_wc, &a.v_bc))) {
+  } else if ((rc = pack_classifier(m, nullptr, C, &a.v_wc, &a.v_bc))) {
     return rc;
   }
   m->h_chunk_off.push_back((int)m->h_stream.size());
@@ -463,34 +483,29 @@ int pack_gru(wekws_model* m) {
   memset(&a, 0, sizeof(a));
   int rc = pack_common_front(m, &a.v_mean, &a.v_istd);
   if (rc) return rc;
-  GET(wp, "preprocessing.out.0.weight", (size_t)H * idim);
-  GET(bp, "preprocessing.out.0.bias", (size_t)H);
-  a.v_wp = (int)m->h_vec.size();
-  for (int k = 0; k < idim; ++k)
-    for (int j = 0; j < H; ++j) m->h_vec.push_back(wp[j * idim + k]);
-  a.v_bp = (int)m->h_vec.size();
-  m->h_vec.insert(m->h_vec.end(), bp, bp + H);
+  std::vector<PackedParam>* tab = &m->params;
+  a.v_wp = new_block(m, (size_t)idim * H);
+  a.v_bp = new_block(m, H);
+  PLACE(tab, "preprocessing.out.0.weight", H, idim, a.v_wp, H);
+  PLACE(tab, "preprocessing.out.0.bias", H, 1, a.v_bp, 1);
   a.v_layers = (int)m->h_vec.size();
   a.v_layer_stride = 2 * H * G + 2 * G;
   for (int l = 0; l < L; ++l) {
     const std::string sfx = "_l" + std::to_string(l);
-    GET(wih, "backbone.weight_ih" + sfx, (size_t)G * H);
-    GET(whh, "backbone.weight_hh" + sfx, (size_t)G * H);
-    GET(bih, "backbone.bias_ih" + sfx, (size_t)G);
-    GET(bhh, "backbone.bias_hh" + sfx, (size_t)G);
-    for (int k = 0; k < H; ++k) {            // row k: [W_ih[:, k] | W_hh[:, k]]  (768 floats, streamed by TMA)
-      for (int g = 0; g < G; ++g) m->h_vec.push_back(wih[g * H + k]);
-      for (int g = 0; g < G; ++g) m->h_vec.push_back(whh[g * H + k]);
-    }
-    m->h_vec.insert(m->h_vec.end(), bih, bih + G);
-    m->h_vec.insert(m->h_vec.end(), bhh, bhh + G);
+    // row k: [W_ih[:, k] | W_hh[:, k]]  (768 floats, streamed by TMA), then b_ih, b_hh
+    const long long base = new_block(m, a.v_layer_stride);
+    PLACE(tab, "backbone.weight_ih" + sfx, G, H, base, 2 * G);
+    PLACE(tab, "backbone.weight_hh" + sfx, G, H, base + G, 2 * G);
+    PLACE(tab, "backbone.bias_ih" + sfx, G, 1, base + 2LL * H * G, 1);
+    PLACE(tab, "backbone.bias_hh" + sfx, G, 1, base + 2LL * H * G + G, 1);
   }
-  if ((rc = pack_classifier(m, H, &a.v_wc, &a.v_bc))) return rc;
+  if ((rc = pack_classifier(m, tab, H, &a.v_wc, &a.v_bc))) return rc;
   a.L = L; a.H = H; a.idim = idim; a.odim = c.odim; a.act = c.activation; a.has_cmvn = m->has_cmvn ? 1 : 0;
   // tensor-core variant: the per-step weight stream as pre-swizzled bf16 hi|lo operand chunks
   m->tc = TcKernel::None;
   m->h_wimg.clear();
   if (gru_tc_eligible(L, H, idim)) {
+    GET(wp, "preprocessing.out.0.weight", (size_t)H * idim);
     const float* wih[4];
     const float* whh[4];
     for (int l = 0; l < L; ++l) {
@@ -529,55 +544,38 @@ int pack_fsmn(wekws_model* m) {
   if (rc) return rc;
   const int NP = fsmn_pass_cols();
   auto npad = [&](int n) { return (n + NP - 1) / NP * NP; };
-  auto push_wt = [&](const float* W, int N, int K, int* off) {      // W[n][k] -> W^T [K][npad(N)]
-    *off = (int)m->h_vec.size();
-    const int np = npad(N);
-    m->h_vec.resize(m->h_vec.size() + (size_t)K * np, 0.f);
-    for (int k = 0; k < K; ++k)
-      for (int n = 0; n < N; ++n) m->h_vec[*off + (size_t)k * np + n] = W[(size_t)n * K + k];
+  std::vector<PackedParam>* tab = &m->params;
+  // the state_dict Linear `p` ([N][K], with its bias [N] unless o_b is null) -> W^T [K][npad(N)] at o_w, b at o_b
+  auto push_linear = [&](const std::string& p, int N, int K, int* o_w, int* o_b) -> int {
+    *o_w = new_block(m, (size_t)K * npad(N));
+    PLACE(tab, p + ".weight", N, K, *o_w, npad(N));
+    if (o_b) {
+      *o_b = new_block(m, npad(N));
+      PLACE(tab, p + ".bias", N, 1, *o_b, 1);
+    }
+    return WEKWS_OK;
   };
-  auto push_b = [&](const float* b, int N, int* off) {
-    *off = (int)m->h_vec.size();
-    m->h_vec.resize(m->h_vec.size() + npad(N), 0.f);
-    for (int n = 0; n < N; ++n) m->h_vec[*off + n] = b[n];
-  };
-  GET(w1, "backbone.in_linear1.linear.weight", (size_t)A1 * idim);
-  GET(b1, "backbone.in_linear1.linear.bias", (size_t)A1);
-  GET(w2, "backbone.in_linear2.linear.weight", (size_t)D * A1);
-  GET(b2, "backbone.in_linear2.linear.bias", (size_t)D);
-  push_wt(w1, A1, idim, &a.o_w_in1); push_b(b1, A1, &a.o_b_in1);
-  push_wt(w2, D, A1, &a.o_w_in2); push_b(b2, D, &a.o_b_in2);
+  if ((rc = push_linear("backbone.in_linear1.linear", A1, idim, &a.o_w_in1, &a.o_b_in1)) ||
+      (rc = push_linear("backbone.in_linear2.linear", D, A1, &a.o_w_in2, &a.o_b_in2)))
+    return rc;
   a.o_layers = (int)m->h_vec.size();
   for (int l = 0; l < L; ++l) {
     const std::string p = "backbone.fsmn." + std::to_string(l) + ".";
-    GET(wp, p + "0.linear.weight", (size_t)P * D);
-    GET(wl, p + "1.conv_left.weight", (size_t)P * lo);
-    GET(wr, p + "1.conv_right.weight", (size_t)P * ro);
-    GET(wa, p + "2.linear.weight", (size_t)D * P);
-    GET(ba, p + "2.linear.bias", (size_t)D);
     const int base = (int)m->h_vec.size();
-    int off;
-    push_wt(wp, P, D, &off);
-    if (l == 0) a.lo_wp = off - base;
-    off = (int)m->h_vec.size();
-    if (l == 0) a.lo_taps = off - base;
-    m->h_vec.resize(m->h_vec.size() + pad4((size_t)(lo + ro) * P), 0.f);
-    for (int i = 0; i < lo; ++i)
-      for (int ch = 0; ch < P; ++ch) m->h_vec[off + (size_t)i * P + ch] = wl[(size_t)ch * lo + i];
-    for (int j = 0; j < ro; ++j)
-      for (int ch = 0; ch < P; ++ch) m->h_vec[off + (size_t)(lo + j) * P + ch] = wr[(size_t)ch * ro + j];
-    push_wt(wa, D, P, &off);
-    if (l == 0) a.lo_wa = off - base;
-    push_b(ba, D, &off);
-    if (l == 0) a.lo_ba = off - base;
-    if (l == 0) a.layer_stride = (int)m->h_vec.size() - base;
+    int o_wp, o_wa, o_ba;
+    if ((rc = push_linear(p + "0.linear", P, D, &o_wp, nullptr))) return rc;
+    const int o_taps = new_block(m, pad4((size_t)(lo + ro) * P));
+    PLACE(tab, p + "1.conv_left.weight", P, lo, o_taps, P);
+    PLACE(tab, p + "1.conv_right.weight", P, ro, o_taps + (long long)lo * P, P);
+    if ((rc = push_linear(p + "2.linear", D, P, &o_wa, &o_ba))) return rc;
+    if (l == 0) {
+      a.lo_wp = o_wp - base; a.lo_taps = o_taps - base; a.lo_wa = o_wa - base; a.lo_ba = o_ba - base;
+      a.layer_stride = (int)m->h_vec.size() - base;
+    }
   }
-  GET(wo1, "backbone.out_linear1.linear.weight", (size_t)A2 * D);
-  GET(bo1, "backbone.out_linear1.linear.bias", (size_t)A2);
-  GET(wo2, "backbone.out_linear2.linear.weight", (size_t)O * A2);
-  GET(bo2, "backbone.out_linear2.linear.bias", (size_t)O);
-  push_wt(wo1, A2, D, &a.o_w_out1); push_b(bo1, A2, &a.o_b_out1);
-  push_wt(wo2, O, A2, &a.o_w_out2); push_b(bo2, O, &a.o_b_out2);
+  if ((rc = push_linear("backbone.out_linear1.linear", A2, D, &a.o_w_out1, &a.o_b_out1)) ||
+      (rc = push_linear("backbone.out_linear2.linear", O, A2, &a.o_w_out2, &a.o_b_out2)))
+    return rc;
   a.idim = idim; a.aff_in = A1; a.lin = D; a.proj = P; a.aff_out = A2; a.odim = O; a.L = L; a.lorder = lo; a.rorder = ro;
   a.act = c.activation; a.has_cmvn = m->has_cmvn ? 1 : 0; a.norm_var = 1;      // istd already 1 when norm_var is off
   a.np_aff_in = npad(A1); a.np_lin = npad(D); a.np_proj = npad(P); a.np_aff_out = npad(A2); a.np_odim = npad(O);
@@ -698,6 +696,7 @@ extern "C" int wekws_model_set_head(wekws_model* m, int head) {
 
 extern "C" int wekws_model_pack(wekws_model* m) {
   WEKWS_REQUIRE(m, "wekws_model_pack: null handle");
+  m->params.clear();
   if (m->cfg.backbone == WEKWS_BACKBONE_FSMN) return pack_fsmn(m);
   return m->cfg.backbone == WEKWS_BACKBONE_GRU ? pack_gru(m) : pack_conv(m);
 }
@@ -1235,41 +1234,18 @@ extern "C" int wekws_model_load_params(wekws_model* m, const float* const* h_par
   if (rc) return rc;
   WEKWS_REQUIRE(h_params && n == t.n_params, "%s: expected the %d parameters of a %d-layer %s model, got %d", what,
                 t.n_params, m->cfg.num_layers, train_label(t.fam), n);
+  if (m->params.size() != (size_t)n) {
+    set_error("internal: %s: the pack holds %zu parameters, not %d", what, m->params.size(), n);
+    return WEKWS_ERR_INVALID;
+  }
   FsmnPackArgs p{};
   p.packed = m->d_vec;
   p.n = n;
-  int k = 0;                                   // the parameters in order, each [rows][cols] into its place in the pack
-  auto put = [&](int rows, int cols, long long dst, int ld) {
-    FsmnParamCopy& c = p.p[k];
-    c.src = h_params[k]; c.dst = dst; c.rows = rows; c.cols = cols; c.ld = ld;
-    ++k;
-  };
-  if (t.fam == TrainFamily::Fsmn) {            // state_dict order into pack_fsmn's layout
-    const FsmnArgs& a = m->fsmn;
-    const int D = a.lin, P = a.proj;
-    put(a.aff_in, a.idim, a.o_w_in1, a.np_aff_in); put(a.aff_in, 1, a.o_b_in1, 1);
-    put(D, a.aff_in, a.o_w_in2, a.np_lin); put(D, 1, a.o_b_in2, 1);
-    for (int l = 0; l < a.L; ++l) {
-      const long long base = a.o_layers + (long long)l * a.layer_stride;
-      put(P, D, base + a.lo_wp, a.np_proj);
-      put(P, a.lorder, base + a.lo_taps, P);
-      put(P, a.rorder, base + a.lo_taps + (long long)a.lorder * P, P);
-      put(D, P, base + a.lo_wa, a.np_lin); put(D, 1, base + a.lo_ba, 1);
-    }
-    put(a.aff_out, D, a.o_w_out1, a.np_aff_out); put(a.aff_out, 1, a.o_b_out1, 1);
-    put(a.odim, a.aff_out, a.o_w_out2, a.np_odim); put(a.odim, 1, a.o_b_out2, 1);
-  } else {                                     // named_parameters order into pack_gru's layout
-    const GruArgs& a = m->gru;
-    const int H = a.H, G = 3 * H;
-    put(H, a.idim, a.v_wp, H); put(H, 1, a.v_bp, 1);
-    for (int l = 0; l < a.L; ++l) {
-      const long long base = a.v_layers + (long long)l * a.v_layer_stride;
-      put(G, H, base, 2 * G); put(G, H, base + G, 2 * G);
-      put(G, 1, base + 2LL * H * G, 1); put(G, 1, base + 2LL * H * G + G, 1);
-    }
-    put(a.odim, H, a.v_wc, a.odim); put(a.odim, 1, a.v_bc, 1);
+  for (int i = 0; i < n; ++i) {
+    WEKWS_REQUIRE(h_params[i] != nullptr, "%s: parameter %d is null", what, i);
+    const PackedParam& e = m->params[i];
+    p.p[i] = {h_params[i], e.dst, e.rows, e.cols, e.ld};
   }
-  for (int i = 0; i < p.n; ++i) WEKWS_REQUIRE(p.p[i].src != nullptr, "%s: parameter %d is null", what, i);
   return fsmn_pack_launch(p, (cudaStream_t)stream);
 }
 
